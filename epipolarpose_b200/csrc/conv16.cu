@@ -13,13 +13,11 @@
 // of the convolution is the TMA out-of-bounds fill, strided convs use the four parity views of
 // the tensor.  Weight planes are 3-D (k, co, plane) box loads.
 //
-// One persistent CTA per SM, three warpgroups:
-//   warpgroup 0   TMA producer (one lane): A hi/lo + B hi/lo boxes per k-block, S-deep ring;
-//   warpgroups 1-2 consumers: 64 rows each, 4 k-steps x 3 wgmma m64nBNk16 per k-block
-//                 (registers, one k-block in flight); the epilogue writes from the fragment
-//                 (scale, bias, store or add) and sums the BatchNorm statistics in per-warp
-//                 smem slices across the CTA's tiles of one N tile, combined in a fixed order.
-// Every mbarrier wait is bounded (trap instead of hang).
+// One persistent CTA per SM on the pipeline of tc_common.cuh: warpgroup 0 is the TMA
+// producer (one lane: A hi/lo + B hi/lo boxes per k-block), warpgroups 1-2 the consumers
+// (4 k-steps x 3 wgmma m64nBNk16 per k-block).  The epilogue scales, adds the bias, stores
+// or adds, and keeps the BatchNorm statistics of a run of tiles of one N tile in the
+// per-warp slices, flushed once per run.
 #include "split16_common.cuh"
 
 namespace {
@@ -30,17 +28,14 @@ constexpr int kConsumers = 256;
 constexpr int kStageBudget = 200 * 1024;
 
 struct Plan16 {
-  int N, Hp, Wp;                 // phase grid
+  epb_phase_grid grid;           // pixel tiles of the phase grid (M side), tap views
   int Ho, Wo, Cout, os, ph, pw;  // output tensor / phase
   int Wv, Hv;                    // extent of the output phase view (rows beyond it are not stored)
   int T, CB;                     // taps, channel blocks of 64 per tap
-  int tw, th, tn, tiles_w, tiles_h;
-  int m_tiles, n_tiles;
+  int n_tiles;
   int accumulate;
   int m_fastest;                 // tile order: consecutive tiles walk M (statistics runs) or N
   int koff[EPB_MAX_TAPS];        // wt[t] * Cin: k offset of the tap inside a packed weight row
-  short dwq[EPB_MAX_TAPS], dhq[EPB_MAX_TAPS];   // tap offset on its parity view
-  unsigned char map[EPB_MAX_TAPS];              // parity view of the tap
 };
 
 struct Maps16 {
@@ -70,30 +65,19 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
               const float* __restrict__ bias, float* __restrict__ out,
               double* __restrict__ stats) {
   using C = Cfg16<BN>;
+  const epb_phase_grid& G = P.grid;
+  constexpr int CTRL = C::S * C::STAGE;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = tc::smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  uint8_t* ctrl = sm + C::S * C::STAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);          // full[8], empty[8]
-  float* sstat = reinterpret_cast<float*>(ctrl + 256);         // [8 warps][2][BN]
-  const uint32_t bar0 = tc::smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (8 + s); };
+  tc::Ring<C::S, C::STAGE> ring(smem_raw, 0, CTRL, CTRL + 64);     // full[8], empty[8]
+  float* sstat = reinterpret_cast<float*>(ring.sm + CTRL + 256);   // [8 warps][2][BN]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = P.T * P.CB;
-  const int total_tiles = P.m_tiles * P.n_tiles;
-  auto nt_of = [&](int tile) { return P.m_fastest ? tile / P.m_tiles : tile % P.n_tiles; };
-  auto mt_of = [&](int tile) { return P.m_fastest ? tile % P.m_tiles : tile / P.n_tiles; };
+  const int total_tiles = G.tiles * P.n_tiles;
+  auto nt_of = [&](int tile) { return P.m_fastest ? tile / G.tiles : tile % P.n_tiles; };
+  auto mt_of = [&](int tile) { return P.m_fastest ? tile % G.tiles : tile / P.n_tiles; };
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::S; ++s) {
-      tc::mbar_init(full_bar(s), 1);                  // the producer's arrive.expect_tx
-      tc::mbar_init(empty_bar(s), kConsumers / 32);   // one arrive per consumer warp
-    }
-    tc::fence_barrier_init();
-  }
+  if (threadIdx.x == 0) ring.init(1, kConsumers / 32);   // producer's arrive.expect_tx; consumer warps
   __syncthreads();
 
   if (warp < 4) {
@@ -101,22 +85,18 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
     if (warp == 0 && lane == 0) {
       for (int v = 0; v < 4; ++v) tc::tma_prefetch_desc(&maps.a[v]);
       tc::tma_prefetch_desc(&maps.w);
-      int stage = 0;
-      uint32_t phase = 0;
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = nt_of(tile);
-        int it = mt_of(tile);
-        const int w0 = (it % P.tiles_w) * P.tw; it /= P.tiles_w;
-        const int h0 = (it % P.tiles_h) * P.th;
-        const int n0 = (it / P.tiles_h) * P.tn;
+        int w0, h0, n0;
+        G.tile_origin(mt_of(tile), w0, h0, n0);
         int t = 0, cb = 0;
         for (int kb = 0; kb < KB; ++kb) {
-          tc::mbar_wait(empty_bar(stage), phase ^ 1);
-          const uint32_t fb = full_bar(stage);
+          tc::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1);
+          const uint32_t fb = ring.full(ring.stage);
           tc::mbar_arrive_expect_tx(fb, C::STAGE);
-          const uint32_t a_dst = base + stage * C::STAGE;
-          const CUtensorMap* am = &maps.a[P.map[t]];
-          const int cx = cb * 64, wx = w0 + P.dwq[t], hx = h0 + P.dhq[t];
+          const uint32_t a_dst = ring.stage_addr(ring.stage);
+          const CUtensorMap* am = &maps.a[G.map[t]];
+          const int cx = cb * 64, wx = w0 + G.dwq[t], hx = h0 + G.dhq[t];
           tc::tma_load_5d(a_dst, am, fb, cx, wx, hx, n0, 0);
           tc::tma_load_5d(a_dst + C::A_PLANE, am, fb, cx, wx, hx, n0, 1);
           const uint32_t b_dst = a_dst + C::A_BYTES;
@@ -124,7 +104,7 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
           tc::tma_load_3d(b_dst, &maps.w, fb, kx, rx, 0);
           tc::tma_load_3d(b_dst + C::B_PLANE, &maps.w, fb, kx, rx, 1);
           if (++cb == P.CB) { cb = 0; ++t; }
-          if (++stage == C::S) { stage = 0; phase ^= 1; }
+          ring.advance();
         }
       }
     }
@@ -135,83 +115,51 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
   const int wgc = (warp >> 2) - 1;             // rows 64 * wgc .. + 63 of the tile
   const int ct = threadIdx.x - 128;            // 0..255
   float* wstat = sstat + (ct >> 5) * 2 * BN;   // this warp's statistics slice
-  const int lr = (lane >> 2), lc = (lane & 3) * 2;
-  const int ra = wgc * 64 + (warp & 3) * 16 + lr;   // fragment rows ra, ra + 8
+  const int lc = (lane & 3) * 2;
+  const int ra = wgc * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows ra, ra + 8
   const float alpha = in_sc[1] * w_sc[1];
-  const int twh = P.tw * P.th;
+  const int twh = G.tw * G.th;
   if (stats) {
     for (int c = ct; c < (kConsumers / 32) * 2 * BN; c += kConsumers) sstat[c] = 0.f;
     tc::named_sync(1, kConsumers);
   }
-  auto flush_stats = [&](int nt) {
-    // every column below Cout of N tile `nt` carries the sums of all tiles since the last flush
-    tc::named_sync(1, kConsumers);
-    for (int c = ct; c < 2 * BN; c += kConsumers) {
-      const int which = c / BN, col = nt * BN + (c % BN);
-      float v = 0.f;
-#pragma unroll
-      for (int w = 0; w < kConsumers / 32; ++w) {             // fixed order: run-to-run identical
-        v += sstat[w * 2 * BN + c];
-        sstat[w * 2 * BN + c] = 0.f;
-      }
-      if (col < P.Cout) atomicAdd(stats + (int64_t)which * P.Cout + col, (double)v);
-    }
-    tc::named_sync(1, kConsumers);
-  };
 
   float acc[BN / 2];
-  int stage = 0, nt_prev = -1;
-  uint32_t phase = 0;
+  int nt_prev = -1;
   for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
     const int nt = nt_of(tile);
-    if (stats && nt_prev >= 0 && nt != nt_prev) flush_stats(nt_prev);
+    // statistics: one flush per run of tiles of the same N tile
+    if (stats && nt_prev >= 0 && nt != nt_prev)
+      tc::stats_flush<BN, kConsumers / 32>(sstat, ct, nt_prev, P.Cout, stats);
     nt_prev = nt;
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    int prev = -1;
-    for (int kb = 0; kb < KB; ++kb) {
-      tc::mbar_wait(full_bar(stage), phase);
-      const uint32_t a_hi = base + stage * C::STAGE + wgc * 64 * 128;
-      const uint32_t b_hi = base + stage * C::STAGE + C::A_BYTES;
-      tc::fence_acc(acc);
-      tc::wgmma_fence();
+    for (int kb = 0; kb < KB; ++kb)
+      ring.consume(acc, [&](uint32_t st) {
+        const uint32_t a_hi = st + wgc * 64 * 128, b_hi = st + C::A_BYTES;
 #pragma unroll
-      for (int kk = 0; kk < 4; ++kk) {               // 4 x K = 16 fp16 (32 bytes)
-        const uint64_t ah = tc::desc_kmajor_sw128(a_hi + kk * 32);
-        const uint64_t al = tc::desc_kmajor_sw128(a_hi + C::A_PLANE + kk * 32);
-        const uint64_t bh = tc::desc_kmajor_sw128(b_hi + kk * 32);
-        const uint64_t bl = tc::desc_kmajor_sw128(b_hi + C::B_PLANE + kk * 32);
-        tc::wgmma_f16<0, 0>(acc, al, bh, 1);
-        tc::wgmma_f16<0, 0>(acc, ah, bl, 1);
-        tc::wgmma_f16<0, 0>(acc, ah, bh, 1);
-      }
-      tc::wgmma_commit();
-      tc::wgmma_wait<1>();                            // the previous k-block's wgmma are done
-      tc::fence_acc(acc);
-      if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev));
-      prev = stage;
-      if (++stage == C::S) { stage = 0; phase ^= 1; }
-    }
-    tc::wgmma_wait<0>();
-    tc::fence_acc(acc);
-    if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev));
+        for (int kk = 0; kk < 4; ++kk)               // 4 x K = 16 fp16 (32 bytes)
+          tc::mma3_f16<0, 0>(acc, tc::desc_kmajor_sw128(a_hi + kk * 32),
+                             tc::desc_kmajor_sw128(a_hi + C::A_PLANE + kk * 32),
+                             tc::desc_kmajor_sw128(b_hi + kk * 32),
+                             tc::desc_kmajor_sw128(b_hi + C::B_PLANE + kk * 32));
+      });
+    ring.drain(acc);
 
     // ---- epilogue straight from the fragment: rows ra (h = 0) and ra + 8 (h = 1)
-    int it = mt_of(tile);
-    const int w0 = (it % P.tiles_w) * P.tw; it /= P.tiles_w;
-    const int h0 = (it % P.tiles_h) * P.th;
-    const int n0 = (it / P.tiles_h) * P.tn;
+    int w0, h0, n0;
+    G.tile_origin(mt_of(tile), w0, h0, n0);
     float* orow[2];
     bool srow[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = ra + 8 * h;
-      const int w = w0 + r % P.tw, hh = h0 + (r / P.tw) % P.th, n = n0 + r / twh;
-      orow[h] = (w < P.Wv && hh < P.Hv && n < P.N)
+      const int w = w0 + r % G.tw, hh = h0 + (r / G.tw) % G.th, n = n0 + r / twh;
+      orow[h] = (w < P.Wv && hh < P.Hv && n < G.N)
                     ? out + (((int64_t)n * P.Ho + (int64_t)hh * P.os + P.ph) * P.Wo +
                              (int64_t)w * P.os + P.pw) * P.Cout
                     : nullptr;
-      srow[h] = w < P.Wp && hh < P.Hp && n < P.N;
+      srow[h] = w < G.Wp && hh < G.Hp && n < G.N;
     }
 #pragma unroll
     for (int j = 0; j < BN / 8; ++j) {
@@ -233,42 +181,10 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
           *o = x;
         }
       }
-      if (stats) {
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const float x0 = srow[0] ? v[0][e] : 0.f, x1 = srow[1] ? v[1][e] : 0.f;
-          float s1 = x0 + x1, s2 = fmaf(x0, x0, x1 * x1);
-#pragma unroll
-          for (int o = 4; o < 32; o <<= 1) {
-            s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-            s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-          }
-          if (lr == 0) {
-            wstat[cl + e] += s1;
-            wstat[BN + cl + e] += s2;
-          }
-        }
-      }
+      if (stats) tc::stats_add<BN>(wstat, cl, v, srow);
     }
   }
-  if (stats && nt_prev >= 0) flush_stats(nt_prev);
-}
-
-template <int BN>
-int launch16(const Plan16& P, const Maps16& maps, const float* in_sc, const float* w_sc,
-             const float* bias, float* out, double* stats, cudaStream_t st) {
-  using C = Cfg16<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    EPB_CUDA(cudaFuncSetAttribute(conv16_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  C::SMEM));
-    attr_set = true;
-  }
-  const int64_t tiles = (int64_t)P.m_tiles * P.n_tiles;
-  const int grid = (int)(tiles < kNumSMs ? tiles : kNumSMs);
-  conv16_kernel<BN><<<grid, kThreads16, C::SMEM, st>>>(P, maps, in_sc, w_sc, bias, out, stats);
-  EPB_LAUNCH_CHECK();
-  return EPB_OK;
+  if (stats && nt_prev >= 0) tc::stats_flush<BN, kConsumers / 32>(sstat, ct, nt_prev, P.Cout, stats);
 }
 
 }  // namespace
@@ -287,50 +203,16 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   Plan16 P;
   Maps16 maps;
   memset(&maps, 0, sizeof(maps));
-  P.Ho = g->Ho; P.Wo = g->Wo; P.Cout = g->Cout; P.os = g->os; P.ph = g->ph; P.pw = g->pw;
-  P.T = g->T; P.CB = g->Cin / 64; P.accumulate = g->accumulate;
-  // a 1x1 stride-1 layer whose phase grid IS the input and the output grid is a plain
-  // [M][C] matrix: tile it as rows (no waste whatever H and W are)
-  const bool dense = g->T == 1 && g->is == 1 && g->os == 1 && g->dh[0] == 0 && g->dw[0] == 0 &&
-                     g->Hp == g->Hi && g->Wp == g->Wi && g->Hp == g->Ho && g->Wp == g->Wo;
-  int N = g->N, Hi = g->Hi, Wi = g->Wi;
-  P.N = g->N; P.Hp = g->Hp; P.Wp = g->Wp;
-  if (dense) {
-    const int64_t M = (int64_t)g->N * g->Hp * g->Wp;
-    EPB_CHECK_ARG(M < (1LL << 31));
-    N = 1; Hi = 1; Wi = (int)M;
-    P.N = 1; P.Hp = 1; P.Wp = (int)M; P.Ho = 1; P.Wo = (int)M;
-  }
-  P.Wv = dense ? P.Wp : (g->Wo - g->pw + g->os - 1) / g->os;
+  bool dense;
+  rc = epb_plan_phase_grid(g, in, BM, P.grid, maps.a, dense);
+  if (rc) return rc;
+  // a dense layer's output is the same [M][Cout] matrix as its phase grid
+  P.Ho = dense ? 1 : g->Ho; P.Wo = dense ? P.grid.Wp : g->Wo; P.Cout = g->Cout; P.os = g->os;
+  P.ph = dense ? 0 : g->ph; P.pw = dense ? 0 : g->pw;
+  P.Wv = dense ? P.grid.Wp : (g->Wo - g->pw + g->os - 1) / g->os;
   P.Hv = dense ? 1 : (g->Ho - g->ph + g->os - 1) / g->os;
-  if (dense) { P.ph = 0; P.pw = 0; }
-  epb_choose_tile(P.N, P.Hp, P.Wp, BM, P.tw, P.th, P.tn);
-  P.tiles_w = (P.Wp + P.tw - 1) / P.tw;
-  P.tiles_h = (P.Hp + P.th - 1) / P.th;
-  const int64_t mt = (int64_t)P.tiles_w * P.tiles_h * ((P.N + P.tn - 1) / P.tn);
-  EPB_CHECK_ARG(mt < (1LL << 30));
-  P.m_tiles = (int)mt;
-  bool need[4] = {false, false, false, false};
-  for (int t = 0; t < g->T; ++t) {
-    int qh, qw, dq_h, dq_w;
-    epb_tap_split(g->dh[t], g->is, qh, dq_h);
-    epb_tap_split(g->dw[t], g->is, qw, dq_w);
-    P.map[t] = (unsigned char)(qh * 2 + qw);
-    P.dhq[t] = (short)dq_h;
-    P.dwq[t] = (short)dq_w;
-    P.koff[t] = g->wt[t] * g->Cin;
-    need[qh * 2 + qw] = true;
-  }
-  for (int v = 0; v < 4; ++v) {
-    if (!need[v]) continue;
-    rc = epb_make_act_map(&maps.a[v], in, N, Hi, Wi, g->Cin, g->is, v >> 1, v & 1, P.tw, P.th, P.tn);
-    if (rc) return rc;
-  }
-  for (int v = 0; v < 4; ++v)
-    if (!need[v]) {                         // unused slots hold a valid map (they are prefetched)
-      for (int u = 0; u < 4; ++u)
-        if (need[u]) { maps.a[v] = maps.a[u]; break; }
-    }
+  P.T = g->T; P.CB = g->Cin / 64; P.accumulate = g->accumulate;
+  for (int t = 0; t < g->T; ++t) P.koff[t] = g->wt[t] * g->Cin;
   // tile order: statistics want runs of tiles with the same N tile (one flush per run); without
   // statistics, N-fastest lets the concurrently running tiles of one M tile share its A rows in L2
   P.m_fastest = stats != nullptr;
@@ -338,27 +220,19 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   // 64 columns for narrow layers
   const int bn = g->Cout <= 64 ? 64 : 128;
   P.n_tiles = (g->Cout + bn - 1) / bn;
-  {
-    epb_encode_tiled_fn enc = epb_get_encode_tiled();
-    if (!enc) {
-      epb_set_error("cuTensorMapEncodeTiled entry point unavailable");
-      return EPB_ECUDA;
-    }
-    const int64_t K = (int64_t)g->Tw * g->Cin;
-    const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)g->Cout, 2};
-    const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)K * 2 * g->Cout};
-    const cuuint32_t box[3] = {64, (cuuint32_t)bn, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    CUresult cr = enc(&maps.w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, const_cast<epb_half*>(w), dims,
-                      strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (cr != CUDA_SUCCESS) {
-      epb_set_error("cuTensorMapEncodeTiled(weights %d x %lld) failed (%d)", g->Cout, (long long)K,
-                    (int)cr);
-      return EPB_ECUDA;
-    }
-  }
+  const int64_t K = (int64_t)g->Tw * g->Cin;
+  const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)g->Cout, 2};
+  const cuuint64_t strides[2] = {(cuuint64_t)K * 2, (cuuint64_t)K * 2 * g->Cout};
+  const cuuint32_t box[3] = {64, (cuuint32_t)bn, 1};
+  rc = epb_encode_map(&maps.w, CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 3, w, dims, strides, box,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "weights");
+  if (rc) return rc;
+  const int64_t tiles = (int64_t)P.grid.tiles * P.n_tiles;
+  const unsigned grid = (unsigned)(tiles < kNumSMs ? tiles : kNumSMs);
   cudaStream_t st = as_stream(stream);
-  if (bn == 64) return launch16<64>(P, maps, in_sc, w_sc, bias, out, stats, st);
-  return launch16<128>(P, maps, in_sc, w_sc, bias, out, stats, st);
+  if (bn == 64)
+    return tc::launch<conv16_kernel<64>>(grid, kThreads16, Cfg16<64>::SMEM, st, P, maps, in_sc,
+                                         w_sc, bias, out, stats);
+  return tc::launch<conv16_kernel<128>>(grid, kThreads16, Cfg16<128>::SMEM, st, P, maps, in_sc,
+                                        w_sc, bias, out, stats);
 }

@@ -4,13 +4,9 @@
 //   k = (tap, ci);  A gathered from the NHWC input with the producing layer's
 //   BatchNorm+ReLU applied on the fly.
 //
-// One persistent CTA per SM, warp-specialised:
-//   warps 0-7  consumers (two warpgroups, 64 tile rows each): wgmma m64nBNk8 kind tf32 from
-//              the smem ring, FP32 accumulators in registers, one k-block of wgmma in flight
-//              while the next is issued; then the epilogue straight from the accumulator
-//              fragment: bias, stores / accumulate, and the per-channel sum and sum of
-//              squares for the following BatchNorm (per-warp shared-memory partials summed
-//              in a fixed order, one double atomic per column per tile);
+// One persistent CTA per SM on the pipeline of tc_common.cuh:
+//   warps 0-7  consumers: wgmma m64nBNk8 tf32 per k-step; the epilogue adds the bias,
+//              stores or accumulates, and flushes the BatchNorm statistics every tile;
 //   warps 8-15 producers: gather 128 pixel rows x 32 channels (128-byte rows), fused
 //              BN+ReLU, split into TF32 hi (+ lo for the 3xTF32 mode) and store into the
 //              SWIZZLE_128B K-major smem layout wgmma reads; the k-blocks of all tiles of
@@ -18,14 +14,12 @@
 //              (warp-private row tables, no CTA barrier).  The first lane of each group
 //              also issues the TMA loads of the packed weight tile (hi / lo planes) of the
 //              slot it fills.
-// smem ring full/empty mbarriers; every wait is bounded (trap instead of hang).
 //
 // precision 1: TF32 single pass.  precision 3: 3xTF32 error-compensated
 // (a_hi*b_hi + a_lo*b_hi + a_hi*b_lo, FP32 accumulate): fp32-grade results on
 // the tensor pipe, which is what the 1e-3 end-to-end parity bar needs.
 #include <cstdlib>
-#include "conv_common.cuh"
-#include "tc_common.cuh"
+#include "split16_common.cuh"
 
 namespace {
 
@@ -76,17 +70,12 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
   const int tile0 = (int)blockIdx.x;
   const int tstep = (int)gridDim.x;
   auto m_tile_of = [&](int tile) { return tile / n_tiles; };
+  constexpr int CTRL = C::S * C::STAGE;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = tc::smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;               // SWIZZLE_128B needs 1024 B
-  uint8_t* sm = smem_raw + (base - raw);
-  uint8_t* ctrl = sm + C::S * C::STAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);          // full[S], empty[S]
+  tc::Ring<C::S, C::STAGE> ring(smem_raw, 0, CTRL, CTRL + 64);     // full[8], empty[8]
+  uint8_t* ctrl = ring.sm + CTRL;
   RowInfo* rows = reinterpret_cast<RowInfo*>(ctrl + 1024);
   float* sstat = reinterpret_cast<float*>(ctrl + 1024 + sizeof(RowInfo));   // [8 warps][2][BN]
-  const uint32_t bar0 = tc::smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (8 + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int64_t M = (int64_t)g.N * g.Hp * g.Wp;
@@ -94,13 +83,7 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
   const int KB = g.T * CB;                 // k-blocks per tile
   const int total_tiles = m_tiles * n_tiles;
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::S; ++s) {
-      tc::mbar_init(full_bar(s), C::W + 1);        // the group's A warps + its weight TMA
-      tc::mbar_init(empty_bar(s), kConsumerWarps);
-    }
-    tc::fence_barrier_init();
-  }
+  if (threadIdx.x == 0) ring.init(C::W + 1, kConsumerWarps);   // the group's A warps + its weight TMA
   if (stats)
     for (int c = threadIdx.x; c < kConsumerWarps * 2 * BN; c += kThreads) sstat[c] = 0.f;
   __syncthreads();
@@ -244,15 +227,15 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
         sc = *reinterpret_cast<const float4*>(in_scale + ch);
         sh = *reinterpret_cast<const float4*>(in_shift + ch);
       }
-      tc::mbar_wait(empty_bar(st), ph ^ 1);
+      tc::mbar_wait(ring.empty(st), ph ^ 1);
       if (wg == 0 && lane == 0) {
-        const uint32_t b_dst = base + st * C::STAGE + C::A_BYTES;
-        tc::mbar_arrive_expect_tx(full_bar(st), C::B_BYTES);
+        const uint32_t b_dst = ring.stage_addr(st) + C::A_BYTES;
+        tc::mbar_arrive_expect_tx(ring.full(st), C::B_BYTES);
 #pragma unroll
         for (int pl = 0; pl < C::PL; ++pl)
-          tc::tma_load_2d(b_dst + pl * BN * 128, &tmap_w, full_bar(st), kx, pl * npad + nt * BN);
+          tc::tma_load_2d(b_dst + pl * BN * 128, &tmap_w, ring.full(st), kx, pl * npad + nt * BN);
       }
-      uint8_t* a_hi = sm + st * C::STAGE;
+      uint8_t* a_hi = ring.sm + st * C::STAGE;
       float4 xv[NQ];
 #pragma unroll
       for (int q = 0; q < NQ; ++q) xv[q] = v[q];
@@ -280,7 +263,7 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
       }
       tc::fence_proxy_async();
       __syncwarp();
-      if (lane == 0) tc::mbar_arrive(full_bar(st));
+      if (lane == 0) tc::mbar_arrive(ring.full(st));
       st += G;
       ph ^= (uint32_t)((st / C::S) & 1);
       st %= C::S;
@@ -299,44 +282,28 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
   } else {
     // =================================================== consumers (2 warpgroups)
     const int wgc = warp >> 2;                 // rows 64 * wgc .. + 63 of the tile
-    const int lr = lane >> 2, lc = (lane & 3) * 2;
-    const int ra = wgc * 64 + (warp & 3) * 16 + lr;   // fragment rows ra, ra + 8
+    const int lc = (lane & 3) * 2;
+    const int ra = wgc * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows ra, ra + 8
     float acc[BN / 2];
-    int stage = 0;
-    uint32_t phase = 0;
     for (int tile = tile0; tile < total_tiles; tile += tstep) {
       const int mt = m_tile_of(tile), nt = tile % n_tiles;
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-      int prev = -1;
-      for (int kb = 0; kb < KB; ++kb) {
-        tc::mbar_wait(full_bar(stage), phase);
-        const uint32_t a_hi = base + stage * C::STAGE + wgc * 64 * 128;
-        const uint32_t b_hi = base + stage * C::STAGE + C::A_BYTES;
-        tc::fence_acc(acc);
-        tc::wgmma_fence();
+      for (int kb = 0; kb < KB; ++kb)
+        ring.consume(acc, [&](uint32_t st) {
+          const uint32_t a_hi = st + wgc * 64 * 128, b_hi = st + C::A_BYTES;
 #pragma unroll
-        for (int kk = 0; kk < BKE / 8; ++kk) {
-          const uint64_t ah = tc::desc_kmajor_sw128(a_hi + kk * 32);
-          const uint64_t bh = tc::desc_kmajor_sw128(b_hi + kk * 32);
-          if (NS == 3) {
-            const uint64_t al = tc::desc_kmajor_sw128(a_hi + BM * 128 + kk * 32);
-            const uint64_t bl = tc::desc_kmajor_sw128(b_hi + BN * 128 + kk * 32);
-            tc::wgmma_tf32(acc, al, bh, 1);
-            tc::wgmma_tf32(acc, ah, bl, 1);
+          for (int kk = 0; kk < BKE / 8; ++kk) {
+            const uint64_t ah = tc::desc_kmajor_sw128(a_hi + kk * 32);
+            const uint64_t bh = tc::desc_kmajor_sw128(b_hi + kk * 32);
+            if (NS == 3)
+              tc::mma3_tf32(acc, ah, tc::desc_kmajor_sw128(a_hi + BM * 128 + kk * 32), bh,
+                            tc::desc_kmajor_sw128(b_hi + BN * 128 + kk * 32));
+            else
+              tc::wgmma_tf32(acc, ah, bh, 1);
           }
-          tc::wgmma_tf32(acc, ah, bh, 1);
-        }
-        tc::wgmma_commit();
-        tc::wgmma_wait<1>();                   // the previous k-block's wgmma are done
-        tc::fence_acc(acc);
-        if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev));
-        prev = stage;
-        if (++stage == C::S) { stage = 0; phase ^= 1; }
-      }
-      tc::wgmma_wait<0>();
-      tc::fence_acc(acc);
-      if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev));
+        });
+      ring.drain(acc);
 
       // ---- epilogue straight from the fragment: rows ra (h = 0) and ra + 8 (h = 1)
       float* orow[2];
@@ -372,35 +339,10 @@ conv_fprop_tc_kernel(const __grid_constant__ epb_conv_geom g,
             *o = x;
           }
         }
-        if (stats) {
-#pragma unroll
-          for (int e = 0; e < 2; ++e) {
-            const float x0 = orow[0] ? v[0][e] : 0.f, x1 = orow[1] ? v[1][e] : 0.f;
-            float s1 = x0 + x1, s2 = fmaf(x0, x0, x1 * x1);
-#pragma unroll
-            for (int o = 4; o < 32; o <<= 1) {
-              s1 += __shfl_xor_sync(0xffffffffu, s1, o);
-              s2 += __shfl_xor_sync(0xffffffffu, s2, o);
-            }
-            if (lr == 0) {
-              sstat[warp * 2 * BN + cl + e] = s1;
-              sstat[warp * 2 * BN + BN + cl + e] = s2;
-            }
-          }
-        }
+        if (stats)
+          tc::stats_add<BN>(sstat + warp * 2 * BN, cl, v, {orow[0] != nullptr, orow[1] != nullptr});
       }
-      if (stats) {
-        // every column of this N tile that lies below Cout was summed by all eight warps
-        tc::named_sync(1, 32 * kConsumerWarps);
-        for (int c = threadIdx.x; c < 2 * BN; c += 32 * kConsumerWarps) {
-          const int which = c / BN, col = nt * BN + (c % BN);
-          float v = 0.f;
-#pragma unroll
-          for (int w = 0; w < kConsumerWarps; ++w) v += sstat[w * 2 * BN + c];   // fixed order
-          if (col < g.Cout) atomicAdd(stats + (int64_t)which * g.Cout + col, (double)v);
-        }
-        tc::named_sync(1, 32 * kConsumerWarps);
-      }
+      if (stats) tc::stats_flush<BN, kConsumerWarps>(sstat, threadIdx.x, nt, g.Cout, stats);
     }
   }
 }
@@ -425,38 +367,17 @@ template <int BN, int NS>
 int launch_fprop(const epb_conv_geom* g, const CUtensorMap& tmap, const float* in,
                  const float* in_scale, const float* in_shift, const float* bias, float* out,
                  double* stats, int npad, cudaStream_t st) {
-  using C = Cfg<BN, NS>;
   const int64_t M = (int64_t)g->N * g->Hp * g->Wp;
   const int m_tiles = (int)((M + BM - 1) / BM);
   const int n_tiles = npad / BN;
-  static bool attr_set = false;
-  if (!attr_set) {
-    EPB_CUDA(cudaFuncSetAttribute(conv_fprop_tc_kernel<BN, NS>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-    attr_set = true;
-  }
   const int64_t tiles = (int64_t)m_tiles * n_tiles;
-  const int grid = (int)(tiles < kNumSMs ? tiles : kNumSMs);
-  conv_fprop_tc_kernel<BN, NS><<<grid, kThreads, C::SMEM, st>>>(*g, tmap, in, in_scale, in_shift,
-                                                                bias, out, stats, npad, m_tiles,
-                                                                n_tiles);
-  EPB_LAUNCH_CHECK();
-  return EPB_OK;
+  const unsigned grid = (unsigned)(tiles < kNumSMs ? tiles : kNumSMs);
+  return tc::launch<conv_fprop_tc_kernel<BN, NS>>(grid, kThreads, Cfg<BN, NS>::SMEM, st, *g, tmap,
+                                                  in, in_scale, in_shift, bias, out, stats, npad,
+                                                  m_tiles, n_tiles);
 }
 
 }  // namespace
-
-epb_encode_tiled_fn epb_get_encode_tiled() {
-  static epb_encode_tiled_fn fn = nullptr;
-  if (!fn) {
-    void* p = nullptr;
-    cudaDriverEntryPointQueryResult qr;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &p, cudaEnableDefault, &qr) ==
-            cudaSuccess && qr == cudaDriverEntryPointSuccess)
-      fn = reinterpret_cast<epb_encode_tiled_fn>(p);
-  }
-  return fn;
-}
 
 bool epb_conv_wgrad_tc_supported(const epb_conv_geom* g);
 
@@ -487,23 +408,13 @@ int epb_conv_fprop_tc(const epb_conv_geom* g, const float* in, const float* w,
     prep_weight_tc<<<(int)blocks, 256, 0, st>>>(w, wws, g->Cout, K, npad, planes);
     EPB_LAUNCH_CHECK();
   }
-  epb_encode_tiled_fn enc = epb_get_encode_tiled();
-  if (!enc) {
-    epb_set_error("cuTensorMapEncodeTiled entry point unavailable");
-    return EPB_ECUDA;
-  }
   CUtensorMap tmap;
   const cuuint64_t dims[2] = {(cuuint64_t)K, (cuuint64_t)((int64_t)planes * npad)};
   const cuuint64_t strides[1] = {(cuuint64_t)(K * sizeof(float))};
   const cuuint32_t box[2] = {(cuuint32_t)BKE, (cuuint32_t)bn};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult cr = enc(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, wws, dims, strides, box, estr,
-                    CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
-                    CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) {
-    epb_set_error("cuTensorMapEncodeTiled failed (%d)", (int)cr);
-    return EPB_ECUDA;
-  }
+  rc = epb_encode_map(&tmap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, wws, dims, strides, box,
+                      CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "weight planes");
+  if (rc) return rc;
 #define EPB_TC_CASE(BN_, NS_)                   \
   if (bn == BN_ && ns == NS_)                   \
     return launch_fprop<BN_, NS_>(g, tmap, in, in_scale, in_shift, bias, out, stats, npad, st);

@@ -83,23 +83,18 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
   using C = WCfg<BNW, NS>;
   constexpr int QA = WM / 4;                 // float4 per dout row (32)
   constexpr int QB = BNW / 4;                // float4 per input row
+  constexpr int A0 = 0, B0 = C::SA * C::A_TILE, CTRL = B0 + C::SB * C::B_TILE;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = tc::smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  uint8_t* smB = sm + C::SA * C::A_TILE;
-  uint8_t* ctrl = smB + C::SB * C::B_TILE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);   // fullA[2] emptyA[2] fullB[8] emptyB[8]
+  // barriers: fullA[2] emptyA[2] fullB[8] emptyB[8]
+  tc::Ring<C::SA, C::A_TILE> ringA(smem_raw, A0, CTRL, CTRL + 16);
+  tc::Ring<C::SB, C::B_TILE> ringB(smem_raw, B0, CTRL + 32, CTRL + 96);
+  uint8_t* sm = ringA.sm;
+  uint8_t* ctrl = sm + CTRL;
   int* slot_t = reinterpret_cast<int*>(ctrl + 256);          // [kMaxSlots] tap of each slot
   int* slot_cit = slot_t + kMaxSlots;                        // [kMaxSlots] ci tile of each slot
   int* rowtab = slot_cit + kMaxSlots;                        // [kGroups][4][KPIX]
   volatile int* seenA = rowtab + kGroups * 4 * KPIX;         // [SA] uses whose wait has passed
   volatile int* seenB = seenA + C::SA;                       // [SB]
-  const uint32_t bar0 = tc::smem_u32(bars);
-  auto fullA = [&](int s) { return bar0 + 8u * s; };
-  auto emptyA = [&](int s) { return bar0 + 8u * (2 + s); };
-  auto fullB = [&](int s) { return bar0 + 8u * (4 + s); };
-  auto emptyB = [&](int s) { return bar0 + 8u * (12 + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work item decode: blockIdx.x = ((split * co_tiles + cot) * groups + grp)
@@ -117,9 +112,8 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
   const int co0 = cot * WM;
 
   if (threadIdx.x == 0) {
-    for (int s = 0; s < C::SA; ++s) { tc::mbar_init(fullA(s), kProdWarps / kGroups); tc::mbar_init(emptyA(s), kConsWarps); }
-    for (int s = 0; s < C::SB; ++s) { tc::mbar_init(fullB(s), kProdWarps / kGroups); tc::mbar_init(emptyB(s), kConsWarps); }
-    tc::fence_barrier_init();
+    ringA.init(kProdWarps / kGroups, kConsWarps);
+    ringB.init(kProdWarps / kGroups, kConsWarps);
     for (int s = 0; s < C::SA; ++s) seenA[s] = 0;
     for (int s = 0; s < C::SB; ++s) seenB[s] = 0;
     for (int b = 0; b < NB; ++b) {
@@ -254,14 +248,14 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
       if (ie == 0) {
         const int s = iblk % C::SA, use = iblk / C::SA;
         wait_seen(seenA + s, use);
-        tc::mbar_wait(emptyA(s), (use & 1) ^ 1);
+        tc::mbar_wait(ringA.empty(s), (use & 1) ^ 1);
         if (lane == 0) seenA[s] = use + 1;
-        uint8_t* tile = sm + s * C::A_TILE;
+        uint8_t* tile = sm + A0 + s * C::A_TILE;
 #pragma unroll
         for (int k = 0; k < PAg; ++k) split_store(tile, WM * KPIX * 4, ra0 + k * RAg, qa, buf[k]);
         tc::fence_proxy_async();
         __syncwarp();
-        if (lane == 0) tc::mbar_arrive(fullA(s));
+        if (lane == 0) tc::mbar_arrive(ringA.full(s));
       } else {
         const int qn = iblk * NB + (ie - 1);
         const int s = qn % C::SB;
@@ -273,9 +267,9 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
         }
         const int use = qn / C::SB;
         wait_seen(seenB + s, use);
-        tc::mbar_wait(emptyB(s), (use & 1) ^ 1);
+        tc::mbar_wait(ringB.empty(s), (use & 1) ^ 1);
         if (lane == 0) seenB[s] = use + 1;
-        uint8_t* tile = smB + s * C::B_TILE;
+        uint8_t* tile = sm + B0 + s * C::B_TILE;
         if (in_scale) {
           // branch-free affine (+ReLU) on every row; rows that were not loaded (image border,
           // end of the pixel range) are post-activation zeros and are patched afterwards
@@ -291,7 +285,7 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
         for (int k = 0; k < PBg; ++k) split_store(tile, BNW * KPIX * 4, rb0 + k * RBg, qb, buf[k]);
         tc::fence_proxy_async();
         __syncwarp();
-        if (lane == 0) tc::mbar_arrive(fullB(s));
+        if (lane == 0) tc::mbar_arrive(ringB.full(s));
       }
       ie += kGroups;
       while (ie >= per_blk) { ie -= per_blk; ++iblk; }
@@ -305,39 +299,35 @@ conv_wgrad_tc_kernel(const __grid_constant__ epb_conv_geom g, const float* __res
     for (int b = 0; b < NBM; ++b)
 #pragma unroll
       for (int i = 0; i < BNW / 2; ++i) acc[b][i] = 0.f;
-    int sa = 0, sb = 0;
-    uint32_t pha = 0, phb = 0;
     for (int blk = 0; blk < nblk; ++blk) {
-      tc::mbar_wait(fullA(sa), pha);
-      const uint32_t a_hi = base + sa * C::A_TILE + wgc * 64 * 128;
+      tc::mbar_wait(ringA.full(ringA.stage), ringA.phase);
+      const uint32_t a_hi = ringA.stage_addr(ringA.stage) + wgc * 64 * 128;
 #pragma unroll
       for (int b = 0; b < NBM; ++b) {
         if (b < NB) {
-          tc::mbar_wait(fullB(sb), phb);
-          const uint32_t b_hi = base + C::SA * C::A_TILE + sb * C::B_TILE;
+          tc::mbar_wait(ringB.full(ringB.stage), ringB.phase);
+          const uint32_t b_hi = ringB.stage_addr(ringB.stage);
           tc::fence_acc(acc[b]);
           tc::wgmma_fence();
 #pragma unroll
           for (int ks = 0; ks < KPIX / 8; ++ks) {
             const uint64_t ah = tc::desc_kmajor_sw128(a_hi + ks * 32);
             const uint64_t bh = tc::desc_kmajor_sw128(b_hi + ks * 32);
-            if (NS == 3) {
-              const uint64_t al = tc::desc_kmajor_sw128(a_hi + WM * KPIX * 4 + ks * 32);
-              const uint64_t bl = tc::desc_kmajor_sw128(b_hi + BNW * KPIX * 4 + ks * 32);
-              tc::wgmma_tf32(acc[b], al, bh, 1);
-              tc::wgmma_tf32(acc[b], ah, bl, 1);
-            }
-            tc::wgmma_tf32(acc[b], ah, bh, 1);
+            if (NS == 3)
+              tc::mma3_tf32(acc[b], ah, tc::desc_kmajor_sw128(a_hi + WM * KPIX * 4 + ks * 32), bh,
+                            tc::desc_kmajor_sw128(b_hi + BNW * KPIX * 4 + ks * 32));
+            else
+              tc::wgmma_tf32(acc[b], ah, bh, 1);
           }
           tc::wgmma_commit();
           tc::wgmma_wait<0>();
           tc::fence_acc(acc[b]);
-          if (lane == 0) tc::mbar_arrive(emptyB(sb));
-          if (++sb == C::SB) { sb = 0; phb ^= 1; }
+          if (lane == 0) tc::mbar_arrive(ringB.empty(ringB.stage));
+          ringB.advance();
         }
       }
-      if (lane == 0) tc::mbar_arrive(emptyA(sa));
-      if (++sa == C::SA) { sa = 0; pha ^= 1; }
+      if (lane == 0) tc::mbar_arrive(ringA.empty(ringA.stage));
+      ringA.advance();
     }
     // ---- epilogue: add the partial tiles to dw (rows co, columns ci of the slot's tap)
     const int64_t wrow = (int64_t)g.Tw * g.Cin;
@@ -391,18 +381,11 @@ int launch_wgrad(const epb_conv_geom* g, const float* in, const float* dout, con
   int64_t rows = (M + splits - 1) / splits;
   rows = (rows + KPIX - 1) / KPIX * KPIX;
   splits = (M + rows - 1) / rows;
-  static bool attr_set = false;
-  if (!attr_set) {
-    EPB_CUDA(cudaFuncSetAttribute(conv_wgrad_tc_kernel<BNW, NS>,
-                                  cudaFuncAttributeMaxDynamicSharedMemorySize, C::SMEM));
-    attr_set = true;
-  }
   const int64_t grid = tiles * splits;
   EPB_CHECK_ARG(grid < (1LL << 31));
-  conv_wgrad_tc_kernel<BNW, NS><<<(unsigned)grid, kThreadsW, C::SMEM, st>>>(
-      *g, in, dout, in_scale, in_shift, dw, co_tiles, ci_tiles, groups2, nb, (int)rows);
-  EPB_LAUNCH_CHECK();
-  return EPB_OK;
+  return tc::launch<conv_wgrad_tc_kernel<BNW, NS>>((unsigned)grid, kThreadsW, C::SMEM, st, *g, in,
+                                                   dout, in_scale, in_shift, dw, co_tiles,
+                                                   ci_tiles, groups2, nb, (int)rows);
 }
 
 }  // namespace

@@ -2,6 +2,17 @@
 // wgmma (warpgroup MMA: operands in shared memory, FP32 accumulators in registers) with its
 // shared-memory matrix descriptors.  Inline PTX only.
 //
+// The pipeline the four GEMM kernels (conv16.cu, wgrad16.cu, conv_tc.cu, conv_tc_wgrad.cu)
+// share: producers fill the slots of a shared-memory Ring (TMA, or gather + convert + store
+// followed by fence_proxy_async) and complete the slot's full mbarrier; two consumer
+// warpgroups of 64 tile rows each wait on it, issue the slot's wgmma as one commit group
+// and release the slot on its empty mbarrier (one arrive per consumer warp) once the group
+// has completed.  Ring::consume keeps one k-block of wgmma in flight while the next one is
+// issued.  Split operands are multiplied by the three passes of mma3_*.  Epilogues work
+// straight from the accumulator fragment; the conv epilogues sum BatchNorm statistics with
+// stats_add / stats_flush in a fixed order.  Every mbarrier wait is bounded (trap instead of
+// hang).
+//
 // wgmma shared-memory descriptor (PTX ISA "Matrix Descriptor Format"):
 //   [0,14) start addr >> 4 | [16,30) leading byte offset >> 4 | [32,46) stride byte offset >> 4 |
 //   [49,52) base offset (0: every tile is 1024-byte aligned) | [62,64) layout (1 = SWIZZLE_128B)
@@ -11,8 +22,7 @@
 //   d[4j + 2h + e] = D[16 * (t / 32) + (t % 32) / 4 + 8h][8j + 2 * (t % 4) + e].
 #pragma once
 #include <cuda.h>
-#include <cuda_runtime.h>
-#include <stdint.h>
+#include "common.cuh"
 
 namespace tc {
 
@@ -252,6 +262,134 @@ __device__ __forceinline__ void wgmma_tf32(float (&d)[64], uint64_t a, uint64_t 
   wgmma_tf32_n128(d, a, b, sd);
 }
 
+// Error-compensated products of one k-step: a*b ~= a_lo*b_hi + a_hi*b_lo + a_hi*b_hi.  The
+// passes are issued in this order; outputs are bit-identical run to run and build to build
+// only while it stays the same.
+template <int TA, int TB, int R>
+__device__ __forceinline__ void mma3_f16(float (&d)[R], uint64_t ah, uint64_t al, uint64_t bh,
+                                         uint64_t bl) {
+  wgmma_f16<TA, TB>(d, al, bh, 1);
+  wgmma_f16<TA, TB>(d, ah, bl, 1);
+  wgmma_f16<TA, TB>(d, ah, bh, 1);
+}
+template <int R>
+__device__ __forceinline__ void mma3_tf32(float (&d)[R], uint64_t ah, uint64_t al, uint64_t bh,
+                                          uint64_t bl) {
+  wgmma_tf32(d, al, bh, 1);
+  wgmma_tf32(d, ah, bl, 1);
+  wgmma_tf32(d, ah, bh, 1);
+}
+
+// ------------------------------------------------------------------ operand ring
+// S operand slots of STAGE bytes with a full and an empty mbarrier per slot (8 bytes apart
+// from full(0) / empty(0)).  Offsets count from the 1024-byte aligned start `sm` of dynamic
+// shared memory (SWIZZLE_128B atoms); a kernel's barriers and other control data follow its
+// slots.  The producer waits on empty(s) with the opposite parity, fills the slot and
+// completes full(s); the consumers wait on full(s) and each consumer warp arrives on
+// empty(s) once it has finished reading.  `stage` / `phase` are the calling thread's
+// position in the ring.
+template <int S, int STAGE>
+struct Ring {
+  uint8_t* sm;                       // aligned start of dynamic shared memory
+  uint32_t base, full0, empty0;      // shared addresses of slot 0, full(0), empty(0)
+  int stage = 0, prev = -1;          // prev: slot of the consumer's k-block still in flight
+  uint32_t phase = 0;
+
+  __device__ __forceinline__ Ring(uint8_t* smem, uint32_t slots_off, uint32_t full_off,
+                                  uint32_t empty_off) {
+    const uint32_t raw = smem_u32(smem), a = (raw + 1023u) & ~1023u;
+    sm = smem + (a - raw);
+    base = a + slots_off;
+    full0 = smem_u32(sm + full_off);
+    empty0 = full0 + (empty_off - full_off);
+  }
+  __device__ __forceinline__ uint32_t stage_addr(int s) const { return base + s * STAGE; }
+  __device__ __forceinline__ uint32_t full(int s) const { return full0 + 8u * s; }
+  __device__ __forceinline__ uint32_t empty(int s) const { return empty0 + 8u * s; }
+  // one thread, before the CTA barrier that publishes the ring
+  __device__ __forceinline__ void init(uint32_t full_count, uint32_t empty_count) const {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full(s), full_count);
+      mbar_init(empty(s), empty_count);
+    }
+    fence_barrier_init();
+  }
+  __device__ __forceinline__ void advance() {
+    if (++stage == S) { stage = 0; phase ^= 1; }
+  }
+
+  // One k-block of a consumer warpgroup: wait for the slot, issue mma(stage address) as one
+  // wgmma group, then wait for the PREVIOUS k-block's group and release its slot, so one
+  // k-block stays in flight while the next is issued.
+  template <int R, class MMA>
+  __device__ __forceinline__ void consume(float (&acc)[R], MMA&& mma) {
+    mbar_wait(full(stage), phase);
+    fence_acc(acc);
+    wgmma_fence();
+    mma(stage_addr(stage));
+    wgmma_commit();
+    wgmma_wait<1>();
+    fence_acc(acc);
+    if (prev >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(empty(prev));
+    prev = stage;
+    advance();
+  }
+  // end of a run of consume(): the last group completes and its slot is released
+  template <int R>
+  __device__ __forceinline__ void drain(float (&acc)[R]) {
+    wgmma_wait<0>();
+    fence_acc(acc);
+    if (prev >= 0 && (threadIdx.x & 31) == 0) mbar_arrive(empty(prev));
+    prev = -1;
+  }
+};
+
+// ------------------------------------------------------------------ BatchNorm statistics
+// The epilogues sum each output column and its square into a per-warp shared-memory slice
+// [sum | sum of squares][BN]; a flush adds the slices in warp order, so the sums are
+// identical run to run.
+//
+// Adds one fragment column pair cl, cl + 1: v[h][e] is row h (fragment rows r, r + 8) and
+// column e; a row with ok[h] false counts as zero.  The eight lanes of a column are summed
+// with shuffles and added to the slice by lanes 0-3.
+template <int BN>
+__device__ __forceinline__ void stats_add(float* wstat, int cl, const float (&v)[2][2],
+                                          const bool (&ok)[2]) {
+#pragma unroll
+  for (int e = 0; e < 2; ++e) {
+    const float x0 = ok[0] ? v[0][e] : 0.f, x1 = ok[1] ? v[1][e] : 0.f;
+    float s1 = x0 + x1, s2 = fmaf(x0, x0, x1 * x1);
+#pragma unroll
+    for (int o = 4; o < 32; o <<= 1) {
+      s1 += __shfl_xor_sync(0xffffffffu, s1, o);
+      s2 += __shfl_xor_sync(0xffffffffu, s2, o);
+    }
+    if ((threadIdx.x & 31) < 4) {
+      wstat[cl + e] += s1;
+      wstat[BN + cl + e] += s2;
+    }
+  }
+}
+// Adds the slices of the WARPS consumer warps (thread t of 32 * WARPS, named barrier 1) in
+// warp order into stats[sum | sum of squares][cout] for the columns of N tile nt below
+// cout, one double atomic each, and zeroes the slices.
+template <int BN, int WARPS>
+__device__ __forceinline__ void stats_flush(float* sstat, int t, int nt, int cout,
+                                            double* stats) {
+  named_sync(1, 32 * WARPS);
+  for (int c = t; c < 2 * BN; c += 32 * WARPS) {
+    const int which = c / BN, col = nt * BN + (c % BN);
+    float v = 0.f;
+#pragma unroll
+    for (int w = 0; w < WARPS; ++w) {
+      v += sstat[w * 2 * BN + c];
+      sstat[w * 2 * BN + c] = 0.f;
+    }
+    if (col < cout) atomicAdd(stats + (int64_t)which * cout + col, (double)v);
+  }
+  named_sync(1, 32 * WARPS);
+}
+
 // round-to-nearest (ties away) TF32 kept in an fp32 container.  Same result as
 // cvt.rna.tf32.f32 for finite inputs, in 2 integer instructions instead of the 4 the
 // conversion expands to (it adds an Inf/NaN guard the operand split does not need).
@@ -264,12 +402,19 @@ __device__ __forceinline__ float4 bn_act4(float4 x, float4 sc, float4 sh, float 
                      fmaxf(fmaf(x.z, sc.z, sh.z), lb), fmaxf(fmaf(x.w, sc.w, sh.w), lb));
 }
 
-}  // namespace tc
+// ------------------------------------------------------------------ host: launch
+// Launches Kernel with `smem` bytes of dynamic shared memory; the first call of each
+// instantiation raises the kernel's dynamic shared-memory limit to it.
+template <auto Kernel, class... Args>
+int launch(unsigned grid, int threads, int smem, cudaStream_t st, const Args&... args) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    EPB_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set = true;
+  }
+  Kernel<<<grid, threads, smem, st>>>(args...);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
 
-// host side: cuTensorMapEncodeTiled through the runtime's driver entry point
-// (no link-time dependency on libcuda)
-typedef CUresult (*epb_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*,
-                                        const cuuint64_t*, const cuuint64_t*, const cuuint32_t*,
-                                        const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                        CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-epb_encode_tiled_fn epb_get_encode_tiled();
+}  // namespace tc

@@ -23,17 +23,14 @@ constexpr int kThreadsW16 = 384;       // warpgroup 0: TMA producer; warpgroups 
 constexpr int kChunk = KT * 128;       // bytes of one (64 pixels x 64 channels) box
 
 struct PlanW16 {
-  int N, Hp, Wp;
+  epb_phase_grid grid;           // pixel tiles of the phase grid (the reduction), tap views
   int Cin, Cout, Tw;
   int T, CB, CH;                 // taps, 64-channel blocks per tap, chunks = T * CB
-  int tw, th, tn, tiles_w, tiles_h, ptiles;
   int groups, n_tiles, splits, tiles_per_split;
   int swap;                      // 1: M side = 64-channel blocks of dout, N side = input channels
   int Nn;                        // channels on the N side (Cout, or Cin when swapped)
   int bdw, bdh;                  // box offset of the N-side operand (the tap, when swapped)
   int wt[EPB_MAX_TAPS];
-  short dwq[EPB_MAX_TAPS], dhq[EPB_MAX_TAPS];
-  unsigned char map[EPB_MAX_TAPS];
 };
 
 struct MapsW16 {
@@ -58,15 +55,10 @@ wgrad16_kernel(const __grid_constant__ PlanW16 P, const __grid_constant__ MapsW1
                const float* __restrict__ in_sc, const float* __restrict__ dout_sc,
                float* __restrict__ dw, float* __restrict__ ws) {
   using C = CfgW16<BN>;
+  constexpr int CTRL = C::S * C::STAGE;
+  const epb_phase_grid& G = P.grid;
   extern __shared__ uint8_t smem_raw[];
-  const uint32_t raw = tc::smem_u32(smem_raw);
-  const uint32_t base = (raw + 1023u) & ~1023u;
-  uint8_t* sm = smem_raw + (base - raw);
-  uint8_t* ctrl = sm + C::S * C::STAGE;
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ctrl);          // full[8], empty[8]
-  const uint32_t bar0 = tc::smem_u32(bars);
-  auto full_bar = [&](int s) { return bar0 + 8u * s; };
-  auto empty_bar = [&](int s) { return bar0 + 8u * (8 + s); };
+  tc::Ring<C::S, C::STAGE> ring(smem_raw, 0, CTRL, CTRL + 64);     // full[8], empty[8]
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // work item: blockIdx.x = ((split * n_tiles + nt) * groups + grp)
@@ -75,16 +67,10 @@ wgrad16_kernel(const __grid_constant__ PlanW16 P, const __grid_constant__ MapsW1
   const int nt = wi % P.n_tiles;
   const int split = wi / P.n_tiles;
   const int pt0 = split * P.tiles_per_split;
-  const int pt1 = min(P.ptiles, pt0 + P.tiles_per_split);
+  const int pt1 = min(G.tiles, pt0 + P.tiles_per_split);
   const int nst = pt1 - pt0;                                   // stages of this CTA (>= 1)
 
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < C::S; ++s) {
-      tc::mbar_init(full_bar(s), 1);
-      tc::mbar_init(empty_bar(s), 8);                          // one arrive per consumer warp
-    }
-    tc::fence_barrier_init();
-  }
+  if (threadIdx.x == 0) ring.init(1, 8);                       // one arrive per consumer warp
   __syncthreads();
 
   if (warp < 4) {
@@ -99,32 +85,28 @@ wgrad16_kernel(const __grid_constant__ PlanW16 P, const __grid_constant__ MapsW1
         ct[j] = c / P.CB;
         cc[j] = (c % P.CB) * 64;
       }
-      int stage = 0;
-      uint32_t phase = 0;
       for (int pt = pt0; pt < pt1; ++pt) {
-        int it = pt;
-        const int w0 = (it % P.tiles_w) * P.tw; it /= P.tiles_w;
-        const int h0 = (it % P.tiles_h) * P.th;
-        const int n0 = (it / P.tiles_h) * P.tn;
-        tc::mbar_wait(empty_bar(stage), phase ^ 1);
-        const uint32_t fb = full_bar(stage);
+        int w0, h0, n0;
+        G.tile_origin(pt, w0, h0, n0);
+        tc::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1);
+        const uint32_t fb = ring.full(ring.stage);
         tc::mbar_arrive_expect_tx(fb, C::STAGE);
-        const uint32_t a_dst = base + stage * C::STAGE;
+        const uint32_t a_dst = ring.stage_addr(ring.stage);
         const uint32_t b_dst = a_dst + 2 * C::A_PLANE;
 #pragma unroll
         for (int pl = 0; pl < 2; ++pl) {
 #pragma unroll
           for (int j = 0; j < 2; ++j) {
             const int t = ct[j];
-            tc::tma_load_5d(a_dst + pl * C::A_PLANE + j * kChunk, &maps.a[P.map[t]], fb,
-                            cc[j], w0 + P.dwq[t], h0 + P.dhq[t], n0, pl);
+            tc::tma_load_5d(a_dst + pl * C::A_PLANE + j * kChunk, &maps.a[G.map[t]], fb,
+                            cc[j], w0 + G.dwq[t], h0 + G.dhq[t], n0, pl);
           }
 #pragma unroll
           for (int jb = 0; jb < C::BCH; ++jb)
             tc::tma_load_5d(b_dst + pl * C::B_PLANE + jb * kChunk, &maps.d, fb,
                             nt * BN + jb * 64, w0 + P.bdw, h0 + P.bdh, n0, pl);
         }
-        if (++stage == C::S) { stage = 0; phase ^= 1; }
+        ring.advance();
       }
     }
     return;
@@ -135,33 +117,17 @@ wgrad16_kernel(const __grid_constant__ PlanW16 P, const __grid_constant__ MapsW1
   float acc[BN / 2];
 #pragma unroll
   for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-  int stage = 0, prev = -1;
-  uint32_t phase = 0;
-  for (int k = 0; k < nst; ++k) {
-    tc::mbar_wait(full_bar(stage), phase);
-    const uint32_t a_hi = base + stage * C::STAGE + wgc * kChunk;
-    const uint32_t b_hi = base + stage * C::STAGE + 2 * C::A_PLANE;
-    tc::fence_acc(acc);
-    tc::wgmma_fence();
+  for (int k = 0; k < nst; ++k)
+    ring.consume(acc, [&](uint32_t st) {
+      const uint32_t a_hi = st + wgc * kChunk, b_hi = st + 2 * C::A_PLANE;
 #pragma unroll
-    for (int ks = 0; ks < KT / 16; ++ks) {
-      const uint64_t ah = tc::desc_mnmajor16_sw128(a_hi + ks * 2048, kChunk, 1024);
-      const uint64_t al = tc::desc_mnmajor16_sw128(a_hi + C::A_PLANE + ks * 2048, kChunk, 1024);
-      const uint64_t bh = tc::desc_mnmajor16_sw128(b_hi + ks * 2048, kChunk, 1024);
-      const uint64_t bl = tc::desc_mnmajor16_sw128(b_hi + C::B_PLANE + ks * 2048, kChunk, 1024);
-      tc::wgmma_f16<1, 1>(acc, al, bh, 1);
-      tc::wgmma_f16<1, 1>(acc, ah, bl, 1);
-      tc::wgmma_f16<1, 1>(acc, ah, bh, 1);
-    }
-    tc::wgmma_commit();
-    tc::wgmma_wait<1>();
-    tc::fence_acc(acc);
-    if (prev >= 0 && lane == 0) tc::mbar_arrive(empty_bar(prev));
-    prev = stage;
-    if (++stage == C::S) { stage = 0; phase ^= 1; }
-  }
-  tc::wgmma_wait<0>();
-  tc::fence_acc(acc);
+      for (int ks = 0; ks < KT / 16; ++ks)
+        tc::mma3_f16<1, 1>(acc, tc::desc_mnmajor16_sw128(a_hi + ks * 2048, kChunk, 1024),
+                           tc::desc_mnmajor16_sw128(a_hi + C::A_PLANE + ks * 2048, kChunk, 1024),
+                           tc::desc_mnmajor16_sw128(b_hi + ks * 2048, kChunk, 1024),
+                           tc::desc_mnmajor16_sw128(b_hi + C::B_PLANE + ks * 2048, kChunk, 1024));
+    });
+  ring.drain(acc);
 
   const int c = grp * 2 + wgc;                                // chunk of this warpgroup's 64 rows
   if (c >= P.CH) return;
@@ -225,24 +191,16 @@ wgrad16_reduce_kernel(const __grid_constant__ PlanW16 P, const float* __restrict
 template <int BN>
 int launch_w16(const PlanW16& P, const MapsW16& maps, const float* in_sc, const float* dout_sc,
                float* dw, float* ws, cudaStream_t st) {
-  using C = CfgW16<BN>;
-  static bool attr_set = false;
-  if (!attr_set) {
-    EPB_CUDA(cudaFuncSetAttribute(wgrad16_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                  C::SMEM));
-    attr_set = true;
-  }
   const int64_t ctas = (int64_t)P.groups * P.n_tiles * P.splits;
   EPB_CHECK_ARG(ctas < (1LL << 31));
-  wgrad16_kernel<BN><<<(unsigned)ctas, kThreadsW16, C::SMEM, st>>>(P, maps, in_sc, dout_sc, dw, ws);
+  int rc = tc::launch<wgrad16_kernel<BN>>((unsigned)ctas, kThreadsW16, CfgW16<BN>::SMEM, st, P,
+                                          maps, in_sc, dout_sc, dw, ws);
+  if (rc || P.splits == 1) return rc;
+  const int64_t total = (int64_t)P.Cout * P.T * (P.Cin / 4);
+  int64_t blocks = (total + 255) / 256;
+  if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
+  wgrad16_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(P, in_sc, dout_sc, ws, dw);
   EPB_LAUNCH_CHECK();
-  if (P.splits > 1) {
-    const int64_t total = (int64_t)P.Cout * P.T * (P.Cin / 4);
-    int64_t blocks = (total + 255) / 256;
-    if (blocks > kNumSMs * 8) blocks = kNumSMs * 8;
-    wgrad16_reduce_kernel<<<(unsigned)blocks, 256, 0, st>>>(P, in_sc, dout_sc, ws, dw);
-    EPB_LAUNCH_CHECK();
-  }
   return EPB_OK;
 }
 
@@ -265,49 +223,17 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_wgrad(
   // the output channels on the M side instead (D^T; same products, same sums)
   P.swap = (g->T == 1 && P.CH < 2 && g->Cout / 64 > P.CH) ? 1 : 0;
   P.bdw = P.bdh = 0;
-  const bool dense = g->T == 1 && g->is == 1 && g->os == 1 && g->dh[0] == 0 && g->dw[0] == 0 &&
-                     g->Hp == g->Hi && g->Wp == g->Wi && g->Hp == g->Ho && g->Wp == g->Wo;
-  int N = g->N, Hi = g->Hi, Wi = g->Wi, Ho = g->Ho, Wo = g->Wo;
-  P.N = g->N; P.Hp = g->Hp; P.Wp = g->Wp;
-  if (dense) {
-    const int64_t M = (int64_t)g->N * g->Hp * g->Wp;
-    EPB_CHECK_ARG(M < (1LL << 31));
-    N = 1; Hi = Ho = 1; Wi = Wo = (int)M;
-    P.N = 1; P.Hp = 1; P.Wp = (int)M;
-  }
-  epb_choose_tile(P.N, P.Hp, P.Wp, KT, P.tw, P.th, P.tn);
-  P.tiles_w = (P.Wp + P.tw - 1) / P.tw;
-  P.tiles_h = (P.Hp + P.th - 1) / P.th;
-  const int64_t pt = (int64_t)P.tiles_w * P.tiles_h * ((P.N + P.tn - 1) / P.tn);
-  EPB_CHECK_ARG(pt < (1LL << 30));
-  P.ptiles = (int)pt;
-  bool need[4] = {false, false, false, false};
-  for (int t = 0; t < g->T; ++t) {
-    int qh, qw, dq_h, dq_w;
-    epb_tap_split(g->dh[t], g->is, qh, dq_h);
-    epb_tap_split(g->dw[t], g->is, qw, dq_w);
-    P.map[t] = (unsigned char)(qh * 2 + qw);
-    P.dhq[t] = (short)dq_h;
-    P.dwq[t] = (short)dq_w;
-    P.wt[t] = g->wt[t];
-    need[qh * 2 + qw] = true;
-  }
+  for (int t = 0; t < g->T; ++t) P.wt[t] = g->wt[t];
+  bool dense;
   CUtensorMap in_maps[4];
   memset(in_maps, 0, sizeof(in_maps));
-  for (int v = 0; v < 4; ++v) {
-    if (!need[v]) continue;
-    rc = epb_make_act_map(&in_maps[v], in, N, Hi, Wi, g->Cin, g->is, v >> 1, v & 1, P.tw, P.th, P.tn);
-    if (rc) return rc;
-  }
-  for (int v = 0; v < 4; ++v)
-    if (!need[v]) {
-      for (int u = 0; u < 4; ++u)
-        if (need[u]) { in_maps[v] = in_maps[u]; break; }
-    }
-  CUtensorMap d_map;
-  rc = epb_make_act_map(&d_map, dout, N, Ho, Wo, g->Cout, g->os, g->ph, g->pw, P.tw, P.th, P.tn);
+  rc = epb_plan_phase_grid(g, in, KT, P.grid, in_maps, dense);
   if (rc) return rc;
-  int bn;
+  // dout on the phase grid: a dense layer's output is the same [M][Cout] matrix
+  CUtensorMap d_map;
+  rc = epb_make_act_map(&d_map, dout, P.grid.N, dense ? 1 : g->Ho, dense ? P.grid.Wp : g->Wo,
+                        g->Cout, g->os, g->ph, g->pw, P.grid.tw, P.grid.th, P.grid.tn);
+  if (rc) return rc;
   if (!P.swap) {
     for (int v = 0; v < 4; ++v) maps.a[v] = in_maps[v];
     maps.d = d_map;
@@ -315,26 +241,26 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_wgrad(
   } else {
     // M side: the CH' = Cout / 64 blocks of dout (no tap shift); N side: the input, shifted by the tap
     for (int v = 0; v < 4; ++v) maps.a[v] = d_map;
-    maps.d = in_maps[P.map[0]];
-    P.bdw = P.dwq[0]; P.bdh = P.dhq[0];
-    P.map[0] = 0; P.dwq[0] = 0; P.dhq[0] = 0;
+    maps.d = in_maps[P.grid.map[0]];
+    P.bdw = P.grid.dwq[0]; P.bdh = P.grid.dhq[0];
+    P.grid.map[0] = 0; P.grid.dwq[0] = 0; P.grid.dhq[0] = 0;
     P.CB = g->Cout / 64;
     P.CH = P.CB;
     P.Nn = g->Cin;
   }
-  bn = P.Nn <= 64 ? 64 : 128;
+  const int bn = P.Nn <= 64 ? 64 : 128;
   P.n_tiles = (P.Nn + bn - 1) / bn;
   P.groups = (P.CH + 1) / 2;
   // pixel-range splits: fill two waves of CTAs (which also keeps the fp32 accumulation runs
   // short), keep >= 8 stages per CTA, and stay inside the scratch the caller gave
   const int64_t basec = (int64_t)P.groups * P.n_tiles;
   int64_t splits = 2 * kNumSMs / basec;
-  if (splits > P.ptiles / 8) splits = P.ptiles / 8;
+  if (splits > P.grid.tiles / 8) splits = P.grid.tiles / 8;
   const int64_t per_split = (int64_t)g->Cout * g->Tw * g->Cin;
   if (!ws || splits * per_split > ws_floats) splits = ws ? ws_floats / per_split : 1;
   if (splits < 1) splits = 1;
-  P.tiles_per_split = (int)((P.ptiles + splits - 1) / splits);
-  P.splits = (P.ptiles + P.tiles_per_split - 1) / P.tiles_per_split;
+  P.tiles_per_split = (int)((P.grid.tiles + splits - 1) / splits);
+  P.splits = (P.grid.tiles + P.tiles_per_split - 1) / P.tiles_per_split;
   cudaStream_t st = as_stream(stream);
   if (bn == 64) return launch_w16<64>(P, maps, in_sc, dout_sc, dw, ws, st);
   return launch_w16<128>(P, maps, in_sc, dout_sc, dw, ws, st);

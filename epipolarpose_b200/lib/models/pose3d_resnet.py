@@ -25,7 +25,7 @@ from epipolarpose_b200 import _sinks
 BN_MOMENTUM = 0.1
 logger = logging.getLogger(__name__)
 
-# f16x3: split-fp16 operands, three kind::f16 tensor passes (net16.Engine16); plans with
+# f16x3: split-fp16 operands, three wgmma f16 MMAs per k-step (net16.Engine16); plans with
 # channel counts outside whole 64-element TMA boxes keep the 3xTF32 engine
 _PRECISIONS = {"fp32": 0, "tf32": 1, "tf32x3": 3, "f16x3": 4}
 DEFAULT_PRECISION = "f16x3"

@@ -5,7 +5,7 @@ data layout in HBM: every GEMM operand is materialised ONCE as two fp16 planes
 (x * s = hi + lo, include/epb.h "split-fp16 operand family") by the kernel that produces it
 -- the BatchNorm+ReLU(+residual) pass of each conv output, the BatchNorm-backward apply pass
 of each gradient, the weight packer -- so that the conv kernels (csrc/conv16.cu,
-csrc/wgrad16.cu) take both operands by TMA and run three kind::f16 tensor passes per k-step
+csrc/wgrad16.cu) take both operands by TMA and run three wgmma f16 MMAs per k-step
 at twice the TF32 rate, with fp32-grade results (a_lo*b_hi + a_hi*b_lo + a_hi*b_hi).
 
 Kept per conv: the raw output z (fp32, for the BatchNorm backward) and the post-activation
