@@ -58,6 +58,8 @@ _PROTOS = {
     "epb_patch_to_image": (c_int, [c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_p, c_p]),
     "epb_triangulate": (c_int, [c_p, c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p]),
     "epb_triangulate_nview": (c_int, [c_p, c_int, c_p, c_int, c_int, c_int, c_p, c_p, c_p]),
+    "epb_relative_pose": (c_int, [c_p, c_int, c_p, c_p, c_int, c_int, c_d, c_p, c_p, c_p, c_p, c_p, c_p,
+                                  c_p]),
     "epb_project_labels": (c_int, [c_p, c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_p, c_p, c_p]),
     "epb_h36m_eval": (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, ctypes.c_uint32, c_d, c_p, c_p, c_p, c_p, c_p]),
     "epb_add3": (c_int, [c_p, c_p, c_p, c_p, c_i64, c_p]),

@@ -817,6 +817,325 @@ __global__ void h36m_eval_kernel(const double* __restrict__ pred, const double* 
                    poses ? poses + (int64_t)s * J * 9 : nullptr);
 }
 
+// --------------------------------------------------------------- relative pose (no extrinsics)
+// Self-supervision without camera extrinsics: the geometry of a view pair comes from its own
+// predicted 2-D joints.  The reference leaves only the pieces (lib/utils/cameras.py:133-143,
+// Camera.get_essential_matrix / get_fundamental_matrix with cv2.FM_LMEDS, no caller); per pair
+// (a = sample i, b = sample i + B/2):
+//   1. robust F by least median of squares: RP_HYP hypotheses, each fundamental_8point on 8
+//      distinct joints, scored by the lower median over all J joints of the squared Sampson
+//      distance (px^2); best = lowest score, ties to the lowest hypothesis; inliers r^2 <=
+//      max((2.5 sigma)^2, (1e-3 px)^2), sigma = 1.4826 (1 + 5/(J-8)) sqrt(score); refit
+//      fundamental_8point on the inliers.  DEPARTURES from cv2.findFundamentalMat(FM_LMEDS):
+//      the joints of hypothesis h are a FIXED schedule (the first 8 entries of a Fisher-Yates
+//      shuffle of 0..J-1 driven by splitmix64 seeded with h), the same for every pair and step,
+//      so the estimate is deterministic (cv2 draws them at random); the points are not
+//      truncated to integers as the reference's np.int32 cast does.  256 hypotheses draw an
+//      outlier-free 8-set with 99.9 % probability at 6 outliers among 17 joints.
+//   2. E = K_b^T F K_a; E = U diag(s) V^T by the one-sided Jacobi SVD, columns ordered by
+//      decreasing s, u3 = u1 x u2 and v3 = v1 x v2 (det U = det V = +1) and the sign of the
+//      pair (u1, v1) chosen so that the largest-magnitude entry of u3 is positive (this makes
+//      the candidate order independent of the SVD's sign conventions).  Candidates, in order:
+//      (U W V^T, u3), (U W V^T, -u3), (U W^T V^T, u3), (U W^T V^T, -u3); the one with the most
+//      DLT-triangulated inliers in front of both cameras wins (ties to the first).
+//   3. scale (our rule; the reference has none): with |t| = 1 the root joint (0) is
+//      triangulated at depths Z_a, Z_b; s_v = f_x,v rect3d_w / (bb_w,v scale_v Z_v) is the scale
+//      at which the box spans rect3d_w mm at the root's depth -- the assumption the label
+//      arithmetic of project_labels_kernel already makes -- and t <- sqrt(s_a s_b) t.
+//   4. P_a = K_a [I|0], P_b = K_b [R|t]; cam rows a: R = I, T = 0; b: R, T = -R^T t.
+// status 0 (R = I, t = 0, no NaN in any output) for: no valid hypothesis, fewer than 8
+// inliers, a failed refit, fewer than max(8, ceil(n_inl/2)) inliers in front for the winner,
+// Z_a <= 0 or Z_b <= 0, or any non-finite value.  The body is shared by the kernel (one warp per
+// pair: lanes split the hypotheses and the cheirality DLTs) and the CPU harness (one lane).
+constexpr int RP_HYP = 256;
+constexpr int RP_MAXJ = 32;
+
+__host__ __device__ inline uint64_t splitmix64_next(uint64_t& s) {
+  uint64_t z = (s += 0x9E3779B97F4A7C15ull);
+  z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
+  z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
+  return z ^ (z >> 31);
+}
+
+__host__ __device__ inline bool finite2(const double* p) {
+  return isfinite(p[0]) && isfinite(p[1]);
+}
+
+// hypothesis h: fundamental_8point on its 8 scheduled joints (false: a non-finite joint or no F)
+__host__ __device__ inline bool relpose_hypothesis(const double* ua, const double* ub, int su, int J,
+                                                   int h, double* F) {
+  int perm[RP_MAXJ];
+  for (int i = 0; i < J; ++i) perm[i] = i;
+  uint64_t s = (uint64_t)h;
+  double a[16], b[16];
+  for (int k = 0; k < 8; ++k) {
+    const int r = k + (int)(splitmix64_next(s) % (uint64_t)(J - k));
+    const int t = perm[k];
+    perm[k] = perm[r];
+    perm[r] = t;
+    const double* pa = ua + (int64_t)perm[k] * su;
+    const double* pb = ub + (int64_t)perm[k] * su;
+    if (!finite2(pa) || !finite2(pb)) return false;
+    a[2 * k] = pa[0]; a[2 * k + 1] = pa[1];
+    b[2 * k] = pb[0]; b[2 * k + 1] = pb[1];
+  }
+  return fundamental_8point(a, b, 2, 8, F);
+}
+
+// squared Sampson distance (px^2) of the match (a, b) to F; +inf when not finite
+__host__ __device__ inline double sampson2(const double* F, const double* a, const double* b) {
+  const double x1 = a[0], y1 = a[1], x2 = b[0], y2 = b[1];
+  const double f0 = (F[0] * x1 + F[1] * y1) + F[2];       // F (x1, y1, 1)
+  const double f1 = (F[3] * x1 + F[4] * y1) + F[5];
+  const double f2 = (F[6] * x1 + F[7] * y1) + F[8];
+  const double g0 = (F[0] * x2 + F[3] * y2) + F[6];       // F^T (x2, y2, 1)
+  const double g1 = (F[1] * x2 + F[4] * y2) + F[7];
+  const double e = (x2 * f0 + y2 * f1) + f2;
+  const double r = e * e / (((f0 * f0 + f1 * f1) + g0 * g0) + g1 * g1);
+  return isfinite(r) ? r : INFINITY;
+}
+
+// lower median over the J joints of the squared Sampson distance
+__host__ __device__ inline double relpose_score(const double* F, const double* ua, const double* ub,
+                                                int su, int J) {
+  double r[RP_MAXJ];
+  for (int j = 0; j < J; ++j) {
+    const double v = sampson2(F, ua + (int64_t)j * su, ub + (int64_t)j * su);
+    int i = j;
+    for (; i > 0 && r[i - 1] > v; --i) r[i] = r[i - 1];
+    r[i] = v;
+  }
+  return r[(J - 1) / 2];
+}
+
+// per-lane reductions of relpose_pair: one lane on the host, a full warp on the device
+struct RpSerial {
+  int lane = 0, n = 1;
+  __host__ __device__ void argmin(double&, int&) const {}
+  __host__ __device__ int sum(int v) const { return v; }
+};
+struct RpWarp {
+  int lane, n = 32;
+  __host__ __device__ void argmin(double& s, int& h) const {
+#ifdef __CUDA_ARCH__
+    for (int o = 16; o > 0; o >>= 1) {
+      const double os = __shfl_xor_sync(0xffffffffu, s, o);
+      const int oh = __shfl_xor_sync(0xffffffffu, h, o);
+      if (os < s || (os == s && oh < h)) { s = os; h = oh; }
+    }
+#endif
+  }
+  __host__ __device__ int sum(int v) const {
+#ifdef __CUDA_ARCH__
+    return __reduce_add_sync(0xffffffffu, v);
+#else
+    return v;
+#endif
+  }
+};
+
+// candidate c of the decomposition: R (row-major) and unit t
+__host__ __device__ inline void relpose_candidate(const double (&R1)[9], const double (&R2)[9],
+                                                  const double (&u3)[3], int c, double* R, double* t) {
+  for (int k = 0; k < 9; ++k) R[k] = c < 2 ? R1[k] : R2[k];
+  const double sg = (c & 1) ? -1.0 : 1.0;
+  for (int k = 0; k < 3; ++k) t[k] = sg * u3[k];
+}
+
+// K [R|t] (row-major 3x4) from intrinsics f(2) c(2)
+__host__ __device__ inline void relpose_P(const double* in, const double* R, const double* t, double* P) {
+  for (int k = 0; k < 4; ++k) {
+    const double r0 = k < 3 ? R[k] : t[0], r1 = k < 3 ? R[3 + k] : t[1], r2 = k < 3 ? R[6 + k] : t[2];
+    P[k] = in[0] * r0 + in[2] * r2;
+    P[4 + k] = in[1] * r1 + in[3] * r2;
+    P[8 + k] = r2;
+  }
+}
+
+// DLT of joint j with P_a = K_a[I|0], P_b = K_b[R|t]; returns the two depths
+__host__ __device__ inline bool relpose_depths(const double* ua, const double* ub, const double* Pab,
+                                               const double* R, const double* t, double& za,
+                                               double& zb) {
+  const double uu[4] = {ua[0], ua[1], ub[0], ub[1]};
+  double x[3];
+  const int st = dlt_nview<2>(uu, Pab, x);
+  za = x[2];
+  zb = ((R[6] * x[0] + R[7] * x[1]) + R[8] * x[2]) + t[2];
+  return st != 0;
+}
+
+// One view pair.  ia / ib: f(2) c(2); box: c_x c_y w h scale rot.  Outputs as epb_relative_pose;
+// diag (may be null): chosen hypothesis (-1: none), chosen candidate (-1: none), inlier count.
+template <class Red>
+__host__ __device__ void relpose_pair(const Red& red, const double* ua, const double* ub, int su, int J,
+                                      const double* ia, const double* ib, const double* boxa,
+                                      const double* boxb, double rect3d_w, double* Pa, double* Pb,
+                                      double* cama, double* camb, int32_t* inl, int32_t* status,
+                                      int32_t* diag) {
+  // 1. hypotheses: lane l scores h = l, l + n, ...; (score, h) minimum across the lanes
+  double best = INFINITY;
+  int bh = RP_HYP;
+  for (int h = red.lane; h < RP_HYP; h += red.n) {
+    double F[9];
+    if (!relpose_hypothesis(ua, ub, su, J, h, F)) continue;
+    const double s = relpose_score(F, ua, ub, su, J);
+    if (s < best) { best = s; bh = h; }
+  }
+  red.argmin(best, bh);
+  // every lane repeats the (cheap, identical) serial part, so `ok` is warp-uniform
+  bool ok = bh < RP_HYP;
+  double F[9];
+  unsigned mask = 0u;
+  int n_inl = 0;
+  if (ok) {
+    relpose_hypothesis(ua, ub, su, J, bh, F);
+    const double sig = J > 8 ? 1.4826 * (1.0 + 5.0 / (J - 8)) * sqrt(best) : INFINITY;
+    const double thr = J > 8 ? fmax(2.5 * sig * (2.5 * sig), 1e-6) : DBL_MAX;
+    for (int j = 0; j < J; ++j)
+      if (sampson2(F, ua + (int64_t)j * su, ub + (int64_t)j * su) <= thr) { mask |= 1u << j; ++n_inl; }
+  }
+  ok = ok && n_inl >= 8;
+  if (ok) {                                            // refit on the inliers
+    double ga[2 * RP_MAXJ], gb[2 * RP_MAXJ];
+    int n = 0;
+    for (int j = 0; j < J; ++j)
+      if ((mask >> j) & 1u) {
+        ga[2 * n] = ua[(int64_t)j * su]; ga[2 * n + 1] = ua[(int64_t)j * su + 1];
+        gb[2 * n] = ub[(int64_t)j * su]; gb[2 * n + 1] = ub[(int64_t)j * su + 1];
+        ++n;
+      }
+    ok = fundamental_8point(ga, gb, 2, n, F);
+  }
+  // 2. E = K_b^T F K_a and its decomposition
+  double R1[9], R2[9], u3[3];
+  if (ok) {
+    const double Ka[3][3] = {{ia[0], 0, ia[2]}, {0, ia[1], ia[3]}, {0, 0, 1}};
+    const double Kb[3][3] = {{ib[0], 0, ib[2]}, {0, ib[1], ib[3]}, {0, 0, 1}};
+    double M[3][3], A[3][3], V[3][3];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j)
+        M[i][j] = (F[i * 3 + 0] * Ka[0][j] + F[i * 3 + 1] * Ka[1][j]) + F[i * 3 + 2] * Ka[2][j];
+    for (int i = 0; i < 3; ++i)
+      for (int j = 0; j < 3; ++j) {
+        A[i][j] = (Kb[0][i] * M[0][j] + Kb[1][i] * M[1][j]) + Kb[2][i] * M[2][j];
+        ok = ok && isfinite(A[i][j]);
+      }
+    if (ok) {
+      jacobi_onesided<3, 3>(A, V);
+      double sg[3];
+      for (int c = 0; c < 3; ++c) sg[c] = sqrt(A[0][c] * A[0][c] + A[1][c] * A[1][c] + A[2][c] * A[2][c]);
+      int o0 = 0, o1 = 1, o2 = 2, tmp;                   // stable sort, decreasing
+      if (sg[o1] > sg[o0]) { tmp = o0; o0 = o1; o1 = tmp; }
+      if (sg[o2] > sg[o1]) { tmp = o1; o1 = o2; o2 = tmp; }
+      if (sg[o1] > sg[o0]) { tmp = o0; o0 = o1; o1 = tmp; }
+      double u1[3], u2[3], v1[3], v2[3], v3[3];
+      for (int r = 0; r < 3; ++r) {
+        u1[r] = A[r][o0] / sg[o0]; u2[r] = A[r][o1] / sg[o1];
+        v1[r] = V[r][o0]; v2[r] = V[r][o1];
+      }
+      u3[0] = u1[1] * u2[2] - u1[2] * u2[1];
+      u3[1] = u1[2] * u2[0] - u1[0] * u2[2];
+      u3[2] = u1[0] * u2[1] - u1[1] * u2[0];
+      v3[0] = v1[1] * v2[2] - v1[2] * v2[1];
+      v3[1] = v1[2] * v2[0] - v1[0] * v2[2];
+      v3[2] = v1[0] * v2[1] - v1[1] * v2[0];
+      int km = 0;
+      for (int k = 1; k < 3; ++k) if (fabs(u3[k]) > fabs(u3[km])) km = k;
+      if (u3[km] < 0) {
+        for (int k = 0; k < 3; ++k) { u1[k] = -u1[k]; v1[k] = -v1[k]; u3[k] = -u3[k]; v3[k] = -v3[k]; }
+      }
+      // U W V^T = u2 v1^T - u1 v2^T + u3 v3^T,  U W^T V^T = -u2 v1^T + u1 v2^T + u3 v3^T
+      for (int i = 0; i < 3; ++i)
+        for (int j = 0; j < 3; ++j) {
+          const double p = u2[i] * v1[j] - u1[i] * v2[j], q = u3[i] * v3[j];
+          R1[i * 3 + j] = p + q;
+          R2[i * 3 + j] = q - p;
+          ok = ok && isfinite(R1[i * 3 + j]) && isfinite(R2[i * 3 + j]);
+        }
+    }
+  }
+  // cheirality: lanes split the (candidate, joint) DLTs
+  const double I3[9] = {1, 0, 0, 0, 1, 0, 0, 0, 1}, z3[3] = {0, 0, 0};
+  double Pab[24];
+  relpose_P(ia, I3, z3, Pab);
+  int cnt[4] = {0, 0, 0, 0};
+  const bool cheir = ok;
+  if (ok) {
+    for (int i = red.lane; i < 4 * J; i += red.n) {
+      const int c = i / J, j = i - c * J;
+      if (!((mask >> j) & 1u)) continue;
+      double R[9], t[3], za, zb;
+      relpose_candidate(R1, R2, u3, c, R, t);
+      relpose_P(ib, R, t, Pab + 12);
+      if (relpose_depths(ua + (int64_t)j * su, ub + (int64_t)j * su, Pab, R, t, za, zb) && za > 0 && zb > 0)
+        ++cnt[c];
+    }
+  }
+  int win = 0;
+  for (int c = 0; c < 4; ++c) {
+    cnt[c] = red.sum(cnt[c]);
+    if (cnt[c] > cnt[win]) win = c;
+  }
+  ok = ok && cnt[win] >= (n_inl + 1) / 2 && cnt[win] >= 8;
+  // 3. scale from the root joint
+  double R[9], t[3];
+  relpose_candidate(R1, R2, u3, win, R, t);
+  if (ok) {
+    double za, zb;
+    relpose_P(ib, R, t, Pab + 12);
+    ok = relpose_depths(ua, ub, Pab, R, t, za, zb) && za > 0 && zb > 0;
+    if (ok) {
+      const double sa = ia[0] * rect3d_w / (boxa[2] * boxa[4] * za);
+      const double sb = ib[0] * rect3d_w / (boxb[2] * boxb[4] * zb);
+      const double s = sqrt(sa * sb);
+      for (int k = 0; k < 3; ++k) t[k] *= s;
+    }
+  }
+  // 4. outputs
+  double pb[12], T[3];
+  if (ok) {
+    relpose_P(ib, R, t, pb);
+    for (int k = 0; k < 3; ++k) T[k] = -((R[k] * t[0] + R[3 + k] * t[1]) + R[6 + k] * t[2]);
+    for (int k = 0; k < 12; ++k) ok = ok && isfinite(pb[k]) && isfinite(Pab[k]);
+    for (int k = 0; k < 3; ++k) ok = ok && isfinite(T[k]);
+  }
+  if (!ok) {
+    for (int k = 0; k < 9; ++k) R[k] = I3[k];
+    for (int k = 0; k < 3; ++k) { t[k] = 0.0; T[k] = 0.0; }
+    relpose_P(ib, R, t, pb);
+  }
+  if (red.lane != 0) return;
+  for (int k = 0; k < 12; ++k) { Pa[k] = Pab[k]; Pb[k] = pb[k]; }
+  for (int k = 0; k < 9; ++k) { cama[k] = I3[k]; camb[k] = R[k]; }
+  for (int k = 0; k < 3; ++k) { cama[9 + k] = 0.0; camb[9 + k] = T[k]; }
+  for (int k = 0; k < 4; ++k) { cama[12 + k] = ia[k]; camb[12 + k] = ib[k]; }
+  for (int j = 0; j < J; ++j) inl[j] = (mask >> j) & 1u;
+  *status = ok ? 1 : 0;
+  if (diag) {
+    diag[0] = bh < RP_HYP ? bh : -1;
+    diag[1] = cheir ? win : -1;
+    diag[2] = n_inl;
+  }
+}
+
+// u [B][J][stride_u], intr [B][4], box [B][6]; one warp per pair i = (i, i + NP)
+__global__ void relative_pose_kernel(const double* __restrict__ u, int stride_u,
+                                     const double* __restrict__ intr, const double* __restrict__ box,
+                                     int NP, int J, double rect3d_w, double* __restrict__ Pa,
+                                     double* __restrict__ Pb, double* __restrict__ cam,
+                                     int32_t* __restrict__ inl, int32_t* __restrict__ status,
+                                     int32_t* __restrict__ diag) {
+  const int pair = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (pair >= NP) return;                                  // warp-uniform
+  RpWarp red;
+  red.lane = threadIdx.x & 31;
+  const int a = pair, b = pair + NP;
+  relpose_pair(red, u + (int64_t)a * J * stride_u, u + (int64_t)b * J * stride_u, stride_u, J,
+               intr + a * 4, intr + b * 4, box + a * 6, box + b * 6, rect3d_w, Pa + pair * 12,
+               Pb + pair * 12, cam + a * 16, cam + b * 16, inl + (int64_t)pair * J, status + pair,
+               diag ? diag + pair * 3 : nullptr);
+}
+
 // --------------------------------------------------------------- argmax
 // inference.py:24-39: one warp per (n,j) map; (value, index) reduction with
 // smallest-index tie-break == numpy argmax first-occurrence.  NaN: numpy
@@ -880,6 +1199,21 @@ extern "C" __attribute__((visibility("default"))) int epb_triangulate(const doub
   }
   triangulate_kernel<<<(n + 63) / 64, 64, 0, st>>>(u1, u2, stride_u, P1, P2, NP, J, method, tol,
                                                    Fpair, X, status);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_relative_pose(
+    const double* u, int stride_u, const double* intr, const double* box, int B, int J,
+    double rect3d_w, double* Pa, double* Pb, double* cam, int32_t* inliers, int32_t* status,
+    int32_t* diag, epb_stream_t stream) {
+  EPB_CHECK_ARG(u && intr && box && Pa && Pb && cam && inliers && status);
+  EPB_CHECK_ARG(B >= 0 && B % 2 == 0 && J >= 8 && J <= RP_MAXJ && stride_u >= 2);
+  const int NP = B / 2;
+  if (NP == 0) return EPB_OK;
+  const int threads = 128;                         // 4 pairs per block, one warp each
+  relative_pose_kernel<<<(NP * 32 + threads - 1) / threads, threads, 0, as_stream(stream)>>>(
+      u, stride_u, intr, box, NP, J, rect3d_w, Pa, Pb, cam, inliers, status, diag);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

@@ -7,8 +7,10 @@ the six experiments/*.yaml files parse unchanged; unknown keys raise
 ValueError exactly like reference :167,184.
 
 Extra keys (superset, all default-off): TRAIN.ONLINE_TRIANGULATION,
-TRAIN.TRIANGULATION_METHOD, TRAIN.CUDA_GRAPH (default on), MODEL.PRECISION,
-DATASET.SYNTHETIC_LEN.
+TRAIN.TRIANGULATION_METHOD, TRAIN.ESTIMATE_EXTRINSICS (self-supervision without camera
+extrinsics: each view pair's pose is estimated from its 2-D joints; needs
+TRAIN.ONLINE_TRIANGULATION, ValueError otherwise), TRAIN.CUDA_GRAPH (default on),
+MODEL.PRECISION, DATASET.SYNTHETIC_LEN.
 """
 import os
 
@@ -60,7 +62,8 @@ _DEFAULTS = dict(
     TRAIN=dict(LR_FACTOR=0.1, LR_STEP=[90, 110], LR=0.001, OPTIMIZER='adam', MOMENTUM=0.9,
                WD=0.0001, NESTEROV=False, GAMMA1=0.99, GAMMA2=0.0, BEGIN_EPOCH=0, END_EPOCH=140,
                RESUME=False, CHECKPOINT='', BATCH_SIZE=32, SHUFFLE=True,
-               ONLINE_TRIANGULATION=False, TRIANGULATION_METHOD='iterative', CUDA_GRAPH=True),
+               ONLINE_TRIANGULATION=False, TRIANGULATION_METHOD='iterative', ESTIMATE_EXTRINSICS=False,
+               CUDA_GRAPH=True),
     TEST=dict(BATCH_SIZE=32, FLIP_TEST=False, POST_PROCESS=True, SHIFT_HEATMAP=True,
               USE_GT_BBOX=False, OKS_THRE=0.5, IN_VIS_THRE=0.0, COCO_BBOX_FILE='', BBOX_THRE=1.0,
               MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0),
@@ -110,6 +113,15 @@ def update_config(config_file):
             _merge_section(key, val)
         else:
             config[key] = val
+    check_config(config)
+
+
+def check_config(cfg):
+    """Combinations of keys that cannot be trained: ValueError."""
+    train = cfg.get('TRAIN', {})
+    if train.get('ESTIMATE_EXTRINSICS', False) and not train.get('ONLINE_TRIANGULATION', False):
+        raise ValueError("TRAIN.ESTIMATE_EXTRINSICS needs TRAIN.ONLINE_TRIANGULATION: the estimated "
+                         "camera geometry only feeds the online epipolar labels")
 
 
 def gen_config(config_file):

@@ -10,7 +10,9 @@ Differences from the reference body (same observable behaviour):
     batch by the epipolar self-supervision path (lib/utils/img_utils.py
     self_supervision: soft-argmax -> patch->image -> two-view triangulation ->
     re-projection) entirely on the device -- the glue the released reference
-    leaves unwired (SURVEY.md section 3.3);
+    leaves unwired (SURVEY.md section 3.3); with config.TRAIN.ESTIMATE_EXTRINSICS the
+    cameras of each view pair are estimated from the predicted 2-D joints (no R, T or
+    projection matrix needed: the reference's "without R/t" mode);
   * the gradient all-reduce for multi-GPU data parallelism happens inside the
     model's backward (one NCCL call on the flat gradient buffer).
 """
@@ -51,21 +53,37 @@ def _online_tri(config):
     return bool(train is not None and getattr(train, 'ONLINE_TRIANGULATION', False))
 
 
-def online_epipolar_loss(criterion, preds, meta, method="iterative"):
+def _estimate_extrinsics(config):
+    """TRAIN.ESTIMATE_EXTRINSICS: the pair geometry comes from the predicted 2-D joints
+    (self-supervision without camera extrinsics); it only applies to online triangulation."""
+    train = getattr(config, 'TRAIN', None)
+    est = bool(train is not None and getattr(train, 'ESTIMATE_EXTRINSICS', False))
+    if est and not _online_tri(config):
+        raise ValueError("TRAIN.ESTIMATE_EXTRINSICS needs TRAIN.ONLINE_TRIANGULATION")
+    return est
+
+
+def online_epipolar_loss(criterion, preds, meta, method="iterative", estimate_extrinsics=False):
     """criterion(preds, labels(preds), 1) with the labels produced by the epipolar
     self-supervision path from the SAME soft-argmax coordinates the loss uses
-    (labels carry no gradient, reference integral_loss.py:88-91)."""
+    (labels carry no gradient, reference integral_loss.py:88-91).  estimate_extrinsics:
+    the cameras of each view pair are estimated from its own 2-D joints, and pairs whose
+    estimate failed carry weight 0."""
     from .integral_loss import softmax_integral_tensor, _WeightedLossFn
     from ..utils.img_utils import (patch_to_image_device, triangulate_device,
-                                   labels_from_global_coords_device)
+                                   labels_from_global_coords_device,
+                                   labels_estimated_extrinsics_device)
     J = criterion.num_joints
     W, H = preds.shape[-1], preds.shape[-2]
     D = preds.shape[-3] // J
     coords = softmax_integral_tensor(preds, J, True, W, H, D)
     with torch.no_grad():
         kps = patch_to_image_device(coords.detach(), meta)
-        X = triangulate_device(kps, meta, method)
-        label, weight = labels_from_global_coords_device(X, meta)
+        if estimate_extrinsics:
+            label, weight = labels_estimated_extrinsics_device(kps, meta, method)
+        else:
+            X = triangulate_device(kps, meta, method)
+            label, weight = labels_from_global_coords_device(X, meta)
     return _WeightedLossFn.apply(coords, label, weight, criterion._kind, criterion.size_average,
                                  criterion.norm)
 
@@ -78,13 +96,17 @@ class GraphedTrainStep:
     memory (FusedAdam / FusedSGD), so LR schedules keep working.  The first call runs
     eagerly (sizes workspaces, one-time attributes), the second captures and replays."""
 
-    def __init__(self, model, criterion, optimizer, online=False, method="iterative"):
+    def __init__(self, model, criterion, optimizer, online=False, method="iterative",
+                 estimate_extrinsics=False):
         # scripts/train.py:94 wraps the model in nn.DataParallel(device_ids=[k]); with one
         # device id that wrapper only forwards the call (and its scatter is not capturable)
         if isinstance(model, torch.nn.DataParallel) and len(model.device_ids) == 1:
             model = model.module
         self.model, self.criterion, self.optimizer = model, criterion, optimizer
         self.online, self.method = online, method
+        if estimate_extrinsics and not online:
+            raise ValueError("estimate_extrinsics needs online=True")
+        self.estimate_extrinsics = bool(estimate_extrinsics)
         self.graph = None
         self.key = None
         self.warm_key = None          # shape of the last eager (warm-up) step
@@ -112,7 +134,8 @@ class GraphedTrainStep:
         with _fused_head(self.model):
             preds = self.model(x)
         if self.online:
-            loss = online_epipolar_loss(self.criterion, preds, {"_packed": geom}, self.method)
+            loss = online_epipolar_loss(self.criterion, preds, {"_packed": geom}, self.method,
+                                        self.estimate_extrinsics)
         else:
             loss = self.criterion(preds, label, weight)
         loss.backward()
@@ -162,8 +185,8 @@ class GraphedTrainStep:
         geom = None
         if self.online:
             from ..utils.img_utils import pack_meta
-            geom = pack_meta(meta, B, dev)
-        key = (tuple(batch_data.shape), self.online)
+            geom = pack_meta(meta, B, dev, self.estimate_extrinsics)
+        key = (tuple(batch_data.shape), self.online, self.estimate_extrinsics)
         self.calls += 1
         if self.graph is not None and key == self.key:
             self._load_input(batch_data)
@@ -231,13 +254,15 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
     model.train()
     online = _online_tri(config)
     method = getattr(config.TRAIN, 'TRIANGULATION_METHOD', 'iterative') if online else None
+    estimate = _estimate_extrinsics(config)
     pending = []           # (device loss, batch size) not yet folded into `losses`
     use_graph = bool(getattr(config.TRAIN, 'CUDA_GRAPH', True)) and \
         _graph_capable(model, criterion, optimizer)
     stepper = getattr(model, '_epb_graphed_step', None)
     if use_graph and (stepper is None or stepper.optimizer is not optimizer
-                      or stepper.criterion is not criterion or stepper.online != online):
-        stepper = GraphedTrainStep(model, criterion, optimizer, online, method)
+                      or stepper.criterion is not criterion or stepper.online != online
+                      or stepper.estimate_extrinsics != estimate):
+        stepper = GraphedTrainStep(model, criterion, optimizer, online, method, estimate)
         model._epb_graphed_step = stepper
     end = time.time()
     it = iter(train_loader)
@@ -266,7 +291,7 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
                 preds = model(batch_data)
             if online:
                 # one soft-argmax pass serves both the epipolar labels and the loss
-                loss = online_epipolar_loss(criterion, preds, meta, method)
+                loss = online_epipolar_loss(criterion, preds, meta, method, estimate)
                 batch_label = batch_label_weight = None
             else:
                 batch_label = batch_label.cuda(non_blocking=True)

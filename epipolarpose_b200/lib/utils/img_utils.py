@@ -52,12 +52,24 @@ def _cams(meta, B, dev):
                      dim=1).contiguous()
 
 
-def pack_meta(meta, B, dev):
+def _intrinsics(meta, B, dev):
+    """[B,4] float64: f(2) c(2)."""
+    return torch.cat([_t64(meta['f'], dev).reshape(B, 2), _t64(meta['c'], dev).reshape(B, 2)],
+                     dim=1).contiguous()
+
+
+def pack_meta(meta, B, dev, estimate_extrinsics=False):
     """Collated `meta` -> device float64 tensors {box [B,6], cam [B,16], P [B,3,4]} (the
-    form the kernels consume; static-shaped, so a CUDA graph can re-read them)."""
+    form the kernels consume; static-shaped, so a CUDA graph can re-read them).  Meta with
+    intrinsics `f`, `c` but no `R` -- and every meta when estimate_extrinsics is set, which
+    ignores `R`, `T` and `projection_matrix` -- gives {box, intr [B,4] = f(2) c(2)}."""
     if isinstance(meta, dict) and "_packed" in meta:
         return meta["_packed"]
     out = {"box": _boxes(meta, B, dev)}
+    if estimate_extrinsics or ('R' not in meta and 'f' in meta and 'c' in meta):
+        out["intr"] = _intrinsics(meta, B, dev)
+        if estimate_extrinsics:
+            return out
     if 'R' in meta:
         out["cam"] = _cams(meta, B, dev)
     if 'projection_matrix' in meta:
@@ -100,11 +112,39 @@ def labels_from_global_coords_device(X, meta, patch_w=256., patch_h=256., rect_3
     return label, weight
 
 
-def self_supervision_device(preds, meta, method="iterative"):
+def labels_estimated_extrinsics_device(kps, meta, method="iterative", patch_w=256., patch_h=256.,
+                                       rect_3d_w=2000.):
+    """Self-supervision without camera extrinsics: kps [B,J,4] image px -> (label, weight) f32
+    [B, J*3].  Each pair's projection matrices come from its own 2-D joints
+    (triangulation.relative_pose_pairs; only the box and the intrinsics f, c are read), the pair
+    is triangulated with them by `method` -- after the pose has been scaled, so the iterative
+    method's absolute depth tolerance keeps its meaning -- and re-projected with the estimated
+    cameras.  Pairs whose pose could not be estimated get weight 0 (and label 0) in both views.
+    Static shapes, no host synchronisation: capturable in a CUDA graph."""
+    ops = _backend[0]
+    B, J = kps.shape[0], kps.shape[1]
+    half = B // 2
+    dev = kps.device
+    pm = pack_meta(meta, B, dev, estimate_extrinsics=True)
+    Pa, Pb, cam, _, status = _tri.relative_pose_pairs(kps, pm["intr"], pm["box"], rect_3d_w)
+    X, _ = _tri.triangulate_pairs(kps[:half], kps[half:], Pa, Pb, method=method, stride_u=kps.shape[2])
+    X = torch.cat([X, X], dim=0)
+    label = torch.empty((B, J * 3), device=dev, dtype=torch.float32)
+    weight = torch.empty((B, J * 3), device=dev, dtype=torch.float32)
+    ops.project_labels(X, cam, pm["box"], B, J, patch_w, patch_h, rect_3d_w, label, weight)
+    ok = torch.cat([status, status], dim=0).reshape(B, 1) != 0
+    return torch.where(ok, label, 0.0), weight * ok
+
+
+def self_supervision_device(preds, meta, method="iterative", estimate_extrinsics=False):
     """preds: network output [B, J*D, H, W] (CUDA) -> (label, weight) CUDA f32
-    [B, J*3]; labels carry no gradient (reference integral_loss.py:88-91)."""
+    [B, J*3]; labels carry no gradient (reference integral_loss.py:88-91).  With
+    estimate_extrinsics the cameras come from the predicted 2-D joints themselves
+    (labels_estimated_extrinsics_device; meta needs only the box and f, c)."""
     coords = get_joint_location_coords(preds)
     kps = patch_to_image_device(coords, meta)
+    if estimate_extrinsics:
+        return labels_estimated_extrinsics_device(kps, meta, method)
     X = triangulate_device(kps, meta, method)
     return labels_from_global_coords_device(X, meta)
 

@@ -11,7 +11,9 @@ from the projection matrices, cv2.correctMatches = Hartley-Sturm optimal correct
 the homogeneous DLT) runs as method "polynomial" of the same kernel, including the reference's
 8-point fallback (:215-217): when the correction is NaN for every joint of a pair, F is
 re-estimated from the matches (cv2.findFundamentalMat FM_8POINT) on the device and the
-correction repeated; "polynomial_8point" runs that branch unconditionally."""
+correction repeated; "polynomial_8point" runs that branch unconditionally.
+`relative_pose_pairs` estimates each pair's projection matrices from the 2-D joints alone
+(self-supervision without camera extrinsics)."""
 import numpy as np
 import torch
 
@@ -56,6 +58,34 @@ def triangulate_views(u, P):
     if NT * J:
         ops.triangulate_nview(u.contiguous(), u.shape[3], P.reshape(NT, V, 12).contiguous(), NT, V, J, X, status)
     return X, status
+
+
+def relative_pose_pairs(kps, intr, box, rect3d_w=2000.0, diag=False):
+    """Camera geometry of each view pair from its own 2-D joints (no extrinsics; epb_relative_pose):
+    sample i pairs with i + B/2.  kps [B,J,S>=2] image px, intr [B,4] f(2) c(2), box [B,6], all
+    float64 on the device (B even, 8 <= J <= 32) -> (P_a [NP,3,4], P_b [NP,3,4], cam [B,16],
+    inliers [NP,J] int32, status [NP] int32), NP = B/2; with diag=True also diag [NP,3] int32
+    (chosen hypothesis, chosen candidate, inlier count).  P_a = K_a[I|0], P_b = K_b[R|t] with t
+    scaled so that each box spans rect3d_w mm at the root joint's depth; failed pairs have
+    status 0, R = I and t = 0."""
+    ops = _backend[0]
+    B, J = kps.shape[0], kps.shape[1]
+    if B % 2:
+        raise ValueError("relative_pose_pairs pairs sample i with i + B/2: B must be even, got %d" % B)
+    if not 8 <= J <= 32:
+        raise ValueError("relative_pose_pairs needs 8 <= J <= 32 joints, got %d" % J)
+    NP, dev = B // 2, kps.device
+    Pa = torch.empty((NP, 3, 4), device=dev, dtype=torch.float64)
+    Pb = torch.empty((NP, 3, 4), device=dev, dtype=torch.float64)
+    cam = torch.empty((B, 16), device=dev, dtype=torch.float64)
+    inliers = torch.empty((NP, J), device=dev, dtype=torch.int32)
+    status = torch.empty((NP,), device=dev, dtype=torch.int32)
+    dg = torch.empty((NP, 3), device=dev, dtype=torch.int32) if diag else None
+    if NP:
+        ops.relative_pose(kps.contiguous(), kps.shape[2], intr.contiguous(), box.contiguous(), B, J,
+                          rect3d_w, Pa, Pb, cam, inliers, status, dg)
+    out = (Pa, Pb, cam, inliers, status)
+    return out + (dg,) if diag else out
 
 
 def _device():

@@ -380,6 +380,13 @@ def triangulate_nview(u, stride_u, P, NT, V, J, X, status):
           _p(X, torch.float64), _p(status, torch.int32), _stream())
 
 
+def relative_pose(u, stride_u, intr, box, B, J, rect3d_w, Pa, Pb, cam, inliers, status, diag=None):
+    _call("epb_relative_pose", _p(u, torch.float64), stride_u, _p(intr, torch.float64),
+          _p(box, torch.float64), B, J, float(rect3d_w), _p(Pa, torch.float64), _p(Pb, torch.float64),
+          _p(cam, torch.float64), _p(inliers, torch.int32), _p(status, torch.int32),
+          _p(diag, torch.int32), _stream())
+
+
 def project_labels(X, cam, box, B, J, patch_w, patch_h, rect3d_w, label, weight):
     _call("epb_project_labels", _p(X, torch.float64), _p(cam, torch.float64),
           _p(box, torch.float64), B, J, float(patch_w), float(patch_h), float(rect3d_w),

@@ -407,6 +407,21 @@ int epb_triangulate(const double* u1, const double* u2, int stride_u,
  * 2 <= V <= 4 -> X [NT][J][3], status [NT][J] (max |coordinate| <= 1e16). */
 int epb_triangulate_nview(const double* u, int stride_u, const double* P, int NT, int V, int J,
                           double* X, int32_t* status, epb_stream_t stream);
+/* Relative pose of each view pair from its own 2-D joints, for self-supervision without camera
+ * extrinsics.  Stands in for what the reference only sketches in lib/utils/cameras.py:133-143
+ * (Camera.get_essential_matrix = K2^T F K1, get_fundamental_matrix with cv2.FM_LMEDS; no caller):
+ * deterministic LMedS fundamental matrix (256 fixed 8-joint hypotheses, Sampson distance), E =
+ * K_b^T F K_a, the four (R, t) of E with the cheirality test, t scaled so that each box spans
+ * rect3d_w mm at the root joint's depth (geometric mean of the two views).  Sample i pairs with
+ * i + B/2 (B even, NP = B/2, 8 <= J <= 32).  u [B][J][stride_u] f64 image px (first two entries
+ * used), intr [B][4] f64 = f(2) c(2), box [B][6] as above.  Outputs: Pa = K_a[I|0] and Pb =
+ * K_b[R|t] [NP][12]; cam [B][16] in the epb_project_labels layout (view a: R = I, T = 0; view b:
+ * R, T = -R^T t); inliers [NP][J] 0/1; status [NP] 1 = estimated, 0 = failed (then R = I, t = 0,
+ * no NaN anywhere); diag [NP][3] (may be NULL) = chosen hypothesis, chosen candidate (-1: none),
+ * inlier count. */
+int epb_relative_pose(const double* u, int stride_u, const double* intr, const double* box, int B,
+                      int J, double rect3d_w, double* Pa, double* Pb, double* cam, int32_t* inliers,
+                      int32_t* status, int32_t* diag, epb_stream_t stream);
 /* lib/utils/img_utils.py:212-243 + lib/utils/prep_h36m.py:170-204 +
  * integral_loss.py:170-177: X [B][J][3] world -> label,weight [B][J*3] f32.
  * cam [B][16] f64 = R(9) T(3) f(2) c(2); box as above. */
