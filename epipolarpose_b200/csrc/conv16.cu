@@ -15,9 +15,13 @@
 //
 // One persistent CTA per SM on the pipeline of tc_common.cuh: warpgroup 0 is the TMA
 // producer (one lane: A hi/lo + B hi/lo boxes per k-block), warpgroups 1-2 the consumers
-// (4 k-steps x 3 wgmma m64nBNk16 per k-block).  The epilogue scales, adds the bias, stores
-// or adds, and keeps the BatchNorm statistics of a run of tiles of one N tile in the
-// per-warp slices, flushed once per run.
+// (4 k-steps x 3 wgmma m64nBNk16 per k-block).  The epilogue scales and adds the bias; each
+// consumer warp writes its 16 tile rows 32 columns at a time into its own 2 KB staging box and
+// one lane hands the box to a TMA store (a TMA reduce-add with `accumulate`), so the output
+// write runs in the background while the warp goes on to the next chunk and the next tile's
+// MMAs.  The store map has the extents of the output view: TMA drops the rows and columns
+// beyond it.  The BatchNorm statistics of a run of tiles of one N tile are kept in the
+// per-warp slices from the register values, flushed once per run.
 #include "split16_common.cuh"
 
 namespace {
@@ -26,10 +30,11 @@ constexpr int BM = 128;
 constexpr int kThreads16 = 384;
 constexpr int kConsumers = 256;
 constexpr int kStageBudget = 200 * 1024;
+constexpr int kBoxBytes = 16 * 128;   // staging box of a consumer warp: 16 rows x 32 fp32, SWIZZLE_128B
 
 struct Plan16 {
   epb_phase_grid grid;           // pixel tiles of the phase grid (M side), tap views
-  int Ho, Wo, Cout, os, ph, pw;  // output tensor / phase
+  int Cout;
   int Wv, Hv;                    // extent of the output phase view (rows beyond it are not stored)
   int T, CB;                     // taps, channel blocks of 64 per tap
   int n_tiles;
@@ -41,6 +46,7 @@ struct Plan16 {
 struct Maps16 {
   CUtensorMap a[4];
   CUtensorMap w;
+  CUtensorMap out;               // fp32 (Cout, Wv, Hv, N) output view, box 32 x one warp's 16 rows
 };
 
 template <int BN>
@@ -52,8 +58,10 @@ struct Cfg16 {
   static constexpr int STAGE = A_BYTES + B_BYTES;
   static constexpr int S_ = kStageBudget / STAGE;
   static constexpr int S = S_ > 6 ? 6 : S_;
+  static constexpr int BOX_BYTES = (kConsumers / 32) * kBoxBytes;
   static constexpr int STAT_BYTES = (kConsumers / 32) * 2 * BN * 4;   // per warp [sum | sum of squares][BN]
-  static constexpr int SMEM = S * STAGE + 1024 /*align*/ + 256 /*barriers*/ + STAT_BYTES;
+  static constexpr int SMEM =
+      S * STAGE + BOX_BYTES + 1024 /*align*/ + 256 /*barriers*/ + STAT_BYTES;
   static_assert(SMEM <= 227 * 1024, "shared memory budget");
   static_assert(S >= 2, "ring too shallow");
 };
@@ -62,11 +70,11 @@ template <int BN>
 __global__ void __launch_bounds__(kThreads16, 1)
 conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 maps,
               const float* __restrict__ in_sc, const float* __restrict__ w_sc,
-              const float* __restrict__ bias, float* __restrict__ out,
-              double* __restrict__ stats) {
+              const float* __restrict__ bias, double* __restrict__ stats) {
   using C = Cfg16<BN>;
   const epb_phase_grid& G = P.grid;
-  constexpr int CTRL = C::S * C::STAGE;
+  constexpr int BOXES = C::S * C::STAGE;          // staging boxes follow the slots (1024-aligned)
+  constexpr int CTRL = BOXES + C::BOX_BYTES;
   extern __shared__ uint8_t smem_raw[];
   tc::Ring<C::S, C::STAGE> ring(smem_raw, 0, CTRL, CTRL + 64);     // full[8], empty[8]
   float* sstat = reinterpret_cast<float*>(ring.sm + CTRL + 256);   // [8 warps][2][BN]
@@ -85,6 +93,7 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
     if (warp == 0 && lane == 0) {
       for (int v = 0; v < 4; ++v) tc::tma_prefetch_desc(&maps.a[v]);
       tc::tma_prefetch_desc(&maps.w);
+      tc::tma_prefetch_desc(&maps.out);
       for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
         const int nt = nt_of(tile);
         int w0, h0, n0;
@@ -116,7 +125,14 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
   const int ct = threadIdx.x - 128;            // 0..255
   float* wstat = sstat + (ct >> 5) * 2 * BN;   // this warp's statistics slice
   const int lc = (lane & 3) * 2;
-  const int ra = wgc * 64 + (warp & 3) * 16 + (lane >> 2);   // fragment rows ra, ra + 8
+  const int rb = wgc * 64 + (warp & 3) * 16;   // this warp's 16 tile rows rb .. rb + 15
+  const int ra = rb + (lane >> 2);             // fragment rows ra, ra + 8
+  // staging box: row i at 128 * i, its 16-byte chunk c at chunk c ^ (i % 8) (SWIZZLE_128B);
+  // this lane's float2 of fragment column group jj (columns 8 jj + lc, + 1 of the 32) in row
+  // lane / 4 (+ 8) lies at box + 128 * (lane / 4) (+ 1024) + chunk(jj)
+  uint8_t* box = ring.sm + BOXES + (ct >> 5) * kBoxBytes;
+  const uint32_t box_addr = tc::smem_u32(box);
+  auto chunk = [&](int jj) { return ((2 * jj + ((lane & 3) >> 1)) ^ (lane >> 2)) * 16 + (lane & 1) * 8; };
   const float alpha = in_sc[1] * w_sc[1];
   const int twh = G.tw * G.th;
   if (stats) {
@@ -146,45 +162,60 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
       });
     ring.drain(acc);
 
-    // ---- epilogue straight from the fragment: rows ra (h = 0) and ra + 8 (h = 1)
+    // ---- epilogue: rows ra (h = 0) and ra + 8 (h = 1) of the fragment
     int w0, h0, n0;
     G.tile_origin(mt_of(tile), w0, h0, n0);
-    float* orow[2];
     bool srow[2];
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
       const int r = ra + 8 * h;
       const int w = w0 + r % G.tw, hh = h0 + (r / G.tw) % G.th, n = n0 + r / twh;
-      orow[h] = (w < P.Wv && hh < P.Hv && n < G.N)
-                    ? out + (((int64_t)n * P.Ho + (int64_t)hh * P.os + P.ph) * P.Wo +
-                             (int64_t)w * P.os + P.pw) * P.Cout
-                    : nullptr;
       srow[h] = w < G.Wp && hh < G.Hp && n < G.N;
     }
+    // the warp's rows are the (bw, bh, bn) sub-box of the tile box at (bx, by, bz), bw * bh *
+    // bn = 16 (tile extents are powers of two); a band that starts past the view is all past it
+    const int bx = w0 + rb % G.tw, by = h0 + (rb / G.tw) % G.th, bz = n0 + rb / twh;
+    const bool band = bx < P.Wv && by < P.Hv && bz < G.N;
 #pragma unroll
-    for (int j = 0; j < BN / 8; ++j) {
-      const int cl = 8 * j + lc, col = nt * BN + cl;
-      float v[2][2];
-      float2 b = make_float2(0.f, 0.f);
-      if (bias && col < P.Cout) b = *reinterpret_cast<const float2*>(bias + col);
+    for (int q = 0; q < BN / 32; ++q) {
+      // the previous store has finished reading the box
+      if (lane == 0) tc::tma_store_wait_read<0>();
+      __syncwarp();
 #pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        v[h][0] = acc[4 * j + 2 * h] * alpha + b.x;
-        v[h][1] = acc[4 * j + 2 * h + 1] * alpha + b.y;
-        if (orow[h] && col < P.Cout) {
-          float2* o = reinterpret_cast<float2*>(orow[h] + col);
-          float2 x = make_float2(v[h][0], v[h][1]);
-          if (P.accumulate) {
-            const float2 pv = *o;
-            x.x += pv.x; x.y += pv.y;
-          }
-          *o = x;
+      float v[4][2][2];
+#pragma unroll
+      for (int jj = 0; jj < 4; ++jj) {
+        const int col = nt * BN + 32 * q + 8 * jj + lc;
+        float2 b = make_float2(0.f, 0.f);
+        if (bias && col < P.Cout) b = *reinterpret_cast<const float2*>(bias + col);
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          v[jj][h][0] = acc[16 * q + 4 * jj + 2 * h] * alpha + b.x;
+          v[jj][h][1] = acc[16 * q + 4 * jj + 2 * h + 1] * alpha + b.y;
+          *reinterpret_cast<float2*>(box + 128 * ((lane >> 2) + 8 * h) + chunk(jj)) =
+              make_float2(v[jj][h][0], v[jj][h][1]);
         }
       }
-      if (stats) tc::stats_add<BN>(wstat, cl, v, srow);
+      tc::fence_proxy_async();
+      __syncwarp();
+      const int c0 = nt * BN + 32 * q;
+      if (lane == 0 && band && c0 < P.Cout) {
+        // With `accumulate` the add of the old value happens in the L2: one fp32 add, round to
+        // nearest even, as old + new in registers.  A subnormal old value is kept, not flushed
+        // (tests/test_gpu_conv16_store.py checks both against numpy's fp32 sum).
+        if (P.accumulate) tc::tma_reduce_add_4d(&maps.out, box_addr, c0, bx, by, bz);
+        else tc::tma_store_4d(&maps.out, box_addr, c0, bx, by, bz);
+        tc::tma_store_commit();
+      }
+      // the statistics (same columns, same order) while the store reads the box
+      if (stats) {
+#pragma unroll
+        for (int jj = 0; jj < 4; ++jj) tc::stats_add<BN>(wstat, 32 * q + 8 * jj + lc, v[jj], srow);
+      }
     }
   }
   if (stats && nt_prev >= 0) tc::stats_flush<BN, kConsumers / 32>(sstat, ct, nt_prev, P.Cout, stats);
+  if (lane == 0) tc::tma_store_wait<0>();   // the output is written before the CTA retires
 }
 
 }  // namespace
@@ -199,7 +230,7 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   EPB_CHECK_ARG(g->is == 1 || g->is == 2);
   EPB_CHECK_ARG(!(stats && g->accumulate));
   EPB_CHECK_ARG((reinterpret_cast<uintptr_t>(in) & 127) == 0 && (reinterpret_cast<uintptr_t>(w) & 15) == 0);
-  EPB_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 7) == 0 && (reinterpret_cast<uintptr_t>(bias) & 7) == 0);
+  EPB_CHECK_ARG((reinterpret_cast<uintptr_t>(out) & 15) == 0 && (reinterpret_cast<uintptr_t>(bias) & 7) == 0);
   Plan16 P;
   Maps16 maps;
   memset(&maps, 0, sizeof(maps));
@@ -207,10 +238,26 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   rc = epb_plan_phase_grid(g, in, BM, P.grid, maps.a, dense);
   if (rc) return rc;
   // a dense layer's output is the same [M][Cout] matrix as its phase grid
-  P.Ho = dense ? 1 : g->Ho; P.Wo = dense ? P.grid.Wp : g->Wo; P.Cout = g->Cout; P.os = g->os;
-  P.ph = dense ? 0 : g->ph; P.pw = dense ? 0 : g->pw;
+  const int64_t Ho = dense ? 1 : g->Ho, Wo = dense ? P.grid.Wp : g->Wo, os = g->os;
+  const int64_t ph = dense ? 0 : g->ph, pw = dense ? 0 : g->pw;
+  P.Cout = g->Cout;
   P.Wv = dense ? P.grid.Wp : (g->Wo - g->pw + g->os - 1) / g->os;
   P.Hv = dense ? 1 : (g->Ho - g->ph + g->os - 1) / g->os;
+  {
+    // (Cout, Wv, Hv, N) view of output phase (ph, pw); Cout % 4 == 0 keeps base and strides
+    // 16-byte aligned.  Box: 32 columns x the 16 tile rows of one consumer warp.
+    const int bw = P.grid.tw < 16 ? P.grid.tw : 16;
+    const int bh = P.grid.th < 16 / bw ? P.grid.th : 16 / bw;
+    const int64_t C4 = (int64_t)g->Cout * 4;
+    const cuuint64_t dims[4] = {(cuuint64_t)g->Cout, (cuuint64_t)P.Wv, (cuuint64_t)P.Hv,
+                                (cuuint64_t)P.grid.N};
+    const cuuint64_t strides[3] = {(cuuint64_t)(os * C4), (cuuint64_t)(os * Wo * C4),
+                                   (cuuint64_t)(Ho * Wo * C4)};
+    const cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)(16 / (bw * bh))};
+    rc = epb_encode_map(&maps.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out + (ph * Wo + pw) * g->Cout,
+                        dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_NONE, "output");
+    if (rc) return rc;
+  }
   P.T = g->T; P.CB = g->Cin / 64; P.accumulate = g->accumulate;
   for (int t = 0; t < g->T; ++t) P.koff[t] = g->wt[t] * g->Cin;
   // tile order: statistics want runs of tiles with the same N tile (one flush per run); without
@@ -232,7 +279,7 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   cudaStream_t st = as_stream(stream);
   if (bn == 64)
     return tc::launch<conv16_kernel<64>>(grid, kThreads16, Cfg16<64>::SMEM, st, P, maps, in_sc,
-                                         w_sc, bias, out, stats);
+                                         w_sc, bias, stats);
   return tc::launch<conv16_kernel<128>>(grid, kThreads16, Cfg16<128>::SMEM, st, P, maps, in_sc,
-                                        w_sc, bias, out, stats);
+                                        w_sc, bias, stats);
 }

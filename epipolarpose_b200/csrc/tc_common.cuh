@@ -9,7 +9,9 @@
 // and release the slot on its empty mbarrier (one arrive per consumer warp) once the group
 // has completed.  Ring::consume keeps one k-block of wgmma in flight while the next one is
 // issued.  Split operands are multiplied by the three passes of mma3_*.  Epilogues work
-// straight from the accumulator fragment; the conv epilogues sum BatchNorm statistics with
+// from the accumulator fragment: conv16 stages it per consumer warp in a shared-memory box
+// that a TMA store (or reduce-add) writes out in the background, the other kernels store it
+// straight to global memory; the conv epilogues sum BatchNorm statistics with
 // stats_add / stats_flush in a fixed order.  Every mbarrier wait is bounded (trap instead of
 // hang).
 //
