@@ -682,18 +682,35 @@ bn_bwd_apply_split_kernel(const float4* dy /* may alias dy_masked */, const floa
   }
 }
 
+// Hard bound of |sc * z + sh| over one channel of M rows from its statistics s1 = sum z, s2 = sum z^2
+// as the conv16 epilogue sums them (tc::stats_add / stats_flush).
+//  * No element of a sample lies further than sqrt(M - 1) standard deviations from its mean.
+//  * The statistics carry the rounding of the epilogue's fp32 partial sums.  A value passes through
+//    at most kappa fp32 roundings before its CTA's partial becomes a double: 5 in the 16-row shuffle
+//    tree (with the square), one per tile the CTA ran for this N tile (the warp slice) and 8 in the
+//    warp-order flush.  A CTA runs at most ceil(tiles / kNumSMs) tiles per N tile, and the tile
+//    planner covers at most 8x the rows of the grid (each power-of-two box extent is below twice the
+//    grid extent it spans, or the whole grid is one tile), so tiles <= M / 16 and
+//    kappa = 16 + ceil(M / (16 kNumSMs)).  With u = 2^-24 and q = s2 / M:
+//    |d s1| <= kappa u sum|z| <= kappa u M sqrt(q) and |d s2| <= kappa u M q.  The mean is then off by
+//    at most kappa u sqrt(q), and var = q - mean^2 under-estimates the variance by at most
+//    3 kappa u q plus second-order terms (taken as 4 kappa u q).
+//  A channel whose rows are all equal shows why both terms are needed: var rounds to <= 0, yet
+//  y = sc * (z - mean) carries the mean's rounding times sc = 1/sqrt(eps).
+__device__ __forceinline__ double channel_bound(double s1, double s2, double sc, double sh, double M) {
+  const double mean = s1 / M, q = s2 / M;
+  double var = q - mean * mean;
+  if (var < 0) var = 0;
+  const double ku = (16.0 + ceil(M / (16.0 * kNumSMs))) * 0x1p-24;
+  return fabs(sc * mean + sh) + fabs(sc) * (sqrt(M * (var + 4.0 * ku * q)) + ku * sqrt(q));
+}
+
 // one CTA: hard bound of a post-activation tensor from the statistics of its conv output(s)
 __device__ __forceinline__ float group_bound(const double* stats, const float* scale,
                                              const float* shift, double M, int C) {
   float b = 0.f;
-  for (int c = threadIdx.x; c < C; c += blockDim.x) {
-    const double mean = stats[c] / M;
-    double var = stats[C + c] / M - mean * mean;
-    if (var < 0) var = 0;
-    const double sc = scale[c], sh = shift[c];
-    // no element of a sample lies further than sqrt(M - 1) standard deviations from its mean
-    b = fmaxf(b, (float)(fabs(sc * mean + sh) + fabs(sc) * sqrt(M * var)));
-  }
+  for (int c = threadIdx.x; c < C; c += blockDim.x)
+    b = fmaxf(b, (float)channel_bound(stats[c], stats[C + c], scale[c], shift[c], M));
   return b;
 }
 
@@ -762,7 +779,7 @@ bn_finalize_scale_kernel(const double* __restrict__ stats, double M, int C,
       running_mean[c] = (float)((1.0 - momentum) * running_mean[c] + momentum * mean);
       running_var[c] = (float)((1.0 - momentum) * running_var[c] + momentum * unbiased);
     }
-    b1 = fmaxf(b1, (float)(fabs((double)scf * mean + (double)shf) + fabs((double)scf) * sqrt(M * var)));
+    b1 = fmaxf(b1, (float)channel_bound(stats[c], stats[C + c], scf, shf, M));
   }
   float b2 = stats2 ? group_bound(stats2, scale2, shift2, M, C) : 0.f;
   b1 = warp_max(b1);

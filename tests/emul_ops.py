@@ -549,10 +549,14 @@ def _pow2_scale(amax):
 def act_scale(stats, scale, shift, M, C, stats2, scale2, shift2, res_sc, sc):
     import math
 
+    # split16.cu channel_bound: kappa u is the rounding of the conv16 epilogue's fp32 sums
+    ku = (16.0 + math.ceil(M / (16.0 * 132))) * 2.0 ** -24
+
     def grp(st, a, b):
-        mean = st[:C] / M
-        var = (st[C:] / M - mean * mean).clamp_min(0)
-        return float(((a.double() * mean + b.double()).abs() + a.double().abs() * torch.sqrt(M * var)).max())
+        mean, q = st[:C] / M, st[C:] / M
+        var = (q - mean * mean).clamp_min(0)
+        dev = torch.sqrt(M * (var + 4.0 * ku * q)) + ku * torch.sqrt(q)
+        return float(((a.double() * mean + b.double()).abs() + a.double().abs() * dev).max())
     bound = grp(stats, scale, shift)
     if stats2 is not None:
         bound += grp(stats2, scale2, shift2)
