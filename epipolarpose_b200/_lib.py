@@ -69,6 +69,7 @@ _PROTOS = {
     "epb_patch_joints": (c_int, [c_p, c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_int, c_p, c_p]),
     "epb_bn_finalize_scale": (c_int, [c_p, c_i64, c_int, c_p, c_p, c_f, c_f] + [c_p] * 12),
     "epb_softargmax_bwd_split": (c_int, [c_p] + [c_int] * 5 + [c_p] * 7),
+    "epb_softargmax_flip_fwd": (c_int, [c_p] + [c_int] * 5 + [ctypes.POINTER(c_int), c_int, c_p, c_p]),
     "epb_act_scale": (c_int, [c_p, c_p, c_p, c_i64, c_int, c_p, c_p, c_p, c_p, c_p, c_p]),
     "epb_bn_act_split": (c_int, [c_p] * 8 + [c_int, c_i64, c_int, c_p, c_p, c_p, c_p]),
     "epb_bn_relu_maxpool_split": (c_int, [c_p] * 6 + [c_int] * 4 + [c_p]),

@@ -210,7 +210,66 @@ __global__ void softargmax_fwd_nhwc(const float* __restrict__ logits, int J, int
   }
 }
 
+// ---------------------------------------------------------------- NHWC fwd, flip test
+// Same partition as softargmax_fwd_nhwc over the first N images of a [x; flip(x)] batch of 2N:
+// every thread averages its quad of image n with the mirrored pixel of image n+N in the paired
+// joint's channels (the flip-back of lib/utils/transforms.py:5-19, optionally shifted one column),
+// so the merged volume is never written.  pi: joint involution, J entries.
+constexpr int kFlipMaxJ = 1024;          // J*D/4 <= 1024 threads per pixel and D >= 4
+
+struct FlipPerm {
+  unsigned short p[kFlipMaxJ];
+};
+
+__global__ void softargmax_fwd_nhwc_flip(const float* __restrict__ logits, int N, int J, int D, int H,
+                                         int W, int S, int ppi, int shift, const FlipPerm pi,
+                                         Part* __restrict__ parts) {
+  extern __shared__ Part shp[];  // [blockDim]
+  __shared__ unsigned short sperm[kFlipMaxJ];
+  for (int j = threadIdx.x; j < J; j += blockDim.x) sperm[j] = pi.p[j];
+  __syncthreads();
+  const int n = blockIdx.y, sp = blockIdx.x;
+  const int C4 = (J * D) >> 2;
+  const int HW = H * W;
+  const int per = (HW + S - 1) / S;
+  const int pbeg = sp * per, pend = min(HW, pbeg + per);
+  const int c4 = threadIdx.x % C4, sub = threadIdx.x / C4;
+  const int D4 = D >> 2;
+  const int k4 = c4 % D4;
+  const int c4f = (int)sperm[c4 / D4] * D4 + k4;      // quad of the paired joint, same depth bins
+  const float z0 = (float)(k4 << 2);
+  const float4* base = reinterpret_cast<const float4*>(logits) + (int64_t)n * HW * C4 + c4;
+  const float4* fbase = reinterpret_cast<const float4*>(logits) + (int64_t)(n + N) * HW * C4 + c4f;
+
+  Part p;
+  part_init(p);
+  int pix = pbeg + sub;
+  int y = pix / W, x = pix - y * W;
+  for (; pix < pend; pix += ppi) {
+    // w' = W-1-w; with the shift column w reads the flip-back's column w-1 (column 0 keeps its own)
+    const int xf = shift ? (x == 0 ? W - 1 : W - x) : W - 1 - x;
+    const float4 a = ldg_stream(base + (int64_t)pix * C4);
+    const float4 b = ldg_stream(fbase + (int64_t)(y * W + xf) * C4);
+    const float4 v = make_float4(0.5f * (a.x + b.x), 0.5f * (a.y + b.y), 0.5f * (a.z + b.z),
+                                 0.5f * (a.w + b.w));
+    acc4_z(p, v, (float)x, (float)y, z0);
+    x += ppi;
+    while (x >= W) { x -= W; ++y; }
+  }
+  shp[threadIdx.x] = p;
+  __syncthreads();
+  if ((int)threadIdx.x < J) {
+    const int j = threadIdx.x;
+    Part q;
+    part_init(q);
+    for (int s2 = 0; s2 < ppi; ++s2)
+      for (int k = 0; k < D4; ++k) part_merge(q, shp[s2 * C4 + j * D4 + k]);
+    parts[((int64_t)n * J + j) * S + sp] = q;
+  }
+}
+
 // ---------------------------------------------------------------- finalize
+// lse may be null (the flip-test forward has no backward)
 __global__ void softargmax_finalize(const Part* __restrict__ parts, int NJ, int S, float invW,
                                     float invH, float invD, float* __restrict__ coords,
                                     float* __restrict__ lse) {
@@ -224,8 +283,10 @@ __global__ void softargmax_finalize(const Part* __restrict__ parts, int NJ, int 
   coords[nj * 3 + 0] = q.sx * inv * invW - 0.5f;
   coords[nj * 3 + 1] = q.sy * inv * invH - 0.5f;
   coords[nj * 3 + 2] = q.sz * inv * invD - 0.5f;
-  lse[nj * 2 + 0] = q.m;
-  lse[nj * 2 + 1] = inv;
+  if (lse) {
+    lse[nj * 2 + 0] = q.m;
+    lse[nj * 2 + 1] = inv;
+  }
 }
 
 // ---------------------------------------------------------------- backward
@@ -547,6 +608,48 @@ extern "C" __attribute__((visibility("default"))) int epb_softargmax_fwd(const f
   EPB_LAUNCH_CHECK();
   softargmax_finalize<<<(NJ + 127) / 128, 128, 0, st>>>(parts, NJ, S, 1.f / W, 1.f / H, 1.f / D,
                                                       coords, lse_ws);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_softargmax_flip_fwd(
+    const float* logits2N, int N, int J, int D, int H, int W, const int* perm_host, int shift,
+    float* coords, epb_stream_t stream) {
+  EPB_CHECK_ARG(logits2N && perm_host && coords);
+  EPB_CHECK_ARG(N > 0 && J > 0 && D > 0 && H > 0 && W > 0);
+  EPB_CHECK_ARG(shift == 0 || shift == 1);
+  EPB_CHECK_ARG(D % 4 == 0);
+  EPB_CHECK_ARG((int64_t)J * D / 4 <= 1024);
+  EPB_CHECK_ARG((reinterpret_cast<uintptr_t>(logits2N) & 15) == 0);
+  FlipPerm pi;
+  for (int j = 0; j < J; ++j) {
+    const int q = perm_host[j];
+    if (q < 0 || q >= J) {
+      epb_set_error("epb_softargmax_flip_fwd: perm[%d] = %d is outside [0, %d)", j, q, J);
+      return EPB_EINVAL;
+    }
+    if (perm_host[q] != j) {
+      epb_set_error("epb_softargmax_flip_fwd: perm is not an involution (perm[%d] = %d, perm[%d] = %d)",
+                    j, q, q, perm_host[q]);
+      return EPB_EINVAL;
+    }
+    pi.p[j] = (unsigned short)q;
+  }
+  cudaStream_t st = as_stream(stream);
+  const int NJ = N * J;
+  const int C4 = J * D / 4;
+  const int ppi = (512 / C4) > 0 ? (512 / C4) : 1;
+  int S = 1;
+  while (N * S < 8 * kNumSMs && (H * W) / (S * 2) >= 16 * ppi) S *= 2;
+  Part* parts = nullptr;
+  int rc = epb_workspace(EPB_WS_SOFTARGMAX, (size_t)NJ * S * sizeof(Part), st, (void**)&parts);
+  if (rc) return rc;
+  const int threads = C4 * ppi;
+  softargmax_fwd_nhwc_flip<<<dim3(S, N), threads, threads * sizeof(Part), st>>>(
+      logits2N, N, J, D, H, W, S, ppi, shift, pi, parts);
+  EPB_LAUNCH_CHECK();
+  softargmax_finalize<<<(NJ + 127) / 128, 128, 0, st>>>(parts, NJ, S, 1.f / W, 1.f / H, 1.f / D,
+                                                      coords, nullptr);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

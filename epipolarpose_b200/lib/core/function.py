@@ -1,7 +1,8 @@
 """Train / validate / evaluate loops -- host-side mirror of the reference
 lib/core/function.py signatures: train_integral(config, train_loader, model,
 criterion, optimizer, epoch) (:14-63), validate_integral(val_loader, model)
-(:66-110), eval_integral(epoch, preds, val_loader, path, debug) (:113-135).
+(:66-110; + the optional flip_test / shift_heatmap keywords), eval_integral(epoch,
+preds, val_loader, path, debug) (:113-135).
 
 Differences from the reference body (same observable behaviour):
   * the loss value is kept on the device and read back only when a log line
@@ -14,7 +15,11 @@ Differences from the reference body (same observable behaviour):
     cameras of each view pair are estimated from the predicted 2-D joints (no R, T or
     projection matrix needed: the reference's "without R/t" mode);
   * the gradient all-reduce for multi-GPU data parallelism happens inside the
-    model's backward (one NCCL call on the flat gradient buffer).
+    model's backward (one NCCL call on the flat gradient buffer);
+  * validate_integral honours TEST.FLIP_TEST and TEST.SHIFT_HEATMAP (reference
+    config.py:118,120, read nowhere by the reference): each batch is one forward of
+    [x; flip(x)] and the logits are merged with their flipped-back mirror before the
+    soft-argmax (integral_loss.get_joint_location_result_flip).
 """
 import logging
 import time
@@ -24,7 +29,7 @@ import torch
 
 from ..utils.img_utils import (self_supervision_device,
                                trans_coords_from_patch_to_org_3d_batch)
-from .integral_loss import get_result_func
+from .integral_loss import get_joint_location_coords_flip, get_result_func, joint_location_result_from_coords
 from ..utils.utils import AverageMeter
 
 logger = logging.getLogger(__name__)
@@ -324,8 +329,57 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
     return losses.avg
 
 
-def validate_integral(val_loader, model):
+def _flip_pairs(dataset):
+    pairs = getattr(dataset, 'flip_pairs', None)
+    if pairs is None:
+        db = getattr(dataset, 'db', None)
+        if db:
+            pairs = db[0].get('flip_pairs') if isinstance(db[0], dict) else None
+    return pairs
+
+
+def _validate_flip(val_loader, model, shift_heatmap):
+    """Flip-test validation: one forward of the 2B images [x; flip(x, 3)] per batch, merged
+    coordinates kept on the device, one copy to the host after the loop."""
+    net = getattr(model, 'module', model)
+    if not getattr(net, 'volume', True):
+        raise ValueError("flip test needs the VOLUME head (MODEL.VOLUME: true); the reference's "
+                         "result function has no flip merge for 2-D heat-maps")
+    pairs = _flip_pairs(val_loader.dataset)
+    if pairs is None:
+        raise ValueError("flip test needs the dataset's joint pairs: neither dataset.flip_pairs nor "
+                         "dataset.db[0]['flip_pairs'] exists")
+    dev = next(model.parameters()).device
+    model.eval()
+    chunks = []
+    with torch.no_grad():
+        for data in val_loader:
+            x = data[0]
+            B = x.shape[0]
+            buf = torch.empty((2 * B,) + tuple(x.shape[1:]), device=dev, dtype=torch.float32)
+            buf[:B].copy_(x, non_blocking=True)
+            buf[B:] = torch.flip(buf[:B], [3])
+            preds = model(buf)
+            chunks.append(get_joint_location_coords_flip(preds, pairs, shift_heatmap))
+            del preds, buf
+    if not chunks:
+        return np.zeros((0, 0, 4))
+    coords = torch.cat(chunks, dim=0).cpu().numpy()
+    out = joint_location_result_from_coords(256, 256, coords)     # hard-coded 256 as reference :87
+    return out[0:len(val_loader.dataset)]
+
+
+def validate_integral(val_loader, model, flip_test=None, shift_heatmap=None):
+    """flip_test / shift_heatmap default to config.TEST.FLIP_TEST / TEST.SHIFT_HEATMAP of the
+    module-global config (filled by update_config)."""
+    from .config import config
+    if flip_test is None:
+        flip_test = bool(config.TEST.FLIP_TEST)
+    if shift_heatmap is None:
+        shift_heatmap = bool(config.TEST.SHIFT_HEATMAP)
     print("Validation stage")
+    if flip_test:
+        return _validate_flip(val_loader, model, shift_heatmap)
     result_func = get_result_func()
     model.eval()
     chunks = []

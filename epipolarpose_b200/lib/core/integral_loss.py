@@ -8,7 +8,7 @@ Same names / arguments / error behaviour as the reference:
   reduce, norm), forward(preds, gt_joints, gt_joints_vis)),
   generate_joint_location_label / reverse_joint_location_label (:170-185),
   get_joint_location_result (:187-207), get_label_func / get_result_func /
-  merge_flip_func / get_merge_func (:209-220).
+  merge_flip_func / get_merge_func (:209-220; merge_flip_func stays the reference's no-op).
 Deviation (documented): L2JointLocationLoss in the reference is broken
 (self.output_3d undefined + stray print, :110-112); here it computes the
 weighted MSE it was evidently meant to.
@@ -21,6 +21,14 @@ SURVEY 8(d) C2(ii)): HeatmapMSELoss / HeatmapJointLoss / heatmap_joint_loss over
 launch epb_heatmap_joint_loss.  The reference ships no heat-map criterion (only the config
 remnants LOSS.USE_TARGET_WEIGHT, lib/core/config.py:32-34); the arithmetic is
 torch.nn.functional.mse_loss on the (weighted) maps.
+
+Addition for flip test (TEST.FLIP_TEST / TEST.SHIFT_HEATMAP, reference config.py:118,120, which the
+reference reads nowhere): get_joint_location_result_flip decodes the logits of the batch
+[x; flip(x)] as the soft-argmax of 0.5 * (L + flip_back(L_flipped)), flip_back on the volume viewed
+as [N, J, D*H, W] (transforms.py:5-19), shifted one column when shift_heatmap.  Channels_last
+logits with D % 4 == 0 and J*D/4 <= 1024 take one fused pass (epb_softargmax_flip_fwd) that never
+writes the merged volume; other layouts and shapes compose it with torch ops (about six passes over
+the volume) and decode it with epb_softargmax_fwd.
 """
 import numpy as np
 import torch
@@ -316,13 +324,83 @@ def get_joint_location_coords(preds):
 
 def get_joint_location_result(patch_width, patch_height, preds):
     """reference :187-207 -> numpy float64 [N, J, 4] (x, y, z in patch px, score 1)."""
-    coords = get_joint_location_coords(preds).detach().cpu().numpy().astype(float)
+    return joint_location_result_from_coords(patch_width, patch_height,
+                                             get_joint_location_coords(preds).detach().cpu().numpy())
+
+
+def joint_location_result_from_coords(patch_width, patch_height, coords):
+    """[N, J*3] normalised coordinates (host array) -> [N, J, 4] float64 as reference :196-205."""
+    coords = coords.astype(float)
     coords = coords.reshape((coords.shape[0], coords.shape[1] // 3, 3))
     coords[:, :, 0] = (coords[:, :, 0] + 0.5) * patch_width
     coords[:, :, 1] = (coords[:, :, 1] + 0.5) * patch_height
     coords[:, :, 2] = coords[:, :, 2] * patch_width
     scores = np.ones((coords.shape[0], coords.shape[1], 1), dtype=float)
     return np.concatenate((coords, scores), axis=2)
+
+
+def flip_permutation(flip_pairs, num_joints):
+    """The joint map of flip_back's pair swaps (transforms.py:13-16): perm[j] is the joint whose
+    flipped map lands on joint j.  ValueError for an index outside [0, J) or pairs that do not
+    make an involution (a joint in two pairs)."""
+    perm = list(range(num_joints))
+    for pair in flip_pairs:
+        a, b = int(pair[0]), int(pair[1])
+        if not (0 <= a < num_joints and 0 <= b < num_joints):
+            raise ValueError("flip pair (%d, %d) is outside [0, %d)" % (a, b, num_joints))
+        perm[a], perm[b] = perm[b], perm[a]
+    if any(perm[perm[j]] != j for j in range(num_joints)):
+        raise ValueError("flip pairs %r do not define an involution of the joints" % (list(flip_pairs),))
+    return perm
+
+
+def softmax_integral_flip(preds2N, num_joints, hm_width, hm_height, hm_depth, flip_pairs,
+                          shift_heatmap):
+    """preds2N [2N, J*D, H, W]: logits of [x; flip(x, 3)] -> merged coordinates [N, J*3] (no
+    gradient).  See the module docstring for the merge."""
+    J, D, H, W = num_joints, hm_depth, hm_height, hm_width
+    if preds2N.dtype != torch.float32:
+        raise TypeError("softmax_integral_flip expects float32 logits")
+    if preds2N.dim() != 4 or preds2N.shape[0] % 2 or tuple(preds2N.shape[1:]) != (J * D, H, W):
+        raise ValueError("expected logits [2N, %d, %d, %d], got %s" % (J * D, H, W, tuple(preds2N.shape)))
+    perm = flip_permutation(flip_pairs, J)
+    N = preds2N.shape[0] // 2
+    ops = _backend[0]
+    preds2N, layout = _layout_of(preds2N.detach(), J, D)
+    if layout == 1 and preds2N.data_ptr() % 16 == 0:
+        coords = torch.empty((N, J * 3), device=preds2N.device, dtype=torch.float32)
+        ops.softargmax_flip_fwd(_storage(preds2N, 1), N, J, D, H, W, perm, int(bool(shift_heatmap)), coords)
+        return coords
+    return flip_merge_torch(preds2N, J, D, H, W, perm, shift_heatmap)
+
+
+def flip_merge_torch(preds2N, J, D, H, W, perm, shift_heatmap):
+    """Any layout / shape: the merge as torch ops (flip-back copy, shift, average: about six
+    passes over the volume), then the ordinary soft-argmax of the merged volume."""
+    N = preds2N.shape[0] // 2
+    with torch.no_grad():
+        v = preds2N.reshape(2 * N, J, D, H, W)
+        fb = v[N:].flip(-1)[:, perm]
+        if shift_heatmap:
+            fb = torch.cat([fb[..., :1], fb[..., :-1]], dim=-1)
+        merged = (0.5 * (v[:N] + fb)).reshape(N, J * D, H, W).contiguous()
+        return softmax_integral_tensor(merged, J, True, W, H, D)
+
+
+def get_joint_location_coords_flip(preds2N, flip_pairs, shift_heatmap):
+    """Device-side half of get_joint_location_result_flip: [N, J*3] float32, D == W as :191-192."""
+    hm_width, hm_height = preds2N.shape[-1], preds2N.shape[-2]
+    hm_depth = hm_width
+    num_joints = preds2N.shape[1] // hm_depth
+    return softmax_integral_flip(preds2N, num_joints, hm_width, hm_height, hm_depth, flip_pairs,
+                                 shift_heatmap)
+
+
+def get_joint_location_result_flip(patch_width, patch_height, preds2N, flip_pairs, shift_heatmap):
+    """Flip-test form of get_joint_location_result: preds2N are the logits of [x; flip(x, 3)]
+    (2N images) -> numpy float64 [N, J, 4] of the merged logits."""
+    coords = get_joint_location_coords_flip(preds2N, flip_pairs, shift_heatmap)
+    return joint_location_result_from_coords(patch_width, patch_height, coords.cpu().numpy())
 
 
 def get_label_func():

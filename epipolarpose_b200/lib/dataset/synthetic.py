@@ -12,10 +12,17 @@ P = K.[R | -R.T].
 Sample order: index = tuple*NUM_CAMS + view.  `pair_batch_sampler` lays a
 batch out as [views 0 and 3 of each tuple | views 1 and 2] so that the
 first-half/second-half pairing of reference img_utils.py:194-199 triangulates
-(0,1) and (3,2), both legal neighbours in reference h36m.py:25."""
+(0,1) and (3,2), both legal neighbours in reference h36m.py:25.
+
+`flip_pairs` (read by the flip test of validate_integral): the MPII pairs for 16 joints, the
+H36M-17 pairs for 17 (reference prep_h36m.py:71,68), none for any other joint count."""
 import numpy as np
 import torch
 from torch.utils.data import Dataset
+
+
+MPII_FLIP_PAIRS = [[0, 5], [1, 4], [2, 3], [10, 15], [11, 14], [12, 13]]
+H36M_FLIP_PAIRS = [[1, 4], [2, 5], [3, 6], [14, 11], [15, 12], [16, 13]]
 
 
 def ring_camera(rng, view):
@@ -41,6 +48,7 @@ class SyntheticH36M(Dataset):
         self.is_train = is_train
         self.num_joints = cfg.MODEL.NUM_JOINTS
         self.num_cams = int(getattr(cfg.DATASET, 'NUM_CAMS', 4))
+        self.flip_pairs = {16: MPII_FLIP_PAIRS, 17: H36M_FLIP_PAIRS}.get(self.num_joints, [])
         self.patch_width, self.patch_height = int(cfg.MODEL.IMAGE_SIZE[0]), int(cfg.MODEL.IMAGE_SIZE[1])
         n_tuples = max(1, int(getattr(cfg.DATASET, 'SYNTHETIC_LEN', 256)) // self.num_cams)
         self.seed = 1000 * rank + (0 if is_train else 7)

@@ -14,7 +14,8 @@ do_augmentation (:28-39), fliplr_joints (:42-60) with the same names and return 
 (cv2.warpAffine), BGR->RGB, colour scale, clip and normalisation run in ONE kernel for the whole
 batch (epb_patch_sample, bit-exact against OpenCV) and the joints -> label half in
 epb_patch_joints; `generate_patch_batch_device` is the batched entry point a GPU data loader
-calls with already decoded frames.  The occluder paste (lib/utils/augmentation.py) is not built:
+calls with already decoded frames.  `flip(tensor, dims)` (:319-331) mirrors the input batch of the
+flip test.  The occluder paste (lib/utils/augmentation.py) is not built:
 `occluder` must be None."""
 import random
 
@@ -203,6 +204,14 @@ def trans_coords_from_patch_to_org_3d_batch(coords, c_x, c_y, bb_w, bb_h, patch_
 
 
 # ---------------------------------------------------------------------- input pipeline
+def flip(tensor, dims):
+    """reference :319-331: a copy of `tensor` reversed along `dims` (an int or a sequence), on the
+    tensor's device.  The reference's index meshgrid selects exactly what torch.flip returns."""
+    if not isinstance(dims, (tuple, list)):
+        dims = [dims]
+    return torch.flip(tensor, list(dims))
+
+
 def do_augmentation():
     """reference :28-39 (scale_factor 0.25, rot_factor 30, color_factor 0.2, rot_aug_rate 0.6,
     do_flip_aug False) -- the same draws from np.random / random in the same order."""

@@ -1,9 +1,21 @@
 """Centre/scale affine helpers used by get_final_preds -- mirror of the
-subset of reference lib/utils/transforms.py (:38-94) on the decode path.
+subset of reference lib/utils/transforms.py (:38-94) on the decode path, and
+flip_back (:5-19) of the flip test.
 The three-point affine that the reference obtains from cv2.getAffineTransform
 is solved directly in float64 numpy (tiny host-side arithmetic; image warps
 and flips belong to the data-loader, which is out of the hot path)."""
 import numpy as np
+
+
+def flip_back(output_flipped, matched_parts):
+    """reference :5-19: mirror a [batch, joints, height, width] array along width and swap each
+    left/right pair of joints, pairs in order.  Like the reference, the result is a reversed view
+    of the input and the swaps write through it."""
+    assert output_flipped.ndim == 4, 'flip_back expects [batch, joints, height, width]'
+    out = output_flipped[..., ::-1]
+    for a, b in matched_parts:
+        out[:, [a, b]] = out[:, [b, a]]          # the right-hand side is a copy
+    return out
 
 
 def _affine_from_points(src, dst):

@@ -17,7 +17,7 @@ launches = 0
 
 # kernels launched per C-ABI call (for the gpu_launches accounting)
 _KERNELS_PER_CALL = {
-    "epb_softargmax_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
+    "epb_softargmax_fwd": 2, "epb_softargmax_flip_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
     "epb_split16_batch": 3, "epb_split16": 3, "epb_bn_bwd_apply_split": 2, "epb_conv16_wgrad": 2,
     "epb_bn_bwd_reduce_mx": 2, "epb_bn_bwd_split": 3, "epb_softargmax_bwd_split": 3,
     "epb_patch_sample": 2, "epb_patch_sample_occ": 2,
@@ -293,6 +293,15 @@ def softargmax_fwd(logits, layout, N, J, D, H, W, coords, lse):
 def softargmax_bwd(logits, layout, N, J, D, H, W, coords, lse, dcoords, dlogits):
     _call("epb_softargmax_bwd", _p(logits), layout, N, J, D, H, W, _p(coords), _p(lse),
           _p(dcoords), _p(dlogits), _stream())
+
+
+def softargmax_flip_fwd(logits2N, N, J, D, H, W, perm, shift, coords):
+    """logits2N: channels_last storage [2N][H][W][J*D] of the batch [x; flip(x)]; perm: host
+    sequence of J joint indices (the flip pairs' involution)."""
+    if len(perm) != J:
+        raise _lib.EpbError("perm has %d entries, expected J = %d" % (len(perm), J))
+    pi = (ctypes.c_int * J)(*[int(v) for v in perm])
+    _call("epb_softargmax_flip_fwd", _p(logits2N), N, J, D, H, W, pi, int(shift), _p(coords), _stream())
 
 
 def jointloss(x, t, w, n, kind, norm, div, loss, dx):

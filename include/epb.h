@@ -335,6 +335,19 @@ int epb_softargmax_bwd(const float* logits, int layout, int N, int J, int D,
 int epb_softargmax_bwd_split(const float* logits, int N, int J, int D, int H, int W,
                              const float* coords, const float* lse_ws, const float* dcoords,
                              epb_half* dlogits16, float* sc, float* dbias, epb_stream_t stream);
+/* Flip test (lib/core/config.py:118,120 TEST.FLIP_TEST / TEST.SHIFT_HEATMAP): the soft-argmax of
+ * the logits merged with the flipped-back logits of the mirrored image, in one pass that never
+ * writes the merged volume.  logits2N: the network output of the batch [x; flip(x, 3)]
+ * (lib/utils/img_utils.py:319-331), layout 1 ([2N][H][W][J*D]).  For n < N:
+ *   merged[n][j*D+d][h][w] = 0.5 * (L[n][j*D+d][h][w] + L[n+N][pi(j)*D+d][h][w'])
+ * w' = W-1-w (flip_back, lib/utils/transforms.py:5-19, on the volume viewed as [N][J][D*H][W]);
+ * shift = 1: w' = W-w for w >= 1 and W-1 for w = 0 (flip_back followed by the one-column shift of
+ * TEST.SHIFT_HEATMAP).  coords [N][J*3] as epb_softargmax_fwd of merged (integral_loss.py:71-86).
+ * perm_host: the joint involution of the flip pairs (db['flip_pairs'], h36m.py:67), J entries;
+ * an entry outside [0, J) or a perm that is not an involution is EPB_EINVAL.  Needs D % 4 == 0,
+ * J*D/4 <= 1024 and a 16-byte aligned logits2N (EPB_EINVAL otherwise).  No lse, no backward. */
+int epb_softargmax_flip_fwd(const float* logits2N, int N, int J, int D, int H, int W,
+                            const int* perm_host, int shift, float* coords, epb_stream_t stream);
 
 /* Fused joint-location loss (integral_loss.py:7-47): kind 0 = weighted MSE,
  * 1 = weighted L1, 2 = weighted SmoothL1(beta=1).  loss = sum(w*l(x-t))/div,
