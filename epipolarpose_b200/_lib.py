@@ -8,6 +8,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("EPB_LIB_PATH") or os.path.join(HERE, "libepb.so")
 
 EPB_MAX_TAPS = 64
+EPB_JPEG_DESC_BYTES = 8192
+EPB_JPEG_PLAN_LEN = 10
+EPB_JPEG_EVENTS = 6
+EPB_JPEG_STATS = 7
 
 c_int, c_i64, c_f, c_d, c_p = (ctypes.c_int, ctypes.c_int64, ctypes.c_float,
                                ctypes.c_double, ctypes.c_void_p)
@@ -88,6 +92,8 @@ _PROTOS = {
     "epb_sgd_step": (c_int, [c_p, c_p, c_p, c_i64, c_f, c_f, c_f, c_int, c_int, c_f, c_p]),
     "epb_adam_step_dev": (c_int, [c_p, c_p, c_p, c_p, c_i64, c_p, c_p, c_p]),
     "epb_sgd_step_dev": (c_int, [c_p, c_p, c_p, c_i64, c_p, c_p, c_p]),
+    "epb_jpeg_parse": (c_int, [c_p, c_p, c_int, c_p, c_p, c_p, c_p, c_p]),
+    "epb_jpeg_decode": (c_int, [c_p, c_p, c_p, c_int, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
 }
 
 EXPORTS = tuple(_PROTOS)

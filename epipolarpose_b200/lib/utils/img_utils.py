@@ -14,7 +14,8 @@ do_augmentation (:28-39), fliplr_joints (:42-60) with the same names and return 
 (cv2.warpAffine), BGR->RGB, colour scale, clip and normalisation run in ONE kernel for the whole
 batch (epb_patch_sample, bit-exact against OpenCV) and the joints -> label half in
 epb_patch_joints; `generate_patch_batch_device` is the batched entry point a GPU data loader
-calls with already decoded frames.  `flip(tensor, dims)` (:319-331) mirrors the input batch of the
+calls with decoded frames (host arrays, or the device frames of `decode_jpeg_batch_device`, the JPEG decode of
+:251-252 on the GPU; `get_patch_batch_device` is the batched form of the whole sample).  `flip(tensor, dims)` (:319-331) mirrors the input batch of the
 flip test.  The occluder paste (lib/utils/augmentation.py) is not built:
 `occluder` must be None."""
 import random
@@ -234,29 +235,150 @@ def fliplr_joints(_joints, _joints_vis, width, matched_parts):
     return joints, joints_vis
 
 
+_IMREAD_FLAGS = 1 | 128                      # cv2.IMREAD_COLOR | cv2.IMREAD_IGNORE_ORIENTATION
+_JPEG_STATUS = {1: "unsupported", 2: "malformed"}
+
+
+class JpegFrames:
+    """B decoded BGR frames on the device in the layout epb_patch_sample reads: frame i is
+    base[offs[i]:] with (H, W, row pitch) = hwp[i]; sizes[i] = (H, W).  status[i] is the device
+    decoder's verdict (0 ok, 1 unsupported, 2 malformed; those frames came from cv2)."""
+
+    def __init__(self, base, offs, hwp, sizes, status):
+        self.base, self.offs, self.hwp, self.sizes, self.status = base, offs, hwp, sizes, status
+
+    def __len__(self):
+        return len(self.sizes)
+
+    def frame(self, i):
+        """Frame i as a uint8 [H, W, 3] device tensor (a view)."""
+        H, W = self.sizes[i]
+        o = int(self._offs_host[i])
+        return self.base[o:o + H * W * 3].view(H, W, 3)
+
+
+def _host_decode(buf, i, why):
+    """The reference's own decode (cv2.imread flags) of blob i, for what the device does not decode."""
+    try:
+        import cv2
+    except ImportError:
+        raise IOError("JPEG blob %d is %s and cv2 is not importable" % (i, why))
+    img = cv2.imdecode(buf, _IMREAD_FLAGS)
+    if not isinstance(img, np.ndarray):
+        raise IOError("Fail to read JPEG blob %d (%s)" % (i, why))
+    return img
+
+
+def _frame_offsets(hw):
+    offs, pos = [], 0
+    for H, W in hw:
+        offs.append(pos)
+        pos += (int(H) * int(W) * 3 + 15) // 16 * 16
+    return np.array(offs, dtype=np.int64), pos
+
+
+def decode_jpeg_batch_device(blobs, stats=None, events=None):
+    """B JPEG files (bytes or 1-D uint8 arrays) -> JpegFrames, decoded on the device bit-exact
+    against cv2.imread(IMREAD_COLOR | IMREAD_IGNORE_ORIENTATION).  One host->device copy carries the
+    compressed bytes and the parsed headers; one epb_jpeg_decode call decodes every image the
+    parser accepts.  Images the parser or the device reports as unsupported or malformed
+    (progressive, 4:1:1, CMYK, truncated, ...) are decoded with cv2.imdecode on the host and copied
+    into their slot; a blob cv2 cannot read either raises IOError naming its index.
+    stats / events: optional int32 [EPB_JPEG_STATS] device tensor and EPB_JPEG_EVENTS recorded
+    torch.cuda.Events (tools/bench_jpeg.py)."""
+    ops = _backend[0]
+    dev = _dev()
+    bufs = [np.frombuffer(b, dtype=np.uint8) if isinstance(b, (bytes, bytearray, memoryview))
+            else np.ascontiguousarray(np.asarray(b, dtype=np.uint8).reshape(-1)) for b in blobs]
+    B = len(bufs)
+    desc, status, hw, out_off, plan = ops.jpeg_parse(bufs)
+    host = {i: _host_decode(bufs[i], i, _JPEG_STATUS[int(s)]) for i, s in enumerate(status) if s != 0}
+    for i, img in host.items():
+        hw[i] = img.shape[:2]
+    out_off, out_bytes = _frame_offsets(hw)
+    hwp = np.stack([hw[:, 0], hw[:, 1], hw[:, 1] * 3], axis=1).astype(np.int32) if B else np.zeros((0, 3), np.int32)
+    # one pinned staging buffer -> one copy: blobs | descriptors | blob offsets | frame offsets | hwp | status
+    blob_off = np.zeros(B, dtype=np.int64)
+    pos = 0
+    for i, b in enumerate(bufs):
+        blob_off[i] = pos
+        pos += (b.size + 16 + 15) // 16 * 16
+    parts = [("desc", desc.reshape(-1)), ("blob_off", blob_off.view(np.uint8)), ("out_off", out_off.view(np.uint8)),
+             ("hwp", hwp.reshape(-1).view(np.uint8)), ("status", status.view(np.uint8))]
+    where, p = {}, pos
+    for name, a in parts:
+        where[name] = (p, a.size)
+        p = (p + a.size + 15) // 16 * 16
+    stage = torch.empty(max(p, 16), dtype=torch.uint8).pin_memory()
+    sn = stage.numpy()
+    for i, b in enumerate(bufs):
+        sn[blob_off[i]:blob_off[i] + b.size] = b
+    for name, a in parts:
+        sn[where[name][0]:where[name][0] + a.size] = a
+    d_stage = stage.to(dev, non_blocking=True)
+
+    def view(name, dtype):
+        o, n = where[name]
+        return d_stage[o:o + n].view(dtype)
+    d_off, d_hwp, d_status = view("out_off", torch.int64), view("hwp", torch.int32), view("status", torch.int32)
+    out = torch.empty(max(out_bytes, 16), dtype=torch.uint8, device=dev)
+    if int(plan[7]):
+        ws = torch.empty(int(plan[0]), dtype=torch.uint8, device=dev)
+        ops.jpeg_decode(d_stage, view("blob_off", torch.int64), view("desc", torch.uint8), B, plan, ws, out,
+                        d_off, d_hwp, d_status, stats, events)
+    dev_status = d_status.cpu().numpy()
+    for i, s in enumerate(dev_status):
+        if s != 0 and i not in host:
+            img = _host_decode(bufs[i], i, _JPEG_STATUS[int(s)])
+            if img.shape[:2] != tuple(hw[i]):
+                raise IOError("JPEG blob %d: cv2 decodes %s, the header says %s" % (i, img.shape[:2], tuple(hw[i])))
+            host[i] = img
+    for i, img in host.items():
+        out[int(out_off[i]):int(out_off[i]) + img.size].copy_(torch.from_numpy(img.reshape(-1)))
+    frames = JpegFrames(out, d_off, d_hwp, [(int(h), int(w)) for h, w in hw], dev_status)
+    frames._offs_host = out_off
+    return frames
+
+
+def read_jpeg_batch_device(paths):
+    """decode_jpeg_batch_device of the files at `paths`."""
+    blobs = []
+    for p in paths:
+        with open(p, "rb") as f:
+            blobs.append(f.read())
+    return decode_jpeg_batch_device(blobs)
+
+
 def generate_patch_batch_device(images, center_x, center_y, width, height, patch_width, patch_height,
                                 scale=None, rot=None, do_flip=None, color_scale=None, mean=None, std=None,
                                 occluders=None):
-    """B decoded BGR frames (uint8 [H,W,3] numpy arrays or tensors, sizes may differ) ->
+    """B decoded BGR frames (uint8 [H,W,3] numpy arrays or tensors, sizes may differ, or the
+    JpegFrames of decode_jpeg_batch_device, read where they are) ->
     (patches float32 [B,3,ph,pw] on the device, trans float64 [B,2,3], box float64 [B,6]).
     occluders: per sample a list of (rgba uint8 [h,w,4], (cx, cy)) pasted onto the uint8 patch
     in order (augmentation.draw_occluders), or None."""
     ops = _backend[0]
     dev = _dev()
     B = len(images)
-    offs, hwp, chunks, pos = [], [], [], 0
-    for im in images:
-        t = im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im))
-        if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
-            raise ValueError("frames must be uint8 [H, W, 3] (cv2.imread layout)")
-        t = t.contiguous()
-        offs.append(pos)
-        hwp.append([t.shape[0], t.shape[1], t.shape[1] * 3])
-        chunks.append(t.reshape(-1))
-        pos += (t.numel() + 15) // 16 * 16
-    base = torch.zeros(max(pos, 16), dtype=torch.uint8)
-    for o, c in zip(offs, chunks):
-        base[o:o + c.numel()] = c.cpu()
+    if isinstance(images, JpegFrames):          # decoded on the device: no host round trip
+        d_base, d_offs, d_hwp = images.base, images.offs, images.hwp
+    else:
+        offs, hwp, chunks, pos = [], [], [], 0
+        for im in images:
+            t = im if isinstance(im, torch.Tensor) else torch.from_numpy(np.ascontiguousarray(im))
+            if t.dtype != torch.uint8 or t.dim() != 3 or t.shape[2] != 3:
+                raise ValueError("frames must be uint8 [H, W, 3] (cv2.imread layout)")
+            t = t.contiguous()
+            offs.append(pos)
+            hwp.append([t.shape[0], t.shape[1], t.shape[1] * 3])
+            chunks.append(t.reshape(-1))
+            pos += (t.numel() + 15) // 16 * 16
+        base = torch.zeros(max(pos, 16), dtype=torch.uint8)
+        for o, c in zip(offs, chunks):
+            base[o:o + c.numel()] = c.cpu()
+        d_base = base.to(dev)
+        d_offs = torch.tensor(offs, dtype=torch.int64, device=dev)
+        d_hwp = torch.tensor(hwp, dtype=torch.int32, device=dev)
     ones, zeros = np.ones(B), np.zeros(B)
     box = np.stack([np.asarray(center_x, dtype=np.float64).reshape(B), np.asarray(center_y, dtype=np.float64).reshape(B),
                     np.asarray(width, dtype=np.float64).reshape(B), np.asarray(height, dtype=np.float64).reshape(B),
@@ -274,12 +396,10 @@ def generate_patch_batch_device(images, center_x, center_y, width, height, patch
     if occluders is not None:
         from .augmentation import pack_occluders
         ob, od, oc = pack_occluders(occluders, dev)
-        ops.patch_sample_occ(base.to(dev), torch.tensor(offs, dtype=torch.int64, device=dev),
-                             torch.tensor(hwp, dtype=torch.int32, device=dev), t_box, t_flip, t_col, ms,
+        ops.patch_sample_occ(d_base, d_offs, d_hwp, t_box, t_flip, t_col, ms,
                              B, int(patch_width), int(patch_height), ob, od, oc, out, trans)
     else:
-        ops.patch_sample(base.to(dev), torch.tensor(offs, dtype=torch.int64, device=dev),
-                         torch.tensor(hwp, dtype=torch.int32, device=dev), t_box, t_flip, t_col, ms, B,
+        ops.patch_sample(d_base, d_offs, d_hwp, t_box, t_flip, t_col, ms, B,
                          int(patch_width), int(patch_height), out, trans)
     return out, trans.reshape(B, 2, 3), t_box
 
@@ -341,3 +461,65 @@ def get_single_patch_sample(img_path, center_x, center_y, width, height,
             joints[n_jt, 2] = joints[n_jt, 2] / den * patch_width
         label, label_weight = label_func(patch_width, patch_height, joints, joints_vis)
     return patches[0].cpu().numpy(), label, label_weight, scale, rot
+
+
+def get_patch_batch_device(img_paths, center_x, center_y, width, height, joints, joints_vis, flip_pairs,
+                           parent_ids, patch_width, patch_height, rect_3d_width, rect_3d_height, mean, std,
+                           do_augment, label_func, depth_in_image=False, occluder=None):
+    """Batched, device-decoded get_single_patch_sample: B image files (or JPEG blobs) and per-sample
+    boxes / joints [B,J,3] / joints_vis [B,J,3] -> (patches float32 [B,3,ph,pw] on the device, label
+    [B,...], label_weight [B,...], scale [B], rot [B]) -- the stack of B sequential
+    get_single_patch_sample calls, with the same np.random / random draws in the same order
+    (do_augmentation(), then draw_occluders, per sample)."""
+    B = len(img_paths)
+    blobs = []
+    for p in img_paths:
+        if isinstance(p, (bytes, bytearray, memoryview, np.ndarray)):
+            blobs.append(p)
+        else:
+            with open(p, "rb") as f:
+                blobs.append(f.read())
+    frames = decode_jpeg_batch_device(blobs)
+    aug, occ = [], [] if occluder else None
+    for _ in range(B):
+        aug.append(do_augmentation() if do_augment else (1.0, 0, False, [1.0, 1.0, 1.0]))
+        if occluder:
+            from .augmentation import draw_occluders
+            occ.append(draw_occluders(int(patch_width), int(patch_height), occluder))
+    scale = np.array([a[0] for a in aug], dtype=np.float64)
+    rot = np.array([a[1] for a in aug], dtype=np.float64)
+    do_flip = [a[2] for a in aug]
+    cx = np.asarray(center_x, dtype=np.float64).reshape(B)
+    cy = np.asarray(center_y, dtype=np.float64).reshape(B)
+    bw = np.asarray(width, dtype=np.float64).reshape(B)
+    bh = np.asarray(height, dtype=np.float64).reshape(B)
+    patches, trans, box = generate_patch_batch_device(frames, cx, cy, bw, bh, patch_width, patch_height, scale, rot,
+                                                      do_flip, [a[3] for a in aug], mean, std, occluders=occ)
+    jts, vis = [], []
+    for i in range(B):
+        j = np.array(joints[i], dtype=np.float64, copy=True)
+        v = np.array(joints_vis[i], copy=True)
+        if do_flip[i]:
+            j, v = fliplr_joints(j, v, frames.sizes[i][1], flip_pairs)
+        jts.append(j)
+        vis.append(v)
+    from ..core.integral_loss import generate_joint_location_label
+    if label_func is None or label_func is generate_joint_location_label or \
+            getattr(label_func, "__name__", "") == "generate_joint_location_label":
+        label = patch_labels_device(np.stack(jts), box, trans, patch_width, patch_height, rect_3d_width,
+                                    depth_in_image).cpu().numpy()
+        label_weight = np.stack([v.reshape(-1) for v in vis])
+    else:
+        tr = trans.cpu().numpy()
+        labels, weights = [], []
+        for i in range(B):
+            j = jts[i]
+            for n_jt in range(len(j)):
+                j[n_jt, 0:2] = np.dot(tr[i], np.array([j[n_jt, 0], j[n_jt, 1], 1.]).T)[0:2]
+                den = (bw[i] * scale[i]) if depth_in_image else (rect_3d_width * scale[i])
+                j[n_jt, 2] = j[n_jt, 2] / den * patch_width
+            lab, w = label_func(patch_width, patch_height, j, vis[i])
+            labels.append(lab)
+            weights.append(w)
+        label, label_weight = np.stack(labels), np.stack(weights)
+    return patches, label, label_weight, scale, rot

@@ -20,7 +20,7 @@ _KERNELS_PER_CALL = {
     "epb_softargmax_fwd": 2, "epb_softargmax_flip_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
     "epb_split16_batch": 3, "epb_split16": 3, "epb_bn_bwd_apply_split": 2, "epb_conv16_wgrad": 2,
     "epb_bn_bwd_reduce_mx": 2, "epb_bn_bwd_split": 3, "epb_softargmax_bwd_split": 3,
-    "epb_patch_sample": 2, "epb_patch_sample_occ": 2,
+    "epb_patch_sample": 2, "epb_patch_sample_occ": 2, "epb_jpeg_decode": 14,
 }
 
 
@@ -370,6 +370,37 @@ def patch_sample_occ(img_base, img_off, img_hwp, box, flip, color, mean_std, B, 
           _p(img_hwp, torch.int32), _p(box, torch.float64), _p(flip, torch.int32), _p(color), ms, B,
           patch_w, patch_h, _p(occ_base, torch.uint8), _p(occ_desc, torch.int64),
           _p(occ_count, torch.int32), _p(out), _p(trans, torch.float64), _stream())
+
+
+def jpeg_parse(blobs):
+    """blobs: B contiguous uint8 numpy arrays (host) -> (desc uint8 [B, EPB_JPEG_DESC_BYTES], status int32
+    [B], hw int32 [B, 2], out_off int64 [B], plan int64 [EPB_JPEG_PLAN_LEN]), all numpy (host)."""
+    import numpy as np
+    B = len(blobs)
+    ptrs = (ctypes.c_void_p * max(B, 1))(*[b.ctypes.data for b in blobs])
+    lens = np.array([b.size for b in blobs] or [0], dtype=np.int64)
+    desc = np.zeros((max(B, 1), _lib.EPB_JPEG_DESC_BYTES), dtype=np.uint8)
+    status = np.zeros(max(B, 1), dtype=np.int32)
+    hw = np.zeros((max(B, 1), 2), dtype=np.int32)
+    out_off = np.zeros(max(B, 1), dtype=np.int64)
+    plan = np.zeros(_lib.EPB_JPEG_PLAN_LEN, dtype=np.int64)
+    _lib.call("epb_jpeg_parse", ptrs, lens.ctypes.data, B, desc.ctypes.data, status.ctypes.data, hw.ctypes.data,
+              out_off.ctypes.data, plan.ctypes.data)
+    return desc[:B], status[:B], hw[:B], out_off[:B], plan
+
+
+def jpeg_decode(blob_base, blob_off, desc, B, plan, ws, out_base, out_off, out_hwp, status, stats=None,
+                events=None):
+    """plan: the host int64 array of jpeg_parse; events: None or EPB_JPEG_EVENTS torch.cuda.Event
+    (enable_timing) recorded between the stages."""
+    import numpy as np
+    plan = np.ascontiguousarray(plan, dtype=np.int64)
+    ev = None
+    if events is not None:
+        ev = (ctypes.c_void_p * len(events))(*[e.cuda_event for e in events])
+    _call("epb_jpeg_decode", _p(blob_base, torch.uint8), _p(blob_off, torch.int64), _p(desc, torch.uint8), B,
+          plan.ctypes.data, _p(ws, torch.uint8), ws.numel(), _p(out_base, torch.uint8), _p(out_off, torch.int64),
+          _p(out_hwp, torch.int32), _p(status, torch.int32), _p(stats, torch.int32), ev, _stream())
 
 
 def patch_joints(joints, box, trans, B, J, patch_w, patch_h, rect_3d_w, depth_in_image, label):

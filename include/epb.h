@@ -514,6 +514,35 @@ int epb_patch_joints(const double* joints, const double* box, const double* tran
                      double* label, epb_stream_t stream);
 
 /* ------------------------------------------------------------------------
+ * JPEG decode (the cv2.imread(path, IMREAD_COLOR | IMREAD_IGNORE_ORIENTATION) call site of
+ * lib/utils/img_utils.py:251-252), bit-exact against libjpeg-turbo: baseline / extended
+ * sequential Huffman, 8-bit, 1 component or YCbCr 4:4:4 / 4:2:2 / 4:4:0 / 4:2:0, one
+ * interleaved scan, restart intervals.  Anything else is reported per image, never guessed.
+ * ---------------------------------------------------------------------- */
+#define EPB_JPEG_OK 0
+#define EPB_JPEG_UNSUPPORTED 1   /* progressive, arithmetic, 12-bit, 4:1:1, CMYK / RGB, ...    */
+#define EPB_JPEG_MALFORMED 2     /* bad header data, or entropy data that ends before the last MCU */
+#define EPB_JPEG_DESC_BYTES 8192 /* one descriptor per image                                  */
+#define EPB_JPEG_PLAN_LEN 10
+#define EPB_JPEG_EVENTS 6        /* stage marks: start, unstuff, phase A, phase B+C, IDCT, colour */
+#define EPB_JPEG_STATS 7         /* [r] != 0: phase-A round r changed a state; [6]: sequential walk ran */
+/* Host only: parses each blob up to SOS.  desc_host [B][EPB_JPEG_DESC_BYTES] (the device copy is
+ * what epb_jpeg_decode reads), status_host [B], hw_host [B][2] = (H, W) (0 when unknown),
+ * out_off_host [B]: 16-byte aligned byte offsets of each H*W*3 frame in the output buffer,
+ * plan_host [EPB_JPEG_PLAN_LEN]: [0] workspace bytes, [1] output bytes, [2..9] launch bounds. */
+int epb_jpeg_parse(const uint8_t* const* blobs_host, const int64_t* lens_host, int B, void* desc_host,
+                   int32_t* status_host, int32_t* hw_host, int64_t* out_off_host, int64_t* plan_host);
+/* Decodes every image whose parse status is OK into out_base + out_off[b] (uint8 BGR, row pitch
+ * out_hwp[b][2] bytes; the layout epb_patch_sample reads) and sets status[b] to OK or MALFORMED;
+ * other images and their status entries are left untouched.  blob_base + blob_off[b]: the blobs;
+ * desc: the parsed descriptors; ws: ws_bytes >= plan_host[0] of scratch.  stats [EPB_JPEG_STATS]
+ * int32 or NULL; events_host: EPB_JPEG_EVENTS cudaEvent_t recorded between stages, or NULL. */
+int epb_jpeg_decode(const uint8_t* blob_base, const int64_t* blob_off, const void* desc, int B,
+                    const int64_t* plan_host, void* ws, int64_t ws_bytes, uint8_t* out_base,
+                    const int64_t* out_off, const int32_t* out_hwp, int32_t* status, int32_t* stats,
+                    void* const* events_host, epb_stream_t stream);
+
+/* ------------------------------------------------------------------------
  * Optimiser (torch.optim.Adam call site lib/utils/utils.py:56-60; betas
  * (0.9,0.999), eps 1e-8, no weight decay) over one flat parameter buffer.
  * step is the 1-based step count.  grad_scale multiplies the gradient first
