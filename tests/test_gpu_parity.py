@@ -696,6 +696,9 @@ def test_network_gradients_vs_oracle_fp64(dev, layers, precision):
 
 
 def test_fused_adam_matches_torch(dev):
+    """Per-tensor path (gradients not flat): each step's UPDATE p1 - p0 against torch.optim.Adam's
+    from the same parameters, within 1e-4 of max|update| (fp32 betas in the kernel: ~1.3e-5
+    relative on 1 - beta2; the final rounding of p: 2^-24 |p| / |update| ~ 1e-5 here)."""
     import lib.utils.utils as U
     torch.manual_seed(0)
     ps = [torch.nn.Parameter(torch.randn(s, device=dev)) for s in ((7, 3), (64,), (5, 5, 3))]
@@ -705,9 +708,13 @@ def test_fused_adam_matches_torch(dev):
         for p, q in zip(ps, qs):
             g = torch.randn_like(p)
             p.grad, q.grad = g.clone(), g.clone()
+            q.data.copy_(p.data)                 # same start every step: compare one update
+        p0 = [p.detach().clone() for p in ps]
         a.step(); b.step()
-    for p, q in zip(ps, qs):
-        assert relerr(p.detach().cpu().numpy(), q.detach().cpu().numpy()) <= 1e-5
+        for p, q, s in zip(ps, qs, p0):
+            du = (p.detach() - s).double().cpu().numpy()
+            dt = (q.detach() - s).double().cpu().numpy()
+            assert relerr(du, dt) <= 1e-4, (it, relerr(du, dt))
 
 
 def test_graphed_train_step_matches_eager(dev):
