@@ -82,6 +82,10 @@ _PROTOS = {
     "epb_split16_batch": (c_int, [c_p, c_int, ctypes.c_longlong, c_p, c_p]),
     "epb_conv16_fprop": (c_int, [ctypes.POINTER(ConvGeom)] + [c_p] * 8),
     "epb_conv16_wgrad": (c_int, [ctypes.POINTER(ConvGeom)] + [c_p] * 6 + [ctypes.c_longlong, c_p]),
+    "epb_conv16_fprop_splitk": (c_int, [ctypes.POINTER(ConvGeom)] + [c_p] * 7 + [c_int, c_p, ctypes.c_longlong,
+                                                                               c_p]),
+    "epb_conv16_splits": (c_int, [ctypes.POINTER(ConvGeom), ctypes.POINTER(c_int),
+                                  ctypes.POINTER(ctypes.c_longlong)]),
     "epb_bn_bwd_reduce_mx": (c_int, [c_p] * 7 + [c_int, c_i64, c_int, c_p, c_p, c_p]),
     "epb_bn_bwd_apply_split": (c_int, [c_p] * 8 + [c_int, c_p, c_p, c_i64, c_int] + [c_p] * 6),
     "epb_bn_bwd_split": (c_int, [c_p] * 9 + [c_int, c_i64, c_int] + [c_p] * 6),

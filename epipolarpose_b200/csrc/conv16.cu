@@ -22,6 +22,13 @@
 // MMAs.  The store map has the extents of the output view: TMA drops the rows and columns
 // beyond it.  The BatchNorm statistics of a run of tiles of one N tile are kept in the
 // per-warp slices from the register values, flushed once per run.
+//
+// Split-K (epb_conv16_fprop_splitk): a layer with few tiles leaves most SMs idle while each CTA
+// walks the whole K loop.  The work items are then (tile, split) pairs, split s covering the
+// contiguous k-blocks [s KB / S, (s + 1) KB / S); the same kernel (SPLIT = true) stores each
+// item's scaled accumulator into a dense fp32 workspace [S][tiles * 128][Cout] through the same
+// staging boxes, and conv16_splitk_reduce sums the splits in the order 0..S-1, adds the bias,
+// writes the output view and adds the statistics of its valid rows.
 #include "split16_common.cuh"
 
 namespace {
@@ -40,13 +47,15 @@ struct Plan16 {
   int n_tiles;
   int accumulate;
   int m_fastest;                 // tile order: consecutive tiles walk M (statistics runs) or N
+  int splits;                    // K splits per tile (SPLIT kernel only)
   int koff[EPB_MAX_TAPS];        // wt[t] * Cin: k offset of the tap inside a packed weight row
 };
 
 struct Maps16 {
   CUtensorMap a[4];
   CUtensorMap w;
-  CUtensorMap out;               // fp32 (Cout, Wv, Hv, N) output view, box 32 x one warp's 16 rows
+  CUtensorMap out;               // fp32 (Cout, Wv, Hv, N) output view, box 32 x one warp's 16 rows;
+                                 // SPLIT: the (Cout, 16, tiles * 8, S) workspace, box 32 x 16 x 1 x 1
 };
 
 template <int BN>
@@ -66,7 +75,7 @@ struct Cfg16 {
   static_assert(S >= 2, "ring too shallow");
 };
 
-template <int BN>
+template <int BN, bool SPLIT>
 __global__ void __launch_bounds__(kThreads16, 1)
 conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 maps,
               const float* __restrict__ in_sc, const float* __restrict__ w_sc,
@@ -82,6 +91,10 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int KB = P.T * P.CB;
   const int total_tiles = G.tiles * P.n_tiles;
+  const int items = SPLIT ? total_tiles * P.splits : total_tiles;
+  // work item -> (tile, split); split s runs k-blocks [kb_lo(s), kb_lo(s + 1))
+  auto tile_of = [&](int item) { return SPLIT ? item % total_tiles : item; };
+  auto kb_lo = [&](int s) { return SPLIT ? (int)((int64_t)s * KB / P.splits) : (s ? KB : 0); };
   auto nt_of = [&](int tile) { return P.m_fastest ? tile / G.tiles : tile % P.n_tiles; };
   auto mt_of = [&](int tile) { return P.m_fastest ? tile % G.tiles : tile / P.n_tiles; };
 
@@ -94,12 +107,14 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
       for (int v = 0; v < 4; ++v) tc::tma_prefetch_desc(&maps.a[v]);
       tc::tma_prefetch_desc(&maps.w);
       tc::tma_prefetch_desc(&maps.out);
-      for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+      for (int item = blockIdx.x; item < items; item += gridDim.x) {
+        const int tile = tile_of(item), s = SPLIT ? item / total_tiles : 0;
         const int nt = nt_of(tile);
         int w0, h0, n0;
         G.tile_origin(mt_of(tile), w0, h0, n0);
-        int t = 0, cb = 0;
-        for (int kb = 0; kb < KB; ++kb) {
+        const int kb0 = kb_lo(s), kb1 = kb_lo(s + 1);
+        int t = kb0 / P.CB, cb = kb0 % P.CB;
+        for (int kb = kb0; kb < kb1; ++kb) {
           tc::mbar_wait(ring.empty(ring.stage), ring.phase ^ 1);
           const uint32_t fb = ring.full(ring.stage);
           tc::mbar_arrive_expect_tx(fb, C::STAGE);
@@ -142,7 +157,8 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
 
   float acc[BN / 2];
   int nt_prev = -1;
-  for (int tile = blockIdx.x; tile < total_tiles; tile += gridDim.x) {
+  for (int item = blockIdx.x; item < items; item += gridDim.x) {
+    const int tile = tile_of(item), s = SPLIT ? item / total_tiles : 0;
     const int nt = nt_of(tile);
     // statistics: one flush per run of tiles of the same N tile
     if (stats && nt_prev >= 0 && nt != nt_prev)
@@ -150,7 +166,7 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
     nt_prev = nt;
 #pragma unroll
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
-    for (int kb = 0; kb < KB; ++kb)
+    for (int kb = kb_lo(s), kb1 = kb_lo(s + 1); kb < kb1; ++kb)
       ring.consume(acc, [&](uint32_t st) {
         const uint32_t a_hi = st + wgc * 64 * 128, b_hi = st + C::A_BYTES;
 #pragma unroll
@@ -175,7 +191,7 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
     // the warp's rows are the (bw, bh, bn) sub-box of the tile box at (bx, by, bz), bw * bh *
     // bn = 16 (tile extents are powers of two); a band that starts past the view is all past it
     const int bx = w0 + rb % G.tw, by = h0 + (rb / G.tw) % G.th, bz = n0 + rb / twh;
-    const bool band = bx < P.Wv && by < P.Hv && bz < G.N;
+    const bool band = SPLIT || (bx < P.Wv && by < P.Hv && bz < G.N);
 #pragma unroll
     for (int q = 0; q < BN / 32; ++q) {
       // the previous store has finished reading the box
@@ -203,7 +219,8 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
         // With `accumulate` the add of the old value happens in the L2: one fp32 add, round to
         // nearest even, as old + new in registers.  A subnormal old value is kept, not flushed
         // (tests/test_gpu_conv16_store.py checks both against numpy's fp32 sum).
-        if (P.accumulate) tc::tma_reduce_add_4d(&maps.out, box_addr, c0, bx, by, bz);
+        if constexpr (SPLIT) tc::tma_store_4d(&maps.out, box_addr, c0, 0, (mt_of(tile) * BM + rb) / 16, s);
+        else if (P.accumulate) tc::tma_reduce_add_4d(&maps.out, box_addr, c0, bx, by, bz);
         else tc::tma_store_4d(&maps.out, box_addr, c0, bx, by, bz);
         tc::tma_store_commit();
       }
@@ -218,11 +235,90 @@ conv16_kernel(const __grid_constant__ Plan16 P, const __grid_constant__ Maps16 m
   if (lane == 0) tc::tma_store_wait<0>();   // the output is written before the CTA retires
 }
 
-}  // namespace
+// Split-K second pass: out = bias + sum over s = 0..S-1 (in that order) of the workspace
+// partials, for the pixels of the phase grid that lie in the output view, and the per-channel
+// sum / sum of squares of every pixel of the phase grid (the rows the fused epilogue counts)
+// added to `stats`.  Threads: 32 column quads x 8 rows; the rows of a column block are summed
+// in double per thread, then over the 8 row lanes in a fixed order, one atomic per channel.
+struct Reduce16 {
+  epb_phase_grid grid;
+  int Cout, Wv, Hv, splits;
+  int64_t sw, sh, sn;            // element strides of w, h, n in the output phase view
+};
 
-extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
-    const epb_conv_geom* g, const epb_half* in, const float* in_sc, const epb_half* w,
-    const float* w_sc, const float* bias, float* out, double* stats, epb_stream_t stream) {
+__global__ void __launch_bounds__(256)
+conv16_splitk_reduce(const __grid_constant__ Reduce16 R, const float* __restrict__ ws,
+                     const float* __restrict__ bias, float* __restrict__ out,
+                     double* __restrict__ stats) {
+  __shared__ double red[2][8][128];
+  const epb_phase_grid& G = R.grid;
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int c = (blockIdx.x * 32 + tx) * 4;
+  const bool cok = c < R.Cout;
+  const int64_t M = (int64_t)G.N * G.Hp * G.Wp;
+  const int64_t split_stride = (int64_t)G.tiles * BM * R.Cout;
+  float b[4] = {0.f, 0.f, 0.f, 0.f};
+  if (bias && cok)
+    for (int e = 0; e < 4; ++e) b[e] = bias[c + e];
+  double s1[4] = {0.0, 0.0, 0.0, 0.0}, s2[4] = {0.0, 0.0, 0.0, 0.0};
+  if (cok) {
+    for (int64_t m = (int64_t)blockIdx.y * 8 + ty; m < M; m += (int64_t)gridDim.y * 8) {
+      const int w = (int)(m % G.Wp);
+      const int64_t q = m / G.Wp;
+      const int h = (int)(q % G.Hp), n = (int)(q / G.Hp);
+      // tile and tile row of pixel (w, h, n): the inverse of tile_origin and the epilogue's rows
+      const int mt = w / G.tw + G.tiles_w * (h / G.th + G.tiles_h * (n / G.tn));
+      const int r = w % G.tw + G.tw * (h % G.th + G.th * (n % G.tn));
+      const float* src = ws + ((int64_t)mt * BM + r) * R.Cout + c;
+      float4 v = *reinterpret_cast<const float4*>(src);
+      for (int s = 1; s < R.splits; ++s) {
+        const float4 u = *reinterpret_cast<const float4*>(src + s * split_stride);
+        v.x += u.x; v.y += u.y; v.z += u.z; v.w += u.w;
+      }
+      v.x += b[0]; v.y += b[1]; v.z += b[2]; v.w += b[3];
+      if (w < R.Wv && h < R.Hv)
+        *reinterpret_cast<float4*>(out + n * R.sn + h * R.sh + w * R.sw + c) = v;
+      const float a[4] = {v.x, v.y, v.z, v.w};
+      for (int e = 0; e < 4; ++e) {
+        s1[e] += a[e];
+        s2[e] += (double)a[e] * a[e];
+      }
+    }
+  }
+  if (!stats) return;
+  for (int e = 0; e < 4; ++e) {
+    red[0][ty][tx * 4 + e] = s1[e];
+    red[1][ty][tx * 4 + e] = s2[e];
+  }
+  __syncthreads();
+  if (ty == 0 && cok)
+    for (int e = 0; e < 4; ++e) {
+      double t1 = 0.0, t2 = 0.0;
+      for (int y = 0; y < 8; ++y) {
+        t1 += red[0][y][tx * 4 + e];
+        t2 += red[1][y][tx * 4 + e];
+      }
+      atomicAdd(stats + c + e, t1);
+      atomicAdd(stats + R.Cout + c + e, t2);
+    }
+}
+
+// N tile: the 128-column accumulator of a consumer warpgroup (64 fp32 registers per thread),
+// 64 columns for narrow layers
+inline int conv16_bn(int Cout) { return Cout <= 64 ? 64 : 128; }
+
+// Shortest K range of a split (k-blocks of 64): a work item also pays the pipeline fill, the
+// epilogue and the partial's round trip through the workspace.  Two or three splits save at most
+// two thirds of the K loop, which pays for the partials and the reduce only when every split is
+// still kSplitLongKB k-blocks long (H100 per-layer table, tools/bench_infer.py, DESIGN.md 5).
+constexpr int kSplitMinKB = 4;
+constexpr int kSplitLongKB = 16;
+
+// One conv16 call: splits == 1 is the fused kernel writing `out`; splits > 1 the SPLIT kernel
+// into `ws` (checked by the caller) followed by conv16_splitk_reduce.
+int conv16_run(const epb_conv_geom* g, const epb_half* in, const float* in_sc, const epb_half* w,
+               const float* w_sc, const float* bias, float* out, double* stats, int splits,
+               float* ws, epb_stream_t stream) {
   int rc = epb_conv_geom_check(g);
   if (rc) return rc;
   EPB_CHECK_ARG(in && in_sc && w && w_sc && out);
@@ -238,12 +334,15 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
   rc = epb_plan_phase_grid(g, in, BM, P.grid, maps.a, dense);
   if (rc) return rc;
   // a dense layer's output is the same [M][Cout] matrix as its phase grid
-  const int64_t Ho = dense ? 1 : g->Ho, Wo = dense ? P.grid.Wp : g->Wo, os = g->os;
+  const int64_t Ho = dense ? 1 : g->Ho, Wo = dense ? P.grid.Wp : g->Wo, os = dense ? 1 : g->os;
   const int64_t ph = dense ? 0 : g->ph, pw = dense ? 0 : g->pw;
   P.Cout = g->Cout;
   P.Wv = dense ? P.grid.Wp : (g->Wo - g->pw + g->os - 1) / g->os;
   P.Hv = dense ? 1 : (g->Ho - g->ph + g->os - 1) / g->os;
-  {
+  P.T = g->T; P.CB = g->Cin / 64; P.accumulate = g->accumulate;
+  P.splits = splits;
+  float* const view = out + (ph * Wo + pw) * g->Cout;
+  if (splits == 1) {
     // (Cout, Wv, Hv, N) view of output phase (ph, pw); Cout % 4 == 0 keeps base and strides
     // 16-byte aligned.  Box: 32 columns x the 16 tile rows of one consumer warp.
     const int bw = P.grid.tw < 16 ? P.grid.tw : 16;
@@ -254,18 +353,26 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
     const cuuint64_t strides[3] = {(cuuint64_t)(os * C4), (cuuint64_t)(os * Wo * C4),
                                    (cuuint64_t)(Ho * Wo * C4)};
     const cuuint32_t box[4] = {32, (cuuint32_t)bw, (cuuint32_t)bh, (cuuint32_t)(16 / (bw * bh))};
-    rc = epb_encode_map(&maps.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, out + (ph * Wo + pw) * g->Cout,
-                        dims, strides, box, CU_TENSOR_MAP_L2_PROMOTION_NONE, "output");
+    rc = epb_encode_map(&maps.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, view, dims, strides, box,
+                        CU_TENSOR_MAP_L2_PROMOTION_NONE, "output");
+    if (rc) return rc;
+  } else {
+    // dense workspace [S][tiles * 128][Cout] as (Cout, 16, tiles * 8, S): one warp's 16 rows per box
+    const int64_t C4 = (int64_t)g->Cout * 4;
+    const cuuint64_t dims[4] = {(cuuint64_t)g->Cout, 16, (cuuint64_t)P.grid.tiles * (BM / 16),
+                                (cuuint64_t)splits};
+    const cuuint64_t strides[3] = {(cuuint64_t)C4, (cuuint64_t)(16 * C4),
+                                   (cuuint64_t)((int64_t)P.grid.tiles * BM * C4)};
+    const cuuint32_t box[4] = {32, 16, 1, 1};
+    rc = epb_encode_map(&maps.out, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ws, dims, strides, box,
+                        CU_TENSOR_MAP_L2_PROMOTION_NONE, "split-K workspace");
     if (rc) return rc;
   }
-  P.T = g->T; P.CB = g->Cin / 64; P.accumulate = g->accumulate;
   for (int t = 0; t < g->T; ++t) P.koff[t] = g->wt[t] * g->Cin;
   // tile order: statistics want runs of tiles with the same N tile (one flush per run); without
   // statistics, N-fastest lets the concurrently running tiles of one M tile share its A rows in L2
   P.m_fastest = stats != nullptr;
-  // N tile: the 128-column accumulator of a consumer warpgroup (64 fp32 registers per thread),
-  // 64 columns for narrow layers
-  const int bn = g->Cout <= 64 ? 64 : 128;
+  const int bn = conv16_bn(g->Cout);
   P.n_tiles = (g->Cout + bn - 1) / bn;
   const int64_t K = (int64_t)g->Tw * g->Cin;
   const cuuint64_t dims[3] = {(cuuint64_t)K, (cuuint64_t)g->Cout, 2};
@@ -275,11 +382,85 @@ extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
                       CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "weights");
   if (rc) return rc;
   const int64_t tiles = (int64_t)P.grid.tiles * P.n_tiles;
-  const unsigned grid = (unsigned)(tiles < kNumSMs ? tiles : kNumSMs);
   cudaStream_t st = as_stream(stream);
-  if (bn == 64)
-    return tc::launch<conv16_kernel<64>>(grid, kThreads16, Cfg16<64>::SMEM, st, P, maps, in_sc,
-                                         w_sc, bias, stats);
-  return tc::launch<conv16_kernel<128>>(grid, kThreads16, Cfg16<128>::SMEM, st, P, maps, in_sc,
-                                        w_sc, bias, stats);
+  if (splits == 1) {
+    const unsigned grid = (unsigned)(tiles < kNumSMs ? tiles : kNumSMs);
+    if (bn == 64)
+      return tc::launch<conv16_kernel<64, false>>(grid, kThreads16, Cfg16<64>::SMEM, st, P, maps,
+                                                  in_sc, w_sc, bias, stats);
+    return tc::launch<conv16_kernel<128, false>>(grid, kThreads16, Cfg16<128>::SMEM, st, P, maps,
+                                                 in_sc, w_sc, bias, stats);
+  }
+  P.m_fastest = 0;
+  const int64_t items = tiles * splits;
+  const unsigned grid = (unsigned)(items < kNumSMs ? items : kNumSMs);
+  const float* no_bias = nullptr;
+  double* no_stats = nullptr;
+  rc = bn == 64 ? tc::launch<conv16_kernel<64, true>>(grid, kThreads16, Cfg16<64>::SMEM, st, P, maps,
+                                                      in_sc, w_sc, no_bias, no_stats)
+                : tc::launch<conv16_kernel<128, true>>(grid, kThreads16, Cfg16<128>::SMEM, st, P,
+                                                       maps, in_sc, w_sc, no_bias, no_stats);
+  if (rc) return rc;
+  Reduce16 R;
+  R.grid = P.grid;
+  R.Cout = g->Cout; R.Wv = P.Wv; R.Hv = P.Hv; R.splits = splits;
+  R.sw = os * g->Cout; R.sh = os * Wo * g->Cout; R.sn = Ho * Wo * g->Cout;
+  const int64_t M = (int64_t)P.grid.N * P.grid.Hp * P.grid.Wp;
+  const unsigned gx = (unsigned)((g->Cout + 127) / 128);
+  int64_t gy = (M + 7) / 8, cap = 4 * kNumSMs / gx + 1;
+  if (gy > cap) gy = cap;
+  conv16_splitk_reduce<<<dim3(gx, (unsigned)gy), dim3(32, 8), 0, st>>>(R, ws, bias, view, stats);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+}  // namespace
+
+extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop(
+    const epb_conv_geom* g, const epb_half* in, const float* in_sc, const epb_half* w,
+    const float* w_sc, const float* bias, float* out, double* stats, epb_stream_t stream) {
+  return conv16_run(g, in, in_sc, w, w_sc, bias, out, stats, 1, nullptr, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_conv16_splits(const epb_conv_geom* g,
+                                                                          int* splits,
+                                                                          long long* ws_floats) {
+  int rc = epb_conv_geom_check(g);
+  if (rc) return rc;
+  EPB_CHECK_ARG(splits && ws_floats && g->Cin % 64 == 0 && g->Cout >= 4);
+  epb_phase_grid G;
+  bool dense;
+  rc = epb_tile_phase_grid(g, BM, G, dense);
+  if (rc) return rc;
+  const int bn = conv16_bn(g->Cout);
+  const int64_t tiles = (int64_t)G.tiles * ((g->Cout + bn - 1) / bn);
+  const int64_t kb = (int64_t)g->T * (g->Cin / 64);
+  // as many splits as keep every SM busy with one work item, none when the tiles already fill
+  // more than half of the SMs (a second split would start a second wave)
+  int64_t s = kNumSMs / tiles;
+  if (s > kb / kSplitMinKB) s = kb / kSplitMinKB;
+  if (s < 4 && kb < kSplitLongKB * s) s = 1;
+  if (s < 1) s = 1;
+  *splits = (int)s;
+  *ws_floats = s > 1 ? s * G.tiles * BM * g->Cout : 0;
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_conv16_fprop_splitk(
+    const epb_conv_geom* g, const epb_half* in, const float* in_sc, const epb_half* w,
+    const float* w_sc, const float* bias, float* out, double* stats, int splits, float* ws,
+    long long ws_floats, epb_stream_t stream) {
+  int rc = epb_conv_geom_check(g);
+  if (rc) return rc;
+  EPB_CHECK_ARG(!g->accumulate);            // an inference forward: no data-gradient accumulate
+  EPB_CHECK_ARG(g->Cin % 64 == 0 && splits >= 1 && splits <= g->T * (g->Cin / 64));
+  if (splits > 1) {
+    epb_phase_grid G;
+    bool dense;
+    rc = epb_tile_phase_grid(g, BM, G, dense);
+    if (rc) return rc;
+    EPB_CHECK_ARG(ws && (reinterpret_cast<uintptr_t>(ws) & 15) == 0);
+    EPB_CHECK_ARG(ws_floats >= (long long)splits * G.tiles * BM * g->Cout);
+  }
+  return conv16_run(g, in, in_sc, w, w_sc, bias, out, stats, splits, ws, stream);
 }

@@ -94,14 +94,11 @@ struct epb_phase_grid {
   }
 };
 
-// Tiles the phase grid of `g` into boxes of `rows` pixels and encodes the parity views of
-// the split input `in` that the taps read (a tap offset d on a stride-s view has parity
-// q = d mod s and quotient (d - q) / s).  Slots no tap uses repeat a used view, since the
-// kernels prefetch all four.  A 1x1 stride-1 layer whose phase grid IS the input and the
-// output grid is a plain [M][C] matrix: it is collapsed to one row of M pixels (no waste
-// whatever H and W are) and `dense` is set.
-inline int epb_plan_phase_grid(const epb_conv_geom* g, const epb_half* in, int rows,
-                               epb_phase_grid& G, CUtensorMap (&maps)[4], bool& dense) {
+// Tiles the phase grid of `g` into boxes of `rows` pixels (G's tap fields are left unset).
+// A 1x1 stride-1 layer whose phase grid IS the input and the output grid is a plain [M][C]
+// matrix: it is collapsed to one row of M pixels (no waste whatever H and W are) and `dense`
+// is set.
+inline int epb_tile_phase_grid(const epb_conv_geom* g, int rows, epb_phase_grid& G, bool& dense) {
   dense = g->T == 1 && g->is == 1 && g->os == 1 && g->dh[0] == 0 && g->dw[0] == 0 &&
           g->Hp == g->Hi && g->Wp == g->Wi && g->Hp == g->Ho && g->Wp == g->Wo;
   G.N = g->N; G.Hp = g->Hp; G.Wp = g->Wp;
@@ -116,6 +113,16 @@ inline int epb_plan_phase_grid(const epb_conv_geom* g, const epb_half* in, int r
   const int64_t tiles = (int64_t)G.tiles_w * G.tiles_h * ((G.N + G.tn - 1) / G.tn);
   EPB_CHECK_ARG(tiles < (1LL << 30));
   G.tiles = (int)tiles;
+  return EPB_OK;
+}
+
+// epb_tile_phase_grid, then encodes the parity views of the split input `in` that the taps
+// read (a tap offset d on a stride-s view has parity q = d mod s and quotient (d - q) / s).
+// Slots no tap uses repeat a used view, since the kernels prefetch all four.
+inline int epb_plan_phase_grid(const epb_conv_geom* g, const epb_half* in, int rows,
+                               epb_phase_grid& G, CUtensorMap (&maps)[4], bool& dense) {
+  const int rc = epb_tile_phase_grid(g, rows, G, dense);
+  if (rc) return rc;
   bool need[4] = {false, false, false, false};
   for (int t = 0; t < g->T; ++t) {
     const int qh = ((g->dh[t] % g->is) + g->is) % g->is;
@@ -128,9 +135,9 @@ inline int epb_plan_phase_grid(const epb_conv_geom* g, const epb_half* in, int r
   const int Hi = dense ? 1 : g->Hi, Wi = dense ? G.Wp : g->Wi;
   for (int v = 0; v < 4; ++v) {
     if (!need[v]) continue;
-    const int rc = epb_make_act_map(&maps[v], in, G.N, Hi, Wi, g->Cin, g->is, v >> 1, v & 1,
+    const int rv = epb_make_act_map(&maps[v], in, G.N, Hi, Wi, g->Cin, g->is, v >> 1, v & 1,
                                     G.tw, G.th, G.tn);
-    if (rc) return rc;
+    if (rv) return rv;
   }
   for (int v = 0; v < 4; ++v)
     if (!need[v]) {

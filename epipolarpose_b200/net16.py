@@ -95,8 +95,33 @@ class Engine16(_net.Engine):
         ops.split16_batch(st["batch"])
         return st["w"]
 
+    def prepare_inference(self, params, dev, state=None):
+        """The weights of an inference forward (forward(..., prepared=...)), prepared once outside
+        the walk: the fp32 pack, the split planes, the BatchNorm eval affines and the final layer's
+        (padded) bias.  With `state` (an earlier result) the same tensors are refilled, so that
+        CUDA graphs captured on them read the new values."""
+        ops, plan = self.ops, self.plan
+        if plan.fc is not None:
+            raise ValueError("the inference forward needs the VOLUME head (MODEL.VOLUME: true)")
+        self.dev = dev
+        packed = self._pack_weights(params)
+        w16 = self._split_weights(packed)
+        bn = state["bn"] if state is not None else {}
+        for name, C in plan.all_bns():
+            if name not in bn:
+                bn[name] = self._bn_eval(name, C, params)
+                continue
+            ops.bn_eval_affine(C, params[name + ".weight"], params[name + ".bias"],
+                               params[name + ".running_mean"], params[name + ".running_var"],
+                               BN_EPS, bn[name].scale, bn[name].shift)
+        fin = plan.final
+        fbias = state["fbias"] if state is not None else torch.zeros(fin.cout_p, device=dev)
+        fbias[:fin.cout].copy_(params[fin.name + ".bias"])
+        return {"packed": packed, "w16": w16, "bn": bn, "fbias": fbias}
+
     # ------------------------------------------------------------------ conv helpers
-    def _conv_fwd16(self, conv, x, x_sc, N, H, W, w16, bias=None, stats=None):
+    def _conv_fwd16(self, conv, x, x_sc, N, H, W, w16, bias=None, stats=None, splitk=False):
+        """splitk: every call takes the split count of the planner (epb_conv16_splits)."""
         ops = self.ops
         Ho, Wo = conv.out_hw(H, W)
         geoms = self._geoms(conv, "f", N, H, W)
@@ -107,7 +132,14 @@ class Engine16(_net.Engine):
             if g is None:
                 continue
             g.in_relu, g.accumulate = 0, 0
-            ops.conv16_fprop(g, x, x_sc, w16[0], w16[1], out, bias, stats)
+            if splitk:
+                splits, n = ops.conv16_splits(g)
+                ws = self._consts()["ws"]
+                if n > ws.numel():
+                    ws = torch.empty(n, device=self.dev, dtype=torch.float32)
+                ops.conv16_fprop_splitk(g, x, x_sc, w16[0], w16[1], out, bias, stats, splits, ws)
+            else:
+                ops.conv16_fprop(g, x, x_sc, w16[0], w16[1], out, bias, stats)
         return out, Ho, Wo
 
     def _conv_dgrad16(self, conv, dz, dz_sc, N, H, W, wd16, accumulate_into=None):
@@ -165,8 +197,14 @@ class Engine16(_net.Engine):
         return dz, dz_sc
 
     # ------------------------------------------------------------------ forward
-    def forward(self, x_nchw, params, training=True, save=True):
+    def forward(self, x_nchw, params, training=True, save=True, prepared=None):
+        """prepared: the result of prepare_inference -- an inference forward (eval BatchNorm, no
+        saved state) that reads those weights instead of `params` and runs every conv through
+        the split-K entry."""
         ops, plan = self.ops, self.plan
+        infer = prepared is not None
+        if infer and (training or save):
+            raise ValueError("a forward on prepared weights is an inference forward (training=False, save=False)")
         self.dev = x_nchw.device
         N, _, H, W = x_nchw.shape
         cst = self._consts()
@@ -196,7 +234,7 @@ class Engine16(_net.Engine):
                 fused = None if sc is None else group2 + (res_sc, sc)
                 st = self._bn_train(name, C, stats_of(name, C), M, params, None, act_scale=fused)
             else:
-                st = self._bn_eval(name, C, params)
+                st = prepared["bn"][name] if infer else self._bn_eval(name, C, params)
                 if sc is not None:
                     ops.act_scale(stats_of(name, C), st.scale, st.shift, M, C, *group2, res_sc, sc)
             S["bn"][name] = st
@@ -204,11 +242,14 @@ class Engine16(_net.Engine):
 
         self._nbt_tick = []
 
-        S["packed"] = self._pack_weights(params)
-        S["w16"] = self._split_weights(S["packed"])
+        if infer:
+            S["packed"], S["w16"] = prepared["packed"], prepared["w16"]
+        else:
+            S["packed"] = self._pack_weights(params)
+            S["w16"] = self._split_weights(S["packed"])
 
-        def w16(conv):
-            return S["w16"][conv.name][0]
+        def conv_fwd(conv, x, x_sc, N, H, W, **kw):
+            return self._conv_fwd16(conv, x, x_sc, N, H, W, S["w16"][conv.name][0], splitk=infer, **kw)
 
         def bn_act(z, name, shape):
             """BatchNorm state of conv output z, its post-BatchNorm/ReLU split tensor and scale"""
@@ -226,7 +267,7 @@ class Engine16(_net.Engine):
         col = self._half(N, H1, W1, kpad)
         isc = cst["img_sc"]
         ops.im2col_split(x_nchw, col, isc, N, 3, H, W, 7, 7, 2, 3, H1, W1, kpad)
-        z0, _, _ = self._conv_fwd16(scol, col, isc, N, H1, W1, w16(stem), stats=stats_of("bn1", 64))
+        z0, _, _ = conv_fwd(scol, col, isc, N, H1, W1, stats=stats_of("bn1", 64))
         cur_sc = new_sc()
         b0 = bn("bn1", 64, N * H1 * W1, cur_sc)
         H2, W2 = (H1 + 2 - 3) // 2 + 1, (W1 + 2 - 3) // 2 + 1
@@ -244,8 +285,7 @@ class Engine16(_net.Engine):
             nconv = len(blk["convs"])
             for ci, conv in enumerate(blk["convs"]):
                 bname, C = blk["bns"][ci]
-                z, ho, wo = self._conv_fwd16(conv, src, src_sc, N, hh, ww, w16(conv),
-                                             stats=stats_of(bname, C))
+                z, ho, wo = conv_fwd(conv, src, src_sc, N, hh, ww, stats=stats_of(bname, C))
                 rec["z"].append(z)
                 rec["hw"].append((hh, ww))
                 hh, ww = ho, wo
@@ -262,8 +302,7 @@ class Engine16(_net.Engine):
             obits = torch.empty(M * Cl // 8, device=self.dev, dtype=torch.uint8) if save else None
             if blk["down"]:
                 dconv, (dname, dC) = blk["down"]
-                zd, _, _ = self._conv_fwd16(dconv, cur, cur_sc, N, h, w, w16(dconv),
-                                            stats=stats_of(dname, dC))
+                zd, _, _ = conv_fwd(dconv, cur, cur_sc, N, h, w, stats=stats_of(dname, dC))
                 dst = bn(dname, dC, M)
                 rec["zd"] = zd
                 last = bn(lname, Cl, M, out_sc, (stats_of(dname, dC), dst.scale, dst.shift))
@@ -284,7 +323,7 @@ class Engine16(_net.Engine):
         S["deconv"] = []
         zlast, stlast = None, None
         for conv, (bname, C) in plan.deconvs:
-            z, ho, wo = self._conv_fwd16(conv, src, src_sc, N, h, w, w16(conv), stats=stats_of(bname, C))
+            z, ho, wo = conv_fwd(conv, src, src_sc, N, h, w, stats=stats_of(bname, C))
             S["deconv"].append((src, src_sc, z, h, w))
             st, src, src_sc = bn_act(z, bname, (N, ho, wo, conv.cout_p))
             h, w = ho, wo
@@ -293,12 +332,15 @@ class Engine16(_net.Engine):
             raise RuntimeError("the split path expects at least one deconv layer")
         # ---- final 1x1 / 3x3 conv with bias (:199)
         fin = plan.final
-        fbias = params[fin.name + ".bias"]
-        if fin.cout_p != fin.cout:
-            fb = torch.zeros(fin.cout_p, device=self.dev)
-            fb[:fin.cout] = fbias
-            fbias = fb
-        logits, ho, wo = self._conv_fwd16(fin, src, src_sc, N, h, w, w16(fin), bias=fbias)
+        if infer:
+            fbias = prepared["fbias"]
+        else:
+            fbias = params[fin.name + ".bias"]
+            if fin.cout_p != fin.cout:
+                fb = torch.zeros(fin.cout_p, device=self.dev)
+                fb[:fin.cout] = fbias
+                fbias = fb
+        logits, ho, wo = conv_fwd(fin, src, src_sc, N, h, w, bias=fbias)
         # the final layer's backward: split operands when the head has whole 64-channel blocks,
         # else the 3xTF32 kernels from (z, BatchNorm affine)
         S["final"] = (zlast, (stlast.scale, stlast.shift), h, w)

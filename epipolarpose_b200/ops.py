@@ -255,6 +255,24 @@ def conv16_fprop(g, x, x_sc, w, w_sc, out, bias=None, stats=None):
           _p(out), _p(stats, torch.float64), _stream())
 
 
+def conv16_splits(g):
+    """Split planner of conv16_fprop_splitk (host only): (splits, workspace floats)."""
+    s, n = ctypes.c_int(), ctypes.c_longlong()
+    _lib.call("epb_conv16_splits", ctypes.byref(g), ctypes.byref(s), ctypes.byref(n))
+    return s.value, n.value
+
+
+def conv16_fprop_splitk(g, x, x_sc, w, w_sc, out, bias, stats, splits, ws):
+    """conv16_fprop with each tile's K loop cut into `splits` ranges (statistics are ADDED to
+    `stats`); ws: fp32 workspace of at least conv16_splits(g)[1] floats at that split count."""
+    global launches
+    _call("epb_conv16_fprop_splitk", ctypes.byref(g), _p(x, _H), _p(x_sc), _p(w, _H), _p(w_sc), _p(bias),
+          _p(out), _p(stats, torch.float64), int(splits), _p(ws), ws.numel() if ws is not None else 0,
+          _stream())
+    if splits > 1:
+        launches += 1                     # the reduce kernel
+
+
 def conv16_wgrad(g, x, x_sc, dout, dout_sc, dw, ws):
     _call("epb_conv16_wgrad", ctypes.byref(g), _p(x, _H), _p(x_sc), _p(dout, _H), _p(dout_sc),
           _p(dw), _p(ws), ws.numel() if ws is not None else 0, _stream())

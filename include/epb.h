@@ -270,6 +270,24 @@ int epb_split16(const float* src, long long n, epb_half* dst, float* sc, uint32_
 int epb_conv16_fprop(const epb_conv_geom* g, const epb_half* in, const float* in_sc,
                      const epb_half* w, const float* w_sc, const float* bias,
                      float* out, double* stats, epb_stream_t stream);
+/* Split-K form of epb_conv16_fprop for layers whose tiles fill few SMs (small batches): each
+ * 128-row tile's K loop (K/64 k-blocks) is cut into `splits` contiguous ranges that run as
+ * separate work items; each stores acc / (s_in * s_w) as fp32 into `ws` [splits][tiles * 128]
+ * [Cout], and a second kernel sums the splits in the order 0..splits-1 (same inputs, same bits),
+ * adds the bias, writes the output view as epb_conv16_fprop does and ADDS the per-channel sum /
+ * sum of squares of the valid rows to `stats` (the phase calls of a transposed conv share one
+ * buffer).  splits == 1 is epb_conv16_fprop (bit-identical; ws unused).  EPB_EINVAL for
+ * g->accumulate, splits outside [1, K/64] or ws_floats below the size epb_conv16_splits
+ * reports. */
+int epb_conv16_fprop_splitk(const epb_conv_geom* g, const epb_half* in, const float* in_sc,
+                            const epb_half* w, const float* w_sc, const float* bias,
+                            float* out, double* stats, int splits, float* ws,
+                            long long ws_floats, epb_stream_t stream);
+/* Host-only split planner of epb_conv16_fprop_splitk: splits = min(SMs / tiles, K/64 / 4),
+ * where tiles = M tiles x N tiles; a count below 4 only while every split keeps >= 16
+ * k-blocks, else 1; 1 whenever the tiles fill more than half of the SMs.  ws_floats =
+ * splits * (M tiles * 128) * Cout (0 when splits == 1). */
+int epb_conv16_splits(const epb_conv_geom* g, int* splits, long long* ws_floats);
 /* epb_conv_wgrad on split operands (in as above, dout [2][N,Ho,Wo,Cout]); both operands
  * MN-major by TMA, reduction over pixel tiles split across CTAs and summed in a FIXED
  * order from `ws` (deterministic): dw[co][wt[t]][ci] += sum.  ws: >= ws_floats floats of
