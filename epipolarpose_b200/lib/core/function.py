@@ -16,6 +16,10 @@ Differences from the reference body (same observable behaviour):
     projection matrix needed: the reference's "without R/t" mode);
   * the gradient all-reduce for multi-GPU data parallelism happens inside the
     model's backward (one NCCL call on the flat gradient buffer);
+  * loader batches of deferred samples (lib/dataset/deferred.py: the h36m / mpii_integral
+    datasets indexed in DataLoader workers) are assembled on the device, and a TRI batch
+    {'cam_1', 'cam_2'} becomes one batch [cam_1 ; cam_2] (`loader_batch`); the graphed step
+    assembles batch i+1 on a side stream while step i replays;
   * validate_integral honours TEST.FLIP_TEST and TEST.SHIFT_HEATMAP (reference
     config.py:118,120, read nowhere by the reference): each batch is one forward of
     [x; flip(x)] and the logits are merged with their flipped-back mirror before the
@@ -31,8 +35,23 @@ from ..utils.img_utils import (self_supervision_device,
                                trans_coords_from_patch_to_org_3d_batch)
 from .integral_loss import get_joint_location_coords_flip, get_result_func, joint_location_result_from_coords
 from ..utils.utils import AverageMeter
+from ..dataset.deferred import assemble_batch, cat_meta, is_deferred
 
 logger = logging.getLogger(__name__)
+
+
+def loader_batch(data):
+    """(batch_data, label, weight, meta) of a loader batch.  A batch of deferred samples (a
+    dataset indexed in DataLoader workers) is assembled on the device; a TRI batch
+    {'cam_1', 'cam_2'} becomes one batch [cam_1 ; cam_2], the first-half / second-half pairing
+    of online triangulation (reference img_utils.py:194-199)."""
+    if is_deferred(data):
+        return assemble_batch(data)
+    if isinstance(data, dict) and 'cam_1' in data and 'cam_2' in data:
+        a, b = data['cam_1'], data['cam_2']
+        return (torch.cat([a[0], b[0]]), torch.cat([a[1], b[1]]), torch.cat([a[2], b[2]]),
+                cat_meta(a[3], b[3]))
+    return data
 
 
 class _fused_head:
@@ -118,6 +137,7 @@ class GraphedTrainStep:
         self.failed = False
         self.calls = 0
         self.copy_stream, self.pending, self.stage_next = None, None, 0
+        self.assemble_stream, self.staged = None, None
         # eager warm-up and capture share ONE side stream so that the parameters'
         # AccumulateGrad nodes are never bound to the legacy default stream (which
         # may not join a capture)
@@ -170,6 +190,31 @@ class GraphedTrainStep:
             self.stage_evt[k].record(self.copy_stream)
         self.pending = (batch_data, k)
         self.stage_next = 1 - k
+
+    def stage_batch(self, batch):
+        """Assemble a deferred loader batch (lib/dataset/deferred.py) on a side stream, so that
+        its decode, crop and labels overlap the replay of the current step; `take` hands it over."""
+        if self.graph is None or not torch.cuda.is_available() or not is_deferred(batch):
+            return
+        if self.assemble_stream is None:
+            self.assemble_stream = torch.cuda.Stream()
+        with torch.cuda.stream(self.assemble_stream):
+            out = assemble_batch(batch)
+            ev = torch.cuda.Event()
+            ev.record(self.assemble_stream)
+        self.staged = (batch, out, ev)
+
+    def take(self, batch):
+        """(batch_data, label, weight, meta) of a loader batch; a batch `stage` assembled is
+        handed over to the current stream."""
+        staged, self.staged = self.staged, None
+        if staged is None or staged[0] is not batch:
+            return loader_batch(batch)
+        cur = torch.cuda.current_stream()
+        cur.wait_event(staged[2])
+        for t in staged[1][:3]:
+            t.record_stream(cur)
+        return staged[1]
 
     def _load_input(self, batch_data):
         if self.pending is not None and self.pending[0] is batch_data:
@@ -277,7 +322,8 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
         data, i = nxt, i + 1
         nxt = next(it, None)
         data_time.update(time.time() - end)
-        batch_data, batch_label, batch_label_weight, meta = data
+        batch_data, batch_label, batch_label_weight, meta = \
+            stepper.take(data) if use_graph else loader_batch(data)
         batch_size = batch_data.size(0)
         if use_graph:
             if stepper.pending is None and stepper.graph is not None:
@@ -285,8 +331,11 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
             loss = stepper(batch_data, batch_label, batch_label_weight, meta)
             if stepper.graph is not None:
                 loss = loss.clone()      # the static loss buffer is overwritten by the next replay
-                if nxt is not None:
-                    stepper.prefetch(nxt[0])     # H2D of the next batch overlaps this step
+                if nxt is not None:      # H2D / device assembly of the next batch overlaps this step
+                    if is_deferred(nxt):
+                        stepper.stage_batch(nxt)
+                    elif isinstance(nxt, (list, tuple)):
+                        stepper.prefetch(nxt[0])
             pending.append((loss, batch_size))
             del loss
         else:
@@ -354,7 +403,7 @@ def _validate_flip(val_loader, model, shift_heatmap):
     chunks = []
     with torch.no_grad():
         for data in val_loader:
-            x = data[0]
+            x = loader_batch(data)[0]
             B = x.shape[0]
             buf = torch.empty((2 * B,) + tuple(x.shape[1:]), device=dev, dtype=torch.float32)
             buf[:B].copy_(x, non_blocking=True)
@@ -385,7 +434,7 @@ def validate_integral(val_loader, model, flip_test=None, shift_heatmap=None):
     chunks = []
     with torch.no_grad():
         for i, data in enumerate(val_loader):
-            batch_data = data[0].cuda(non_blocking=True)
+            batch_data = loader_batch(data)[0].cuda(non_blocking=True)
             preds = model(batch_data)
             chunks.append(result_func(256, 256, preds))     # hard-coded 256 as reference :87
             del preds, batch_data

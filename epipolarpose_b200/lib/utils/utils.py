@@ -312,6 +312,18 @@ def save_checkpoint(states, is_best, output_dir, filename='checkpoint.pth.tar'):
         torch.save(states['state_dict'], os.path.join(output_dir, 'model_best.pth.tar'))
 
 
+def calc_kpt_bound(kpts, kpts_vis):
+    """reference :96-112: (up, down, left, right) of the joints whose visibility is not 0;
+    (10000, -1, 10000, -1) when none is."""
+    u, d, l, r = 10000, -1, 10000, -1
+    for idx, vis in enumerate(kpts_vis[:, 0]):
+        if vis == 0:
+            continue
+        u, d = min(u, kpts[idx, 1]), max(d, kpts[idx, 1])
+        l, r = min(l, kpts[idx, 0]), max(r, kpts[idx, 0])
+    return u, d, l, r
+
+
 class AverageMeter(object):
     """reference :199-214."""
 
