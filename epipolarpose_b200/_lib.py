@@ -66,6 +66,11 @@ _PROTOS = {
                                   c_p]),
     "epb_project_labels": (c_int, [c_p, c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_p, c_p, c_p]),
     "epb_h36m_eval": (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, ctypes.c_uint32, c_d, c_p, c_p, c_p, c_p, c_p]),
+    "epb_pose_normalize": (c_int, [c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
+    "epb_kmeans_workspace": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_i64)]),
+    "epb_kmeans_fit": (c_int, [c_p, c_int, c_int, c_int, ctypes.c_uint64, c_int, c_int, c_p, c_p, c_p, c_p, c_p,
+                               c_i64, ctypes.POINTER(c_d), ctypes.POINTER(ctypes.c_int32), c_p]),
+    "epb_kmeans_assign": (c_int, [c_p, c_int, c_int, c_p, c_int, c_p, c_p, c_p]),
     "epb_add3": (c_int, [c_p, c_p, c_p, c_p, c_i64, c_p]),
     "epb_mask_scale": (c_int, [c_p, c_p, c_f, c_p, c_i64, c_p]),
     "epb_patch_sample": (c_int, [c_p, c_p, c_p, c_p, c_p, c_p, c_p, c_int, c_int, c_int, c_p, c_p, c_p]),

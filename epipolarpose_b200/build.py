@@ -12,7 +12,8 @@ LIB = os.path.join(HERE, "libepb.so")
 
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo",
               "-std=c++17", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden"]
-PER_FILE = {"geometry.cu": ["--fmad=false"], "input.cu": ["--fmad=false"]}   # double rounding as on the CPU
+PER_FILE = {"geometry.cu": ["--fmad=false"], "input.cu": ["--fmad=false"],    # double rounding as on the CPU
+            "pss.cu": ["--fmad=false"]}
 
 
 def _nvcc():

@@ -30,7 +30,7 @@ void epb_set_error(const char* fmt, ...);
 
 // per-(purpose, device, stream) internal scratch; see core.cu
 enum { EPB_WS_SOFTARGMAX = 1, EPB_WS_HMLOSS = 2, EPB_WS_BNCOEF = 3, EPB_WS_WPLANES = 4,
-       EPB_WS_FPAIR = 5, EPB_WS_BNPART = 6, EPB_WS_SABWD = 7, EPB_WS_PATCHINV = 8 };
+       EPB_WS_FPAIR = 5, EPB_WS_BNPART = 6, EPB_WS_SABWD = 7, EPB_WS_PATCHINV = 8, EPB_WS_KMEANS = 9 };
 int epb_workspace(int kind, size_t bytes, cudaStream_t st, void** out);
 
 static inline cudaStream_t as_stream(epb_stream_t s) { return (cudaStream_t)s; }

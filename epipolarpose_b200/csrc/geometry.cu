@@ -10,6 +10,7 @@
 // and latency-bound at real sizes (64 pairs x 17 joints); no tensor cores.
 // Compiled with --fmad=false so that a*b+c rounds twice as on the CPU.
 #include "common.cuh"
+#include "camera.cuh"
 #include <float.h>
 
 namespace {
@@ -687,15 +688,8 @@ __host__ __device__ void h36m_eval_sample(const double* p, const double* q, cons
                                           int J, int root, unsigned j14mask, double pck_thr,
                                           double* metrics, double* per_joint, int32_t* pck,
                                           double* poses) {
-  const double fx = cam[0], fy = cam[1], cx = cam[2], cy = cam[3];
-  const double zr = cam[4];
   // back projection (h36m.py:228-240): X = gt (targets), Y = prediction (inputs)
-  auto bp = [&](const double* a, int j, double (&o)[3]) {
-    const double d = a[j * 3 + 2] + zr;
-    o[0] = (a[j * 3 + 0] - cx) / fx * d;
-    o[1] = (a[j * 3 + 1] - cy) / fy * d;
-    o[2] = d;
-  };
+  auto bp = [&](const double* a, int j, double (&o)[3]) { cam_back_proj(a, j, cam, o); };
   double muX[3] = {0, 0, 0}, muY[3] = {0, 0, 0};
   for (int j = 0; j < J; ++j) {
     double x[3], y[3];

@@ -10,7 +10,9 @@ Extra keys (superset, all default-off): TRAIN.ONLINE_TRIANGULATION,
 TRAIN.TRIANGULATION_METHOD, TRAIN.ESTIMATE_EXTRINSICS (self-supervision without camera
 extrinsics: each view pair's pose is estimated from its 2-D joints; needs
 TRAIN.ONLINE_TRIANGULATION, ValueError otherwise), TRAIN.CUDA_GRAPH (default on),
-MODEL.PRECISION, DATASET.SYNTHETIC_LEN.
+MODEL.PRECISION, DATASET.SYNTHETIC_LEN, TEST.PSS_K (list of k: the H36M evaluation appends
+PSS@k, lib/core/pss.py; default []), TEST.PSS_CENTROIDS (.npz of `k<k>` centroids used instead
+of fitting them on train-fs; default '').
 """
 import os
 
@@ -66,7 +68,7 @@ _DEFAULTS = dict(
                CUDA_GRAPH=True),
     TEST=dict(BATCH_SIZE=32, FLIP_TEST=False, POST_PROCESS=True, SHIFT_HEATMAP=True,
               USE_GT_BBOX=False, OKS_THRE=0.5, IN_VIS_THRE=0.0, COCO_BBOX_FILE='', BBOX_THRE=1.0,
-              MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0),
+              MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0, PSS_K=[], PSS_CENTROIDS=''),
     DEBUG=dict(DEBUG=False, SAVE_BATCH_IMAGES_GT=False, SAVE_BATCH_IMAGES_PRED=False,
                SAVE_HEATMAPS_GT=False, SAVE_HEATMAPS_PRED=False, SAVE_3D=False),
 )

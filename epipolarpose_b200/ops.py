@@ -433,6 +433,39 @@ def h36m_eval(pred, gt, cam, S, J, root, j14mask, pck_thr, metrics, per_joint, p
           _p(per_joint, torch.float64), _p(pck, torch.int32), _p(poses, torch.float64), _stream())
 
 
+def pose_normalize(pose, cam, S, J, root, out):
+    _call("epb_pose_normalize", _p(pose, torch.float64), _p(cam, torch.float64), S, J, root,
+          _p(out, torch.float64), _stream())
+
+
+def kmeans_workspace(N, d, k):
+    """Bytes of the epb_kmeans_fit workspace (host only)."""
+    n = ctypes.c_int64()
+    _lib.call("epb_kmeans_workspace", N, d, k, ctypes.byref(n))
+    return n.value
+
+
+def kmeans_fit(x, N, d, k, seed, restart, max_iter, centroids, labels, init_idx, trace, ws):
+    """One k-means restart (synchronises the stream); returns (inertia, updates done)."""
+    global launches
+    inertia, n_iter = ctypes.c_double(), ctypes.c_int32()
+    _lib.call("epb_kmeans_fit", _p(x, torch.float64), N, d, k, int(seed), restart, max_iter,
+              _p(centroids, torch.float64), _p(labels, torch.int32), _p(init_idx, torch.int32),
+              _p(trace, torch.int32), _p(ws, torch.uint8), ws.numel(), ctypes.byref(inertia),
+              ctypes.byref(n_iter), _stream())
+    # finiteness check, k-means++ (select / distance / chunk sums), pass 0, 4 per iteration, inertia
+    launches += 1 + k + 2 * (k - 1) + 1 + 4 * n_iter.value + 2
+    return inertia.value, n_iter.value
+
+
+def kmeans_assign(x, N, d, centroids, k, labels, dist2):
+    """Assignment of x to the centroids (synchronises the stream after its finiteness check)."""
+    global launches
+    _call("epb_kmeans_assign", _p(x, torch.float64), N, d, _p(centroids, torch.float64), k,
+          _p(labels, torch.int32), _p(dist2, torch.float64), _stream())
+    launches += 2
+
+
 def triangulate_nview(u, stride_u, P, NT, V, J, X, status):
     _call("epb_triangulate_nview", _p(u, torch.float64), stride_u, _p(P, torch.float64), NT, V, J,
           _p(X, torch.float64), _p(status, torch.int32), _stream())

@@ -477,6 +477,45 @@ int epb_h36m_eval(const double* pred, const double* gt, const double* cam, int S
                   int root, uint32_t j14mask, double pck_thr, double* metrics,
                   double* per_joint, int32_t* pck, double* poses, epb_stream_t stream);
 
+/* Pose Structure Score (the EpipolarPose paper's PSS@k, Sec. 3.3; the reference release has no
+ * PSS code, the definition is lib/core/pss.py's).  float64, --fmad=false, every summation order
+ * fixed, so that a numpy restatement reproduces each result bit for bit.
+ *
+ * Normalised pose: CamBackProj (lib/utils/prep_h36m.py:85-89, the arithmetic of epb_h36m_eval) of
+ * every joint, minus the root joint, divided by the Frobenius norm (a zero pose stays zero).
+ *   pose [S][J][3] image-space joints, cam [S][5] as epb_h36m_eval, out [S][3J]. */
+int epb_pose_normalize(const double* pose, const double* cam, int S, int J, int root, double* out,
+                       epb_stream_t stream);
+/* Host only: bytes of the workspace epb_kmeans_fit needs for N points of d coordinates, k
+ * clusters.  EPB_EINVAL for k < 1, k > N, or k, d whose assignment pass does not fit in shared
+ * memory ((k*d + 128*(d|1)) * 8 bytes <= 227 KB). */
+int epb_kmeans_workspace(int N, int d, int k, int64_t* ws_bytes);
+/* One k-means restart on x [N][d] (scikit-learn's KMeans(algorithm='lloyd') with the orders
+ * pinned):
+ *   k-means++, one candidate per step: u_j = top 53 bits of splitmix64 draw j of the state
+ *     seed ^ (restart * 0xD1B54A32D192ED03); centre 0 = floor(u_0 N); centre j = the first point
+ *     whose inclusive prefix of D^2 exceeds u_j * sum(D^2) (prefix and sum: chunks of 1024
+ *     points in index order, chunk totals in chunk order).  init_idx [k] gets the indices.
+ *   Lloyd: assignment = argmin of sum_t (x_t - c_t)^2 in coordinate order, lowest centre on ties;
+ *     update = member sum (chunk partials in index order, combined in chunk order) / count; an
+ *     empty cluster, in cluster order, takes the point farthest from its centre (lowest index on
+ *     ties, no point twice).  Pass 0 assigns to the seeds; each update is followed by a pass;
+ *     stops when a pass changes no label or after max_iter updates.  The host reads 4 bytes
+ *     per iteration (the "changed" flag), so the call returns when the fit is done.
+ * Outputs: centroids [k][d], labels [N] (the last pass: argmin of the returned centroids),
+ * trace [(max_iter+1)][N] or NULL (the labels of every pass), *inertia_host = sum of the last
+ * pass's squared distances (two-level order), *n_iter_host = updates done.  EPB_EINVAL as
+ * epb_kmeans_workspace, and for a non-finite input, sum(D^2) = 0 (fewer than k distinct points)
+ * or ws_bytes below the query. */
+int epb_kmeans_fit(const double* x, int N, int d, int k, uint64_t seed, int restart, int max_iter,
+                   double* centroids, int32_t* labels, int32_t* init_idx, int32_t* trace, void* ws,
+                   int64_t ws_bytes, double* inertia_host, int32_t* n_iter_host, epb_stream_t stream);
+/* labels [N] and squared distances dist2 [N] (or NULL) of x [N][d] to centroids [k][d], as the
+ * assignment pass of epb_kmeans_fit.  Checks x and the centroids for non-finite values first
+ * (EPB_EINVAL), which reads 4 bytes back: the call synchronises the stream. */
+int epb_kmeans_assign(const double* x, int N, int d, const double* centroids, int k, int32_t* labels,
+                      double* dist2, epb_stream_t stream);
+
 /* Element-wise helpers of the refiner MLP (refiner/model.py:39-68,117-143): out = a + b (+ c when
  * c != NULL) -- the residual sums -- and nn.Dropout with an explicit keep mask:
  * out = mask ? x * scale : 0  (scale = 1 / (1 - p); the backward is the same call on the gradient). */
