@@ -103,6 +103,8 @@ _PROTOS = {
     "epb_sgd_step_dev": (c_int, [c_p, c_p, c_p, c_i64, c_p, c_p, c_p]),
     "epb_jpeg_parse": (c_int, [c_p, c_p, c_int, c_p, c_p, c_p, c_p, c_p]),
     "epb_jpeg_decode": (c_int, [c_p, c_p, c_p, c_int, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
+    "epb_softargmax_flip_lse_fwd": (c_int, [c_p] + [c_int] * 5 + [ctypes.POINTER(c_int), c_int, c_p, c_p, c_p]),
+    "epb_triangulate_robust": (c_int, [c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p, c_p, c_p]),
 }
 
 EXPORTS = tuple(_PROTOS)

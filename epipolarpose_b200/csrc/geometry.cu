@@ -1130,6 +1130,224 @@ __global__ void relative_pose_kernel(const double* __restrict__ u, int stride_u,
                diag ? diag + pair * 3 : nullptr);
 }
 
+// --------------------------------------------------------------- robust V-view triangulation
+// Inference on a calibrated rig (2 <= V <= 8 views; not in the reference, which only pairs two
+// views): per (tuple, joint) a consensus over the view pairs instead of one DLT over all views, so
+// that a wrong 2-D joint in one view (occlusion, left / right swap) is left out and reported.
+//   usable views: weight > 0 (and finite) and a finite image point.
+//   1. hypotheses: every pair of usable views in the order (0,1), (0,2), .., (V-2,V-1) (<= 28),
+//      each dlt_nview<2>.
+//   2. score: a usable view is an inlier when the hypothesis lies in front of it (third row of P
+//      times (X, 1) > 0) and reprojects within thr px; cost = sum over the usable views of e^2 for
+//      inliers and thr^2 otherwise (MSAC).  Best = most inliers, then lowest cost, then lowest
+//      hypothesis index: a total order, so the choice does not depend on the reduction's shape.
+//   3. refit: DLT over the inlier views, rows scaled by the weights; the inlier set is taken again
+//      against the refit point and, when it changed, the fit repeated once on the new set.
+//   4. inliers = the views of the last fit, resid = RMS reprojection error (px) over them.
+// status 0 with X = 0, inliers = 0, resid = 0 for: fewer than two inlier views at any stage, a
+// refit system of rank < 3 (the views' rays are one line), a non-finite coordinate or residual,
+// |coordinate| > 1e16.  The body is shared by the kernel (one
+// warp per (tuple, joint): lane h owns hypothesis h, every lane repeats the refit) and the CPU
+// harness (one lane).
+constexpr int RB_MAXV = 8;
+
+struct RbSerial {
+  int lane = 0, n = 1;
+  __host__ __device__ void best(int&, double&, int&) const {}
+};
+struct RbWarp {
+  int lane, n = 32;
+  __host__ __device__ void best(int& cnt, double& cost, int& h) const {
+#ifdef __CUDA_ARCH__
+    for (int o = 16; o > 0; o >>= 1) {
+      const int oc = __shfl_xor_sync(0xffffffffu, cnt, o);
+      const double os = __shfl_xor_sync(0xffffffffu, cost, o);
+      const int oh = __shfl_xor_sync(0xffffffffu, h, o);
+      if (oc > cnt || (oc == cnt && (os < cost || (os == cost && oh < h)))) { cnt = oc; cost = os; h = oh; }
+    }
+#endif
+  }
+};
+
+__host__ __device__ inline int robust_count(unsigned m) {
+  int n = 0;
+  for (; m; m &= m - 1) ++n;
+  return n;
+}
+
+// views (a, b) of hypothesis h, generated from V
+__host__ __device__ inline void robust_pair_of(int h, int V, int& a, int& b) {
+  a = 0;
+  while (h >= V - 1 - a) { h -= V - 1 - a; ++a; }
+  b = a + 1 + h;
+}
+
+// squared reprojection error (px^2) of x in one view; false when x is not in front of the camera
+// or the error is not finite
+__host__ __device__ inline bool robust_reproj2(const double* u, const double* P, const double* x,
+                                               double& e2) {
+  const double z = ((P[8] * x[0] + P[9] * x[1]) + P[10] * x[2]) + P[11];
+  const double dx = (((P[0] * x[0] + P[1] * x[1]) + P[2] * x[2]) + P[3]) / z - u[0];
+  const double dy = (((P[4] * x[0] + P[5] * x[1]) + P[6] * x[2]) + P[7]) / z - u[1];
+  e2 = dx * dx + dy * dy;
+  return z > 0.0 && isfinite(e2);
+}
+
+// inlier views of x among `usable` and the MSAC cost over the usable views
+__host__ __device__ inline unsigned robust_inliers(const double* u, const double* P, int V,
+                                                   unsigned usable, const double* x, double thr2,
+                                                   double& cost) {
+  unsigned m = 0u;
+  cost = 0.0;
+  for (int v = 0; v < V; ++v) {
+    if (!((usable >> v) & 1u)) continue;
+    double e2;
+    const bool in = robust_reproj2(u + 2 * v, P + 12 * v, x, e2) && e2 <= thr2;
+    if (in) m |= 1u << v;
+    cost += in ? e2 : thr2;
+  }
+  return m;
+}
+
+// the two-view DLT of hypothesis h (false: a view of the pair is not usable, or no finite point)
+__host__ __device__ inline bool robust_hypothesis(const double* u, const double* P, int V,
+                                                  unsigned usable, int h, double* x) {
+  int a, b;
+  robust_pair_of(h, V, a, b);
+  if (!((usable >> a) & 1u) || !((usable >> b) & 1u)) return false;
+  const double uu[4] = {u[2 * a], u[2 * a + 1], u[2 * b], u[2 * b + 1]};
+  double pp[24];
+  for (int k = 0; k < 12; ++k) { pp[k] = P[12 * a + k]; pp[12 + k] = P[12 * b + k]; }
+  return dlt_nview<2>(uu, pp, x) != 0;
+}
+
+// weighted DLT over the views of `mask` (a view outside it contributes two rows of zeros, which
+// change no sum of the Jacobi sweeps: with weights 1 and two views this is dlt_nview<2> bit for bit)
+template <int VM>
+__host__ __device__ inline bool dlt_masked(const double* u, const double* P, const double* w, int V,
+                                           unsigned mask, double* x) {
+  double A[2 * VM][4], Vm[4][4];
+  for (int v = 0; v < VM; ++v) {
+    const bool on = v < V && ((mask >> v) & 1u);
+    for (int k = 0; k < 4; ++k) {
+      A[2 * v + 0][k] = on ? w[v] * (u[v * 2 + 0] * P[v * 12 + 8 + k] - P[v * 12 + 0 + k]) : 0.0;
+      A[2 * v + 1][k] = on ? w[v] * (u[v * 2 + 1] * P[v * 12 + 8 + k] - P[v * 12 + 4 + k]) : 0.0;
+    }
+  }
+  jacobi_onesided<2 * VM, 4>(A, Vm);
+  int best = 0;
+  double bn = DBL_MAX, n2s[4], big = 0.0;
+  for (int j = 0; j < 4; ++j) {
+    double n2 = 0;
+    for (int i = 0; i < 2 * VM; ++i) n2 += A[i][j] * A[i][j];
+    n2s[j] = n2;
+    big = fmax(big, n2);
+    if (n2 < bn) { bn = n2; best = j; }
+  }
+  // rank 3 or the point is not determined (all rays the same line: identical cameras): the second
+  // smallest singular value must stand clear of rounding, sigma > 1e-10 sigma_max
+  double second = DBL_MAX;
+  for (int j = 0; j < 4; ++j)
+    if (j != best) second = fmin(second, n2s[j]);
+  if (!(second > 1e-20 * big)) return false;
+  double h[4];
+  for (int i = 0; i < 4; ++i) {
+    h[i] = Vm[i][0];
+    for (int j = 1; j < 4; ++j)
+      if (best == j) h[i] = Vm[i][j];
+  }
+  x[0] = h[0] / h[3]; x[1] = h[1] / h[3]; x[2] = h[2] / h[3];
+  const double mx = fmax(fabs(x[0]), fmax(fabs(x[1]), fabs(x[2])));
+  return isfinite(x[0]) && isfinite(x[1]) && isfinite(x[2]) && mx <= 1.e16;
+}
+
+// One (tuple, joint): u [V][2], P [V][12], w [V] (non-negative), 2 <= V <= RB_MAXV.
+template <class Red>
+__host__ __device__ void robust_point(const Red& red, const double* u, const double* P,
+                                      const double* w, int V, double thr, double* X, int32_t* inl,
+                                      double* resid, int32_t* status) {
+  const double thr2 = thr * thr;
+  unsigned usable = 0u;
+  for (int v = 0; v < V; ++v)
+    if (w[v] > 0.0 && isfinite(w[v]) && finite2(u + 2 * v)) usable |= 1u << v;
+  // 1. + 2.: lane l scores hypotheses l, l + n, ..; the best (count, cost, h) across the lanes
+  const int nh = V * (V - 1) / 2;
+  int bn = -1, bh = nh;
+  double bc = INFINITY;
+  for (int h = red.lane; h < nh; h += red.n) {
+    double x[3], c;
+    if (!robust_hypothesis(u, P, V, usable, h, x)) continue;
+    const int n = robust_count(robust_inliers(u, P, V, usable, x, thr2, c));
+    if (n > bn || (n == bn && c < bc)) { bn = n; bc = c; bh = h; }
+  }
+  red.best(bn, bc, bh);
+  // 3.: every lane repeats the (identical) refit, so `ok` is warp-uniform
+  bool ok = bn >= 2;
+  double x[3] = {0.0, 0.0, 0.0}, r = 0.0;
+  unsigned mask = 0u;
+  if (ok) {
+    double c;
+    robust_hypothesis(u, P, V, usable, bh, x);
+    mask = robust_inliers(u, P, V, usable, x, thr2, c);
+    auto refit = [&](unsigned m) {
+      return V <= 4 ? dlt_masked<4>(u, P, w, V, m, x) : dlt_masked<RB_MAXV>(u, P, w, V, m, x);
+    };
+    ok = refit(mask);
+    if (ok) {
+      const unsigned m1 = robust_inliers(u, P, V, usable, x, thr2, c);
+      if (m1 != mask) {
+        mask = m1;
+        ok = robust_count(m1) >= 2 && refit(m1);
+      }
+    }
+    if (ok) {                                              // 4.
+      double s2 = 0.0;
+      for (int v = 0; v < V; ++v) {
+        if (!((mask >> v) & 1u)) continue;
+        double e2;
+        robust_reproj2(u + 2 * v, P + 12 * v, x, e2);
+        s2 += e2;
+      }
+      r = sqrt(s2 / robust_count(mask));
+      ok = isfinite(r);
+    }
+  }
+  if (red.lane != 0) return;
+  for (int k = 0; k < 3; ++k) X[k] = ok ? x[k] : 0.0;
+  *inl = ok ? (int32_t)mask : 0;
+  *resid = ok ? r : 0.0;
+  *status = ok ? 1 : 0;
+}
+
+// u [NT][V][J][stride_u], P [NT][V][12], w [NT][V][J] or null (ones); one warp per (tuple, joint),
+// its views staged in shared memory (lanes >= V load no point, lanes stride over the V*12 entries of P)
+constexpr int kRobustWarps = 4;
+
+__global__ void __launch_bounds__(kRobustWarps * 32)
+triangulate_robust_kernel(const double* __restrict__ u, int stride_u, const double* __restrict__ P,
+                          const double* __restrict__ w, int NT, int V, int J, double thr,
+                          double* __restrict__ X, int32_t* __restrict__ inl,
+                          double* __restrict__ resid, int32_t* __restrict__ status) {
+  __shared__ double sP[kRobustWarps][RB_MAXV * 12], sU[kRobustWarps][RB_MAXV * 2],
+      sW[kRobustWarps][RB_MAXV];
+  const int wid = threadIdx.x >> 5;
+  const int64_t idx = (int64_t)blockIdx.x * kRobustWarps + wid;
+  if (idx >= (int64_t)NT * J) return;                      // warp-uniform
+  RbWarp red;
+  red.lane = threadIdx.x & 31;
+  const int64_t t = idx / J, j = idx - t * J;
+  for (int k = red.lane; k < V * 12; k += 32) sP[wid][k] = P[t * V * 12 + k];
+  if (red.lane < V) {
+    const int64_t o = (t * V + red.lane) * J + j;
+    sU[wid][2 * red.lane + 0] = u[o * stride_u + 0];
+    sU[wid][2 * red.lane + 1] = u[o * stride_u + 1];
+    sW[wid][red.lane] = w ? w[o] : 1.0;
+  }
+  __syncwarp();
+  robust_point(red, sU[wid], sP[wid], sW[wid], V, thr, X + idx * 3, inl + idx, resid + idx,
+               status + idx);
+}
+
 // --------------------------------------------------------------- argmax
 // inference.py:24-39: one warp per (n,j) map; (value, index) reduction with
 // smallest-index tie-break == numpy argmax first-occurrence.  NaN: numpy
@@ -1271,6 +1489,23 @@ extern "C" __attribute__((visibility("default"))) int epb_triangulate_nview(
   if (NT * J == 0) return EPB_OK;
   const int n = NT * J;
   triangulate_nview_kernel<<<(n + 63) / 64, 64, 0, as_stream(stream)>>>(u, stride_u, P, NT, V, J, X, status);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_triangulate_robust(
+    const double* u, int stride_u, const double* P, const double* w, int NT, int V, int J,
+    double threshold_px, double* X, int32_t* inliers, double* resid, int32_t* status,
+    epb_stream_t stream) {
+  EPB_CHECK_ARG(u && P && X && inliers && resid && status);
+  EPB_CHECK_ARG(NT >= 0 && J >= 0 && stride_u >= 2 && V >= 2 && V <= RB_MAXV);
+  EPB_CHECK_ARG(isfinite(threshold_px) && threshold_px > 0.0);
+  EPB_CHECK_ARG((int64_t)NT * J <= 0x7fffffff);
+  if ((int64_t)NT * J == 0) return EPB_OK;
+  const int64_t n = (int64_t)NT * J;
+  triangulate_robust_kernel<<<(unsigned)((n + kRobustWarps - 1) / kRobustWarps), kRobustWarps * 32, 0,
+                              as_stream(stream)>>>(u, stride_u, P, w, NT, V, J, threshold_px, X,
+                                                   inliers, resid, status);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

@@ -612,9 +612,10 @@ extern "C" __attribute__((visibility("default"))) int epb_softargmax_fwd(const f
   return EPB_OK;
 }
 
-extern "C" __attribute__((visibility("default"))) int epb_softargmax_flip_fwd(
-    const float* logits2N, int N, int J, int D, int H, int W, const int* perm_host, int shift,
-    float* coords, epb_stream_t stream) {
+// shared by the two flip-test entries; lse_ws may be null
+static int softargmax_flip_run(const float* logits2N, int N, int J, int D, int H, int W,
+                               const int* perm_host, int shift, float* coords, float* lse_ws,
+                               epb_stream_t stream) {
   EPB_CHECK_ARG(logits2N && perm_host && coords);
   EPB_CHECK_ARG(N > 0 && J > 0 && D > 0 && H > 0 && W > 0);
   EPB_CHECK_ARG(shift == 0 || shift == 1);
@@ -649,9 +650,22 @@ extern "C" __attribute__((visibility("default"))) int epb_softargmax_flip_fwd(
       logits2N, N, J, D, H, W, S, ppi, shift, pi, parts);
   EPB_LAUNCH_CHECK();
   softargmax_finalize<<<(NJ + 127) / 128, 128, 0, st>>>(parts, NJ, S, 1.f / W, 1.f / H, 1.f / D,
-                                                      coords, nullptr);
+                                                      coords, lse_ws);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_softargmax_flip_fwd(
+    const float* logits2N, int N, int J, int D, int H, int W, const int* perm_host, int shift,
+    float* coords, epb_stream_t stream) {
+  return softargmax_flip_run(logits2N, N, J, D, H, W, perm_host, shift, coords, nullptr, stream);
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_softargmax_flip_lse_fwd(
+    const float* logits2N, int N, int J, int D, int H, int W, const int* perm_host, int shift,
+    float* coords, float* lse_ws, epb_stream_t stream) {
+  EPB_CHECK_ARG(lse_ws);
+  return softargmax_flip_run(logits2N, N, J, D, H, W, perm_host, shift, coords, lse_ws, stream);
 }
 
 extern "C" __attribute__((visibility("default"))) int epb_softargmax_bwd(const float* logits, int layout, int N, int J, int D, int H,

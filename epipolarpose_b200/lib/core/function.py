@@ -457,3 +457,70 @@ def eval_integral(epoch, preds_in_patch_with_score, val_loader, final_output_pat
     for name, value in name_value:
         logger.info('Epoch[%d] Validation-%s %f', epoch, name, value)
     return perf
+
+
+def world_joints_of_record(rec):
+    """Ground-truth joints of one H36M record in the world frame [J, 3] (mm).  The records carry no
+    world-frame joints: `joints_3d` holds image x, y (px) and the depth relative to the pelvis (mm),
+    `pelvis` the camera-frame pelvis, `fl` / `c_p` the intrinsics.  They are back-projected to the
+    camera frame as the evaluation does (prep_h36m.py:85-89) and brought to the world frame with the
+    record's cam.R, cam.T: X = R^T X_cam + T, the inverse of the X_cam = R (X - T) that
+    epb_project_labels applies."""
+    j = np.asarray(rec['joints_3d'], dtype=np.float64)
+    fl = np.asarray(rec['fl'], dtype=np.float64).reshape(-1)
+    cp = np.asarray(rec['c_p'], dtype=np.float64).reshape(-1)
+    d = j[:, 2] + np.asarray(rec['pelvis'], dtype=np.float64).reshape(-1)[2]
+    xc = np.stack([(j[:, 0] - cp[0]) / fl[0] * d, (j[:, 1] - cp[1]) / fl[1] * d, d], axis=1)
+    R = np.asarray(rec['cam'].R, dtype=np.float64).reshape(3, 3)
+    T = np.asarray(rec['cam'].T, dtype=np.float64).reshape(1, 3)
+    return xc @ R + T
+
+
+def validate_multiview(dataset, predictor, tuples_per_batch=8):
+    """Multi-view inference over every view tuple of `dataset` (H36M_Integral.view_tuples()):
+    each frame is read and cropped through the dataset's sample path with augmentation off, the
+    views go through `predictor(images [T,V,3,H,W], boxes, P [T,V,3,4])` (a MultiViewPredictor) with
+    P from each record's cam.projection_matrix, and the triangulated pose is compared with the
+    ground truth in the world frame: world_joints_of_record of every view (see there for the
+    fields used), averaged over the views.
+
+    Returns a dict: mpjpe (mm, mean over the joints with status 1), inlier_views (mean number of
+    inlier views per joint, a failed joint counting 0), failed (share of joints with status 0),
+    tuples, and -- when the records carry `action` -- per_action: {action: the same three}."""
+    import copy
+    recs = [dataset.tuple_records(r) for r in dataset.view_tuples()]
+    was_train, dataset.is_train = dataset.is_train, False        # crop without augmentation
+    err, ninl, stat, acts = [], [], [], []
+    try:
+        for b in range(0, len(recs), max(1, int(tuples_per_batch))):
+            chunk = recs[b:b + max(1, int(tuples_per_batch))]
+            views = [[dataset.get_data(copy.deepcopy(r)) for r in tup] for tup in chunk]
+            images = np.stack([np.stack([v[0] for v in tup]) for tup in views]).astype(np.float32)
+            metas = [v[3] for tup in views for v in tup]
+            boxes = {k: np.array([float(m[k]) for m in metas])
+                     for k in ('center_x', 'center_y', 'width', 'height', 'scale', 'rot')}
+            P = np.stack([np.stack([np.asarray(v[3]['projection_matrix'], dtype=np.float64)[0:3, 0:4]
+                                    for v in tup]) for tup in views])
+            out = predictor(images, boxes, P)
+            gt = np.stack([np.mean([world_joints_of_record(r) for r in tup], axis=0) for tup in chunk])
+            err.append(np.linalg.norm(out['world'] - gt, axis=2))
+            stat.append(np.asarray(out['status']) != 0)
+            ninl.append(np.array([[bin(int(m)).count('1') for m in row] for row in out['inliers']]))
+            acts.extend(tup[0].get('action') for tup in chunk)
+    finally:
+        dataset.is_train = was_train
+    if not err:
+        return {'mpjpe': float('nan'), 'inlier_views': float('nan'), 'failed': float('nan'), 'tuples': 0}
+    err, stat, ninl = np.concatenate(err), np.concatenate(stat), np.concatenate(ninl)
+
+    def summary(sel):
+        e, s = err[sel], stat[sel]
+        return {'mpjpe': float(e[s].mean()) if s.any() else float('nan'),
+                'inlier_views': float(ninl[sel].mean()), 'failed': float(1.0 - s.mean())}
+
+    res = summary(np.ones(len(err), dtype=bool))
+    res['tuples'] = int(len(err))
+    if all(a is not None for a in acts):
+        acts = np.array(acts)
+        res['per_action'] = {str(a): summary(acts == a) for a in sorted(set(acts.tolist()))}
+    return res

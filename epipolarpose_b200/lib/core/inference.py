@@ -5,7 +5,9 @@ tie-break == numpy.argmax; indices are bit-exact).  numpy in / numpy out like
 the reference; `get_max_preds_device` is the tensor-in / tensor-out variant.
 
 Addition: `PosePredictor`, images -> 3-D joints as one CUDA-graph replay per call (the
-`model.eval(); get_joint_location_result(W, H, model(img))` of demo.ipynb and scripts/valid.py)."""
+`model.eval(); get_joint_location_result(W, H, model(img))` of demo.ipynb and scripts/valid.py).
+`MultiViewPredictor`: the calibrated views of a rig -> world-frame joints, the same network on
+every view followed by the robust V-view triangulation inside the same graph."""
 import numpy as np
 import torch
 
@@ -160,6 +162,10 @@ class PosePredictor:
         B = 2 * N if self.flip_test else N
         box = torch.tensor([[W / 2.0, H / 2.0, W, H, 1.0, 0.0]], dtype=torch.float64).repeat(N, 1)
         ent = {"x": torch.zeros((B, 3, H, W), device=self.dev), "box": box.to(self.dev)}
+        return self._record((N, H, W), ent)
+
+    def _record(self, key, ent):
+        """Warm up and capture self._forward(ent) as the graph of `key`."""
         cur = torch.cuda.current_stream(self.dev)
         # warm-up then capture on a side stream (GraphedTrainStep): the eager run sets the
         # kernels' one-time attributes and the geometry caches
@@ -172,7 +178,7 @@ class PosePredictor:
             self._forward(ent)
         cur.wait_stream(self.stream)
         ent["graph"] = graph
-        self.graphs[(N, H, W)] = ent
+        self.graphs[key] = ent
         return ent
 
     def __call__(self, images, boxes=None):
@@ -200,3 +206,108 @@ class PosePredictor:
             out = np.ones((N, J, 4), dtype=np.float64)
             out[:, :, :3] = ent["kps"][:, :, :3].cpu().numpy()
             return out
+
+
+class MultiViewPredictor(PosePredictor):
+    """Calibrated views of one person -> world-frame joints, one CUDA-graph replay per call: the
+    network on the T*V images (PosePredictor's engine, snapshot and refresh()), the soft-argmax
+    with its per-joint confidence, the patch -> image transform and the robust V-view
+    triangulation (epb_triangulate_robust), one graph per (T, V, H, W).  The boxes and the
+    projection matrices live in static device buffers that every call fills before the replay.
+
+    pred(images, boxes, P): images float32 [T, V, 3, H, W] (host or device), 2 <= V <= 8; boxes
+    holds center_x, center_y, width, height and optionally scale (default 1) and rot (default 0),
+    T*V values each in (tuple, view) order; P float64 [T, V, 3, 4] maps world coordinates to
+    original-image pixels.  Returns a dict of numpy arrays:
+      world   [T, J, 3]    float64, in the frame and unit of P (mm for Human3.6M); 0 where status is 0
+      kps     [T, V, J, 4] float64 per view: image x, y, root-relative z (mm), confidence
+      inliers [T, J]       int32 bit mask: bit v set <=> view v is in the final fit
+      resid   [T, J]       float64 RMS reprojection error (px) over the inlier views
+      status  [T, J]       int32 1 = triangulated from at least two agreeing views, else 0
+    The confidence is the peak softmax probability of the joint's volume (with flip test, of the
+    merged volume).  use_confidence: the confidences weigh the views in the refit (they never decide
+    which views agree).  threshold_px: the reprojection error, in original-image pixels, up to which
+    a view agrees with a hypothesis; the default is a guess that has not been tuned on real
+    predictions.  Constructor refusals as PosePredictor."""
+
+    def __init__(self, model, flip_test=None, shift_heatmap=None, flip_pairs=None, threshold_px=15.0,
+                 use_confidence=True):
+        if not (np.isfinite(threshold_px) and threshold_px > 0):
+            raise ValueError("threshold_px must be a positive number of pixels, got %r" % (threshold_px,))
+        super().__init__(model, flip_test, shift_heatmap, flip_pairs)
+        self.threshold_px = float(threshold_px)
+        self.use_confidence = bool(use_confidence)
+
+    def _forward(self, ent):
+        """The captured work: [flip,] network, soft-argmax + confidence, patch -> image, triangulation."""
+        from .integral_loss import get_joint_location_coords_peak, get_joint_location_coords_flip_peak
+        from ..utils.img_utils import patch_to_image_device
+        from ..utils.triangulation import triangulate_views_robust
+        x, box, P = ent["x"], ent["box"], ent["P"]
+        (T, V), N, H, W = P.shape[:2], box.shape[0], x.shape[2], x.shape[3]
+        if self.flip_test:
+            x[N:] = torch.flip(x[:N], [3])
+        logits, _, _ = self.eng.forward(x, None, training=False, save=False, prepared=self.state)
+        out = logits.permute(0, 3, 1, 2)
+        fin = self.eng.plan.final
+        if out.shape[1] != fin.cout:
+            out = out[:, :fin.cout]
+        if self.flip_test:
+            coords, peak = get_joint_location_coords_flip_peak(out, self.flip_pairs, self.shift_heatmap)
+        else:
+            coords, peak = get_joint_location_coords_peak(out)
+        kps = patch_to_image_device(coords, {"_packed": {"box": box}}, W, H, self.RECT_3D_W)
+        conf = peak.double()
+        kps[:, :, 3] = conf
+        J = kps.shape[1]
+        ent["logits"], ent["coords"], ent["kps"] = out, coords, kps
+        ent["w"] = conf.reshape(T, V, J).contiguous() if self.use_confidence else None
+        if "tri" not in ent:
+            ent["tri"] = (torch.empty((T, J, 3), device=self.dev, dtype=torch.float64),
+                          torch.empty((T, J), device=self.dev, dtype=torch.int32),
+                          torch.empty((T, J), device=self.dev, dtype=torch.int32),
+                          torch.empty((T, J), device=self.dev, dtype=torch.float64))
+        triangulate_views_robust(kps.view(T, V, J, 4), P, ent["w"], self.threshold_px, out=ent["tri"])
+
+    def __call__(self, images, boxes=None, P=None):
+        if boxes is None or P is None:
+            raise ValueError("MultiViewPredictor needs the boxes and the projection matrices of every view")
+        x = torch.as_tensor(images)
+        if x.dim() != 5 or x.shape[2] != 3:
+            raise ValueError("expected images [T, V, 3, H, W], got %s" % (tuple(x.shape),))
+        if x.dtype != torch.float32:
+            raise TypeError("expected float32 images, got %s" % x.dtype)
+        T, V, _, H, W = x.shape
+        if T < 1 or not 2 <= V <= 8:
+            raise ValueError("expected T >= 1 tuples of 2..8 views, got T = %d, V = %d" % (T, V))
+        Pm = torch.as_tensor(P)
+        if tuple(Pm.shape) != (T, V, 3, 4) or Pm.dtype != torch.float64:
+            raise ValueError("expected P float64 [%d, %d, 3, 4], got %s %s" % (T, V, Pm.dtype, tuple(Pm.shape)))
+        N = T * V
+        from ..utils.img_utils import _boxes
+        meta = {k: np.asarray(v, dtype=np.float64).reshape(-1) for k, v in dict(boxes).items()}
+        meta.setdefault("scale", np.ones(N))
+        meta.setdefault("rot", np.zeros(N))
+        for k in ("center_x", "center_y", "width", "height", "scale", "rot"):
+            if k not in meta or meta[k].size != N:
+                raise ValueError("boxes[%r] must hold T*V = %d values" % (k, N))
+        with torch.cuda.device(self.dev):
+            key = (T, V, H, W)
+            ent = self.graphs.get(key)
+            if ent is None:
+                B = 2 * N if self.flip_test else N
+                box0 = torch.tensor([[W / 2.0, H / 2.0, W, H, 1.0, 0.0]], dtype=torch.float64).repeat(N, 1)
+                ent = {"x": torch.zeros((B, 3, H, W), device=self.dev), "box": box0.to(self.dev),
+                       "P": torch.zeros((T, V, 3, 4), device=self.dev, dtype=torch.float64)}
+                ent["P"].copy_(Pm)             # the warm-up run sees real cameras
+                self._record(key, ent)
+            ent["x"][:N].copy_(x.reshape(N, 3, H, W), non_blocking=x.is_cuda)
+            ent["box"].copy_(_boxes(meta, N, torch.device("cpu")))
+            ent["P"].copy_(Pm)
+            ent["graph"].replay()
+            self.logits = ent["logits"]
+            X, status, inliers, resid = ent["tri"]
+            J = X.shape[1]
+            return {"world": X.cpu().numpy(), "kps": ent["kps"].cpu().numpy().reshape(T, V, J, 4),
+                    "inliers": inliers.cpu().numpy(), "resid": resid.cpu().numpy(),
+                    "status": status.cpu().numpy()}

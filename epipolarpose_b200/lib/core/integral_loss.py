@@ -396,6 +396,57 @@ def get_joint_location_coords_flip(preds2N, flip_pairs, shift_heatmap):
                                  shift_heatmap)
 
 
+def _coords_and_peak(preds, J, D, H, W):
+    """softmax_integral_tensor without autograd that keeps what the forward leaves in its lse
+    workspace: (coords [N, J*3], peak [N, J]), peak = 1 / sum exp(l - max) = the largest softmax
+    probability of the joint's volume."""
+    ops = _backend[0]
+    preds, layout = _layout_of(preds.detach(), J, D)
+    N = preds.shape[0]
+    coords = torch.empty((N, J * 3), device=preds.device, dtype=torch.float32)
+    lse = torch.empty((N * J * 2,), device=preds.device, dtype=torch.float32)
+    ops.softargmax_fwd(_storage(preds, layout), layout, N, J, D, H, W, coords, lse)
+    return coords, lse.view(N, J, 2)[:, :, 1]
+
+
+def get_joint_location_coords_peak(preds):
+    """get_joint_location_coords plus the per-joint confidence: (coords [N, J*3] float32,
+    peak [N, J] float32 in (0, 1], the peak softmax probability of each joint's volume)."""
+    if preds.dtype != torch.float32:
+        raise TypeError("get_joint_location_coords_peak expects float32 logits")
+    W, H = preds.shape[-1], preds.shape[-2]
+    D = W                                     # reference :191-192 assumes D == W
+    return _coords_and_peak(preds, preds.shape[1] // D, D, H, W)
+
+
+def get_joint_location_coords_flip_peak(preds2N, flip_pairs, shift_heatmap):
+    """get_joint_location_coords_flip plus the peak softmax probability of the MERGED volume:
+    (coords [N, J*3], peak [N, J]).  The fused pass is epb_softargmax_flip_lse_fwd."""
+    if preds2N.dtype != torch.float32:
+        raise TypeError("get_joint_location_coords_flip_peak expects float32 logits")
+    if preds2N.dim() != 4 or preds2N.shape[0] % 2:
+        raise ValueError("expected logits [2N, J*D, H, W], got %s" % (tuple(preds2N.shape),))
+    W, H = preds2N.shape[-1], preds2N.shape[-2]
+    D = W
+    J, N = preds2N.shape[1] // D, preds2N.shape[0] // 2
+    perm = flip_permutation(flip_pairs, J)
+    ops = _backend[0]
+    preds2N, layout = _layout_of(preds2N.detach(), J, D)
+    if layout == 1 and preds2N.data_ptr() % 16 == 0:
+        coords = torch.empty((N, J * 3), device=preds2N.device, dtype=torch.float32)
+        lse = torch.empty((N * J * 2,), device=preds2N.device, dtype=torch.float32)
+        ops.softargmax_flip_lse_fwd(_storage(preds2N, 1), N, J, D, H, W, perm, int(bool(shift_heatmap)),
+                                    coords, lse)
+        return coords, lse.view(N, J, 2)[:, :, 1]
+    with torch.no_grad():                      # as flip_merge_torch
+        v = preds2N.reshape(2 * N, J, D, H, W)
+        fb = v[N:].flip(-1)[:, perm]
+        if shift_heatmap:
+            fb = torch.cat([fb[..., :1], fb[..., :-1]], dim=-1)
+        merged = (0.5 * (v[:N] + fb)).reshape(N, J * D, H, W).contiguous()
+    return _coords_and_peak(merged, J, D, H, W)
+
+
 def get_joint_location_result_flip(patch_width, patch_height, preds2N, flip_pairs, shift_heatmap):
     """Flip-test form of get_joint_location_result: preds2N are the logits of [x; flip(x, 3)]
     (2N images) -> numpy float64 [N, J, 4] of the merged logits."""

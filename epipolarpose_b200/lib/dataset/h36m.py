@@ -56,7 +56,36 @@ class H36M_Integral(JointsIntegralDataset):
         return self.sample(image_file, the_db, joints_vis, the_db['flip_pairs'], the_db['parent_ids'], meta)
 
     def _load(self):
-        return load_pickle(os.path.join(self.root, 'annot', self.image_set + '.pkl'))
+        anno = load_pickle(os.path.join(self.root, 'annot', self.image_set + '.pkl'))
+        self._dict_form = isinstance(anno, dict)
+        return anno
+
+    def view_tuples(self):
+        """int array [T, V]: row k holds, camera by camera, the db indices that show frame k.
+        The dict-form annotation keeps one frame-aligned list per camera and _per_camera applies
+        one permutation to all of them, so in the validation db (flattened camera by camera) row
+        k is [cid * T + k for cid in range(NUM_CAMS)]; in the DATASET.TRI training db, which stays
+        per camera, entry [k, cid] indexes self.db[cid] (it is k).  tuple_records(row) returns the
+        records either way.  A list-form pickle, and the shuffled non-TRI training db, carry no
+        such alignment: ValueError."""
+        tri = self.is_train and self.cfg.DATASET.TRI
+        if not self._dict_form or (self.is_train and not tri):
+            raise ValueError("view_tuples needs frame-aligned cameras: a dict-form annotation pickle (one list "
+                             "per camera), read as the validation db or as the DATASET.TRI training db; a "
+                             "list-form pickle or a shuffled training db does not say which records show the "
+                             "same frame")
+        V = self.num_cams
+        if tri:
+            T = len(self.db[0])
+            return np.repeat(np.arange(T, dtype=np.int64)[:, None], V, axis=1)
+        T = len(self.db) // V
+        return np.arange(T, dtype=np.int64)[:, None] + T * np.arange(V, dtype=np.int64)[None, :]
+
+    def tuple_records(self, row):
+        """The V records of one row of view_tuples()."""
+        if self.is_train and self.cfg.DATASET.TRI:
+            return [self.db[cid][int(i)] for cid, i in enumerate(row)]
+        return [self.db[int(i)] for i in row]
 
     @staticmethod
     def _per_camera(anno, num_cams):

@@ -13,7 +13,10 @@ the homogeneous DLT) runs as method "polynomial" of the same kernel, including t
 re-estimated from the matches (cv2.findFundamentalMat FM_8POINT) on the device and the
 correction repeated; "polynomial_8point" runs that branch unconditionally.
 `relative_pose_pairs` estimates each pair's projection matrices from the 2-D joints alone
-(self-supervision without camera extrinsics)."""
+(self-supervision without camera extrinsics).
+`triangulate_views_robust` / `robust_nview_triangulation` (not in the reference) triangulate each
+joint of a calibrated rig of 2..8 views by consensus over the view pairs, leaving out and reporting
+the views that disagree (epb_triangulate_robust)."""
 import numpy as np
 import torch
 
@@ -58,6 +61,37 @@ def triangulate_views(u, P):
     if NT * J:
         ops.triangulate_nview(u.contiguous(), u.shape[3], P.reshape(NT, V, 12).contiguous(), NT, V, J, X, status)
     return X, status
+
+
+DEFAULT_THRESHOLD_PX = 15.0
+
+
+def triangulate_views_robust(u, P, weights=None, threshold_px=DEFAULT_THRESHOLD_PX, out=None):
+    """Robust V-view triangulation (2 <= V <= 8; epb_triangulate_robust, see include/epb.h):
+    u [NT,V,J,S>=2] float64 image px, P [NT,V,3,4] float64, weights [NT,V,J] float64 >= 0 or None
+    (ones; 0 = the view is absent for that joint), all on the device -> (X [NT,J,3] float64,
+    status [NT,J] int32, inliers [NT,J] int32 bit mask over the views, resid [NT,J] float64 RMS
+    reprojection error in px over the inlier views).  Joints with status 0 have X = 0, inliers = 0
+    and resid = 0.  `out`: the four result tensors to write into (for graph capture)."""
+    ops = _backend[0]
+    NT, V, J = u.shape[0], u.shape[1], u.shape[2]
+    if not 2 <= V <= 8:
+        raise ValueError("triangulate_views_robust handles 2..8 views per tuple, got %d" % V)
+    if not (np.isfinite(threshold_px) and threshold_px > 0):
+        raise ValueError("threshold_px must be a positive number of pixels, got %r" % (threshold_px,))
+    if weights is not None and tuple(weights.shape) != (NT, V, J):
+        raise ValueError("weights must be [NT, V, J] = %s, got %s" % ((NT, V, J), tuple(weights.shape)))
+    if out is None:
+        out = (torch.empty((NT, J, 3), device=u.device, dtype=torch.float64),
+               torch.empty((NT, J), device=u.device, dtype=torch.int32),
+               torch.empty((NT, J), device=u.device, dtype=torch.int32),
+               torch.empty((NT, J), device=u.device, dtype=torch.float64))
+    X, status, inliers, resid = out
+    if NT * J:
+        ops.triangulate_robust(u.contiguous(), u.shape[3], P.reshape(NT, V, 12).contiguous(),
+                               None if weights is None else weights.contiguous(), NT, V, J,
+                               threshold_px, X, inliers, resid, status)
+    return X, status, inliers, resid
 
 
 def relative_pose_pairs(kps, intr, box, rect3d_w=2000.0, diag=False):
@@ -124,3 +158,19 @@ def iterative_LS_triangulation(u1, P1, u2, P2, tolerance=3.e-5):
 def polynomial_triangulation(u1, P1, u2, P2):
     x, st = _run(u1, P1, u2, P2, "polynomial")
     return x.astype(output_dtype), st.astype(bool)
+
+
+def robust_nview_triangulation(us, Ps, weights=None, threshold_px=DEFAULT_THRESHOLD_PX):
+    """One tuple of a calibrated rig, numpy in / numpy out: us [V,J,>=2], Ps [V,>=3,4], weights [V,J]
+    or None -> (x [J,3] of output_dtype, status [J] bool, inliers [J] int bit mask over the views,
+    resid [J] px).  See triangulate_views_robust.  The default threshold, in original-image pixels,
+    is a guess: it has not been tuned on real predictions."""
+    us = np.ascontiguousarray(us, dtype=np.float64)
+    assert us.ndim == 3 and us.shape[2] >= 2
+    dev = _device()
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a, dtype=np.float64)).to(dev)
+    P = np.stack([np.asarray(p, dtype=np.float64)[0:3, 0:4] for p in Ps])
+    X, st, inl, res = triangulate_views_robust(t(us)[None], t(P)[None],
+                                               None if weights is None else t(weights)[None], threshold_px)
+    return (X[0].cpu().numpy().astype(output_dtype), st[0].cpu().numpy().astype(bool),
+            inl[0].cpu().numpy().astype(int), res[0].cpu().numpy())

@@ -17,7 +17,7 @@ launches = 0
 
 # kernels launched per C-ABI call (for the gpu_launches accounting)
 _KERNELS_PER_CALL = {
-    "epb_softargmax_fwd": 2, "epb_softargmax_flip_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
+    "epb_softargmax_fwd": 2, "epb_softargmax_flip_fwd": 2, "epb_softargmax_flip_lse_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
     "epb_split16_batch": 3, "epb_split16": 3, "epb_bn_bwd_apply_split": 2, "epb_conv16_wgrad": 2,
     "epb_bn_bwd_reduce_mx": 2, "epb_bn_bwd_split": 3, "epb_softargmax_bwd_split": 3,
     "epb_patch_sample": 2, "epb_patch_sample_occ": 2, "epb_jpeg_decode": 14,
@@ -322,6 +322,15 @@ def softargmax_flip_fwd(logits2N, N, J, D, H, W, perm, shift, coords):
     _call("epb_softargmax_flip_fwd", _p(logits2N), N, J, D, H, W, pi, int(shift), _p(coords), _stream())
 
 
+def softargmax_flip_lse_fwd(logits2N, N, J, D, H, W, perm, shift, coords, lse):
+    """softargmax_flip_fwd that also writes lse [N*J*2] = (max, 1 / sum exp) of the merged volume."""
+    if len(perm) != J:
+        raise _lib.EpbError("perm has %d entries, expected J = %d" % (len(perm), J))
+    pi = (ctypes.c_int * J)(*[int(v) for v in perm])
+    _call("epb_softargmax_flip_lse_fwd", _p(logits2N), N, J, D, H, W, pi, int(shift), _p(coords), _p(lse),
+          _stream())
+
+
 def jointloss(x, t, w, n, kind, norm, div, loss, dx):
     _call("epb_jointloss_fwd_bwd", _p(x), _p(t), _p(w), n, kind, int(norm), float(div),
           _p(loss), _p(dx), _stream())
@@ -469,6 +478,12 @@ def kmeans_assign(x, N, d, centroids, k, labels, dist2):
 def triangulate_nview(u, stride_u, P, NT, V, J, X, status):
     _call("epb_triangulate_nview", _p(u, torch.float64), stride_u, _p(P, torch.float64), NT, V, J,
           _p(X, torch.float64), _p(status, torch.int32), _stream())
+
+
+def triangulate_robust(u, stride_u, P, w, NT, V, J, threshold_px, X, inliers, resid, status):
+    _call("epb_triangulate_robust", _p(u, torch.float64), stride_u, _p(P, torch.float64),
+          _p(w, torch.float64), NT, V, J, float(threshold_px), _p(X, torch.float64),
+          _p(inliers, torch.int32), _p(resid, torch.float64), _p(status, torch.int32), _stream())
 
 
 def relative_pose(u, stride_u, intr, box, B, J, rect3d_w, Pa, Pb, cam, inliers, status, diag=None):

@@ -366,6 +366,12 @@ int epb_softargmax_bwd_split(const float* logits, int N, int J, int D, int H, in
  * J*D/4 <= 1024 and a 16-byte aligned logits2N (EPB_EINVAL otherwise).  No lse, no backward. */
 int epb_softargmax_flip_fwd(const float* logits2N, int N, int J, int D, int H, int W,
                             const int* perm_host, int shift, float* coords, epb_stream_t stream);
+/* epb_softargmax_flip_fwd that also writes lse_ws [N*J*2] = (max, 1 / sum exp(l - max)) of the
+ * merged volume, as epb_softargmax_fwd does: the second entry is the peak softmax probability of
+ * joint j, the confidence of multi-view inference.  Same checks; coords bit-identical. */
+int epb_softargmax_flip_lse_fwd(const float* logits2N, int N, int J, int D, int H, int W,
+                                const int* perm_host, int shift, float* coords, float* lse_ws,
+                                epb_stream_t stream);
 
 /* Fused joint-location loss (integral_loss.py:7-47): kind 0 = weighted MSE,
  * 1 = weighted L1, 2 = weighted SmoothL1(beta=1).  loss = sum(w*l(x-t))/div,
@@ -438,6 +444,24 @@ int epb_triangulate(const double* u1, const double* u2, int stride_u,
  * 2 <= V <= 4 -> X [NT][J][3], status [NT][J] (max |coordinate| <= 1e16). */
 int epb_triangulate_nview(const double* u, int stride_u, const double* P, int NT, int V, int J,
                           double* X, int32_t* status, epb_stream_t stream);
+/* Robust V-view triangulation on a calibrated rig, 2 <= V <= 8 (not in the reference): per
+ * (tuple, joint) the two-view DLT of every pair of usable views, in the order (0,1), (0,2), ..,
+ * (V-2,V-1), is scored by its inlier views (in front of the camera, reprojection error <=
+ * threshold_px) -- most inliers, then the lowest MSAC cost sum(inlier ? e^2 : thr^2), then the
+ * lowest pair index -- and the winner's inlier views are refitted by a DLT with rows scaled by the
+ * weights; the inlier set is taken once more against the refit and the fit repeated if it changed.
+ * u [NT][V][J][stride_u] f64 (first two entries used), P [NT][V][12] f64 with a third row that is
+ * positive in front of the camera (K [R|t]), w [NT][V][J] f64 non-negative or NULL (ones).  A view
+ * with weight 0 (or a non-finite weight or image point) is absent for that joint: the result is
+ * that of the tuple without it.  X [NT][J][3]; inliers [NT][J] bit v set <=> view v is in the
+ * final fit; resid [NT][J] RMS reprojection error (px) over those views; status [NT][J] 1 = at
+ * least two inlier views, a refit system of rank 3 (second smallest singular value > 1e-10 of the
+ * largest: the rays are not one line) and finite coordinates with |x| <= 1e16, else 0 with X = 0,
+ * inliers = 0, resid = 0 (no NaN or Inf is ever written).  Deterministic.  EPB_EINVAL: V outside 2..8,
+ * stride_u < 2, a negative size, NT*J > 2^31-1, threshold_px not finite or <= 0. */
+int epb_triangulate_robust(const double* u, int stride_u, const double* P, const double* w, int NT,
+                           int V, int J, double threshold_px, double* X, int32_t* inliers,
+                           double* resid, int32_t* status, epb_stream_t stream);
 /* Relative pose of each view pair from its own 2-D joints, for self-supervision without camera
  * extrinsics.  Stands in for what the reference only sketches in lib/utils/cameras.py:133-143
  * (Camera.get_essential_matrix = K2^T F K1, get_fundamental_matrix with cv2.FM_LMEDS; no caller):
