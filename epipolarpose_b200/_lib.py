@@ -66,6 +66,12 @@ _PROTOS = {
                                   c_p]),
     "epb_project_labels": (c_int, [c_p, c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_p, c_p, c_p]),
     "epb_h36m_eval": (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, ctypes.c_uint32, c_d, c_p, c_p, c_p, c_p, c_p]),
+    "epb_pose_errors": (c_int, [c_p, c_p, c_int, c_int, ctypes.c_uint32, c_p, c_p, c_p]),
+    "epb_pose_to_camera": (c_int, [c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
+    "epb_refiner_sizes": (c_int, [c_int, c_int, c_int, c_int, ctypes.POINTER(c_i64), ctypes.POINTER(c_i64)]),
+    "epb_refiner_prepare": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_p), c_f, c_p, c_p]),
+    "epb_refiner_forward": (c_int, [c_int, c_int, c_int, c_p, c_p, c_int, c_int, c_int, c_p, c_p, c_i64, c_int,
+                                    c_p]),
     "epb_pose_normalize": (c_int, [c_p, c_p, c_int, c_int, c_int, c_p, c_p]),
     "epb_kmeans_workspace": (c_int, [c_int, c_int, c_int, ctypes.POINTER(c_i64)]),
     "epb_kmeans_fit": (c_int, [c_p, c_int, c_int, c_int, ctypes.c_uint64, c_int, c_int, c_p, c_p, c_p, c_p, c_p,

@@ -677,32 +677,27 @@ __global__ void project_labels_kernel(const double* __restrict__ X, const double
 }
 
 // --------------------------------------------------------------- evaluation (H36M protocol)
-// lib/dataset/h36m.py:168-378 per sample: back-projection of image-space joints
-// (lib/utils/prep_h36m.py:85-89), similarity (Procrustes) alignment with optimal scale
-// (:108-168, numpy SVD there; here the one-sided Jacobi on the 3x3 covariance -- V*U^T does
-// not depend on the ordering / paired signs of the singular triplets), root alignment and
-// the nine protocol means.  One thread per sample, float64, J <= 32.
-//   metrics[s] = { e, e_align, e_norm, e14, e14_align, e14_norm, ex, ey, ez }   (means over joints)
-// (also compiled for the host: tests/harness/host_geometry.cu runs this exact code on the CPU)
-__host__ __device__ void h36m_eval_sample(const double* p, const double* q, const double* cam,
-                                          int J, int root, unsigned j14mask, double pck_thr,
-                                          double* metrics, double* per_joint, int32_t* pck,
-                                          double* poses) {
-  // back projection (h36m.py:228-240): X = gt (targets), Y = prediction (inputs)
-  auto bp = [&](const double* a, int j, double (&o)[3]) { cam_back_proj(a, j, cam, o); };
+// compute_similarity_transform(X, Y, compute_optimal_scale=True) (lib/utils/prep_h36m.py:108-168,
+// numpy SVD there; here the one-sided Jacobi on the 3x3 covariance -- V*U^T does not depend on the
+// ordering / paired signs of the singular triplets): X (targets) ~ b * Y (inputs) * T + c.
+// X(j, o) / Y(j, o) write joint j of each pose into o[3]; they are called again for every pass
+// over the joints, so a back-projecting caller never stores the camera-frame poses.
+template <class GetX, class GetY>
+__host__ __device__ inline void similarity_transform(int J, GetX X, GetY Y, double (&T)[3][3], double& bsc,
+                                                     double (&cvec)[3]) {
   double muX[3] = {0, 0, 0}, muY[3] = {0, 0, 0};
   for (int j = 0; j < J; ++j) {
     double x[3], y[3];
-    bp(q, j, x);
-    bp(p, j, y);
+    X(j, x);
+    Y(j, y);
     for (int k = 0; k < 3; ++k) { muX[k] += x[k]; muY[k] += y[k]; }
   }
   for (int k = 0; k < 3; ++k) { muX[k] /= J; muY[k] /= J; }
   double ssX = 0, ssY = 0;
   for (int j = 0; j < J; ++j) {
     double x[3], y[3];
-    bp(q, j, x);
-    bp(p, j, y);
+    X(j, x);
+    Y(j, y);
     for (int k = 0; k < 3; ++k) {
       const double a = x[k] - muX[k], b = y[k] - muY[k];
       ssX += a * a;
@@ -713,8 +708,8 @@ __host__ __device__ void h36m_eval_sample(const double* p, const double* q, cons
   double A[3][3] = {{0, 0, 0}, {0, 0, 0}, {0, 0, 0}};     // X0^T Y0 (unit Frobenius norm each)
   for (int j = 0; j < J; ++j) {
     double x[3], y[3];
-    bp(q, j, x);
-    bp(p, j, y);
+    X(j, x);
+    Y(j, y);
     for (int a = 0; a < 3; ++a)
       for (int b = 0; b < 3; ++b)
         A[a][b] += ((x[a] - muX[a]) / normX) * ((y[b] - muY[b]) / normY);
@@ -735,7 +730,6 @@ __host__ __device__ void h36m_eval_sample(const double* p, const double* q, cons
     U[1][jmin] = U[2][a] * U[0][b] - U[0][a] * U[2][b];
     U[2][jmin] = U[0][a] * U[1][b] - U[1][a] * U[0][b];
   }
-  double T[3][3];
   auto make_T = [&]() {
     for (int r = 0; r < 3; ++r)
       for (int c = 0; c < 3; ++c)
@@ -750,10 +744,25 @@ __host__ __device__ void h36m_eval_sample(const double* p, const double* q, cons
   sg[jmin] *= sgn;
   make_T();
   const double trace = sg[0] + sg[1] + sg[2];
-  const double bsc = trace * normX / normY;                    // optimal scale
-  double cvec[3];
+  bsc = trace * normX / normY;                                 // optimal scale
   for (int c = 0; c < 3; ++c)
     cvec[c] = muX[c] - bsc * (muY[0] * T[0][c] + muY[1] * T[1][c] + muY[2] * T[2][c]);
+}
+
+// lib/dataset/h36m.py:168-378 per sample: back-projection of image-space joints
+// (lib/utils/prep_h36m.py:85-89), similarity alignment with optimal scale, root alignment and
+// the nine protocol means.  One thread per sample, float64, J <= 32.
+//   metrics[s] = { e, e_align, e_norm, e14, e14_align, e14_norm, ex, ey, ez }   (means over joints)
+// (also compiled for the host: tests/harness/host_geometry.cu runs this exact code on the CPU)
+__host__ __device__ void h36m_eval_sample(const double* p, const double* q, const double* cam,
+                                          int J, int root, unsigned j14mask, double pck_thr,
+                                          double* metrics, double* per_joint, int32_t* pck,
+                                          double* poses) {
+  // back projection (h36m.py:228-240): X = gt (targets), Y = prediction (inputs)
+  auto bp = [&](const double* a, int j, double (&o)[3]) { cam_back_proj(a, j, cam, o); };
+  double T[3][3], bsc, cvec[3];
+  similarity_transform(J, [&](int j, double (&o)[3]) { bp(q, j, o); },
+                       [&](int j, double (&o)[3]) { bp(p, j, o); }, T, bsc, cvec);
   // root joint of each variant (h36m.py:247-251)
   double xr[3], yr[3], yar[3], ynr[3];
   bp(q, root, xr);
@@ -809,6 +818,69 @@ __global__ void h36m_eval_kernel(const double* __restrict__ pred, const double* 
                    per_joint ? per_joint + (int64_t)s * J : nullptr,
                    pck ? pck + (int64_t)s * J : nullptr,
                    poses ? poses + (int64_t)s * J * 9 : nullptr);
+}
+
+// Per-sample errors of camera-frame poses (the refiner's evaluate, refiner/data.py:78-160 of the
+// reference): no back-projection and no root alignment; X = gt, Y = pred.  float64, J <= 32.
+//   metrics[7] = { e, e_align, e_sub, e_align_sub, |dx|, |dy|, |dz| }   (means over joints)
+// (also compiled for the host: tests/harness/host_pose_eval.cu)
+__host__ __device__ void pose_errors_sample(const double* p, const double* q, int J, unsigned submask,
+                                            double* metrics, double* per_joint) {
+  double T[3][3], bsc, cvec[3];
+  auto at = [](const double* a) {
+    return [a](int j, double (&o)[3]) { o[0] = a[j * 3]; o[1] = a[j * 3 + 1]; o[2] = a[j * 3 + 2]; };
+  };
+  similarity_transform(J, at(q), at(p), T, bsc, cvec);
+  double m[7] = {0, 0, 0, 0, 0, 0, 0};
+  int nsub = 0;
+  for (int j = 0; j < J; ++j) {
+    const double* x = q + j * 3;
+    const double* y = p + j * 3;
+    double d[3], da[3];
+    for (int c = 0; c < 3; ++c) {
+      const double ya = bsc * (y[0] * T[0][c] + y[1] * T[1][c] + y[2] * T[2][c]) + cvec[c];
+      d[c] = x[c] - y[c];
+      da[c] = x[c] - ya;
+    }
+    const double e = sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]);
+    const double ea = sqrt(da[0] * da[0] + da[1] * da[1] + da[2] * da[2]);
+    m[0] += e; m[1] += ea;
+    if ((submask >> j) & 1u) { m[2] += e; m[3] += ea; ++nsub; }
+    m[4] += fabs(d[0]); m[5] += fabs(d[1]); m[6] += fabs(d[2]);
+    if (per_joint) per_joint[j] = e;
+  }
+  for (int k = 0; k < 7; ++k) {
+    const int div = (k == 2 || k == 3) ? (nsub > 0 ? nsub : 1) : J;
+    metrics[k] = m[k] / div;
+  }
+}
+
+__global__ void pose_errors_kernel(const double* __restrict__ pred, const double* __restrict__ gt, int S, int J,
+                                   unsigned submask, double* __restrict__ metrics,
+                                   double* __restrict__ per_joint) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= S) return;
+  pose_errors_sample(pred + (int64_t)s * J * 3, gt + (int64_t)s * J * 3, J, submask, metrics + (int64_t)s * 7,
+                     per_joint ? per_joint + (int64_t)s * J : nullptr);
+}
+
+// Root-relative camera-frame pose of image-space joints: the `pred` column of h36m_eval_sample's
+// poses, with the same arithmetic (CamBackProj of joint j minus CamBackProj of the root).
+__host__ __device__ void pose_to_camera_sample(const double* a, const double* cam, int J, int root, double* out) {
+  double r[3];
+  cam_back_proj(a, root, cam, r);
+  for (int j = 0; j < J; ++j) {
+    double y[3];
+    cam_back_proj(a, j, cam, y);
+    for (int c = 0; c < 3; ++c) out[j * 3 + c] = y[c] - r[c];
+  }
+}
+
+__global__ void pose_to_camera_kernel(const double* __restrict__ joints, const double* __restrict__ cam, int N,
+                                      int J, int root, double* __restrict__ out) {
+  const int s = blockIdx.x * blockDim.x + threadIdx.x;
+  if (s >= N) return;
+  pose_to_camera_sample(joints + (int64_t)s * J * 3, cam + (int64_t)s * 5, J, root, out + (int64_t)s * J * 3);
 }
 
 // --------------------------------------------------------------- relative pose (no extrinsics)
@@ -1477,6 +1549,27 @@ extern "C" __attribute__((visibility("default"))) int epb_h36m_eval(
   h36m_eval_kernel<<<(S + 63) / 64, 64, 0, as_stream(stream)>>>(pred, gt, cam, S, J, root, j14mask,
                                                                pck_thr, metrics, per_joint, pck,
                                                                poses);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_pose_errors(
+    const double* pred, const double* gt, int S, int J, uint32_t submask, double* metrics, double* per_joint,
+    epb_stream_t stream) {
+  EPB_CHECK_ARG(pred && gt && metrics);
+  EPB_CHECK_ARG(S >= 0 && J > 0 && J <= 32);
+  if (S == 0) return EPB_OK;
+  pose_errors_kernel<<<(S + 63) / 64, 64, 0, as_stream(stream)>>>(pred, gt, S, J, submask, metrics, per_joint);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_pose_to_camera(
+    const double* joints, const double* cam, int N, int J, int root, double* out, epb_stream_t stream) {
+  EPB_CHECK_ARG(joints && cam && out);
+  EPB_CHECK_ARG(N >= 0 && J > 0 && root >= 0 && root < J);
+  if (N == 0) return EPB_OK;
+  pose_to_camera_kernel<<<(N + 63) / 64, 64, 0, as_stream(stream)>>>(joints, cam, N, J, root, out);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

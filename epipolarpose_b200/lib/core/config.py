@@ -12,7 +12,9 @@ extrinsics: each view pair's pose is estimated from its 2-D joints; needs
 TRAIN.ONLINE_TRIANGULATION, ValueError otherwise), TRAIN.CUDA_GRAPH (default on),
 MODEL.PRECISION, DATASET.SYNTHETIC_LEN, TEST.PSS_K (list of k: the H36M evaluation appends
 PSS@k, lib/core/pss.py; default []), TEST.PSS_CENTROIDS (.npz of `k<k>` centroids used instead
-of fitting them on train-fs; default '').
+of fitting them on train-fs; default ''), TEST.REFINER (a refiner checkpoint: the H36M evaluation
+also refines its poses and appends the Refined-* entries, lib/core/refine.py; default '') and
+TEST.REFINER_NORM (the refiner's norm.pkl, required with TEST.REFINER).
 """
 import os
 
@@ -68,7 +70,8 @@ _DEFAULTS = dict(
                CUDA_GRAPH=True),
     TEST=dict(BATCH_SIZE=32, FLIP_TEST=False, POST_PROCESS=True, SHIFT_HEATMAP=True,
               USE_GT_BBOX=False, OKS_THRE=0.5, IN_VIS_THRE=0.0, COCO_BBOX_FILE='', BBOX_THRE=1.0,
-              MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0, PSS_K=[], PSS_CENTROIDS=''),
+              MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0, PSS_K=[], PSS_CENTROIDS='',
+              REFINER='', REFINER_NORM=''),
     DEBUG=dict(DEBUG=False, SAVE_BATCH_IMAGES_GT=False, SAVE_BATCH_IMAGES_PRED=False,
                SAVE_HEATMAPS_GT=False, SAVE_HEATMAPS_PRED=False, SAVE_3D=False),
 )

@@ -36,6 +36,7 @@ from ..utils.img_utils import (self_supervision_device,
 from .integral_loss import get_joint_location_coords_flip, get_result_func, joint_location_result_from_coords
 from ..utils.utils import AverageMeter
 from ..dataset.deferred import assemble_batch, cat_meta, is_deferred
+from .refine import export_refiner_pairs  # noqa: F401  (public here, next to eval_integral)
 
 logger = logging.getLogger(__name__)
 

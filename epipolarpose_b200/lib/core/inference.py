@@ -7,7 +7,9 @@ the reference; `get_max_preds_device` is the tensor-in / tensor-out variant.
 Addition: `PosePredictor`, images -> 3-D joints as one CUDA-graph replay per call (the
 `model.eval(); get_joint_location_result(W, H, model(img))` of demo.ipynb and scripts/valid.py).
 `MultiViewPredictor`: the calibrated views of a rig -> world-frame joints, the same network on
-every view followed by the robust V-view triangulation inside the same graph."""
+every view followed by the robust V-view triangulation inside the same graph.
+`RefinedPosePredictor`: images, boxes and cameras -> camera-frame poses and their refinement by the
+paper's refinement unit, in one graph."""
 import numpy as np
 import torch
 
@@ -311,3 +313,82 @@ class MultiViewPredictor(PosePredictor):
             return {"world": X.cpu().numpy(), "kps": ent["kps"].cpu().numpy().reshape(T, V, J, 4),
                     "inliers": inliers.cpu().numpy(), "resid": resid.cpu().numpy(),
                     "status": status.cpu().numpy()}
+
+
+class RefinedPosePredictor(PosePredictor):
+    """Images -> refined camera-frame 3-D poses, one CUDA-graph replay per (N, H, W): the
+    PosePredictor graph (network, soft-argmax, patch -> image), then epb_pose_to_camera (the
+    root-relative camera-frame pose, bit-identical to the `pred` column of the H36M evaluation) and
+    epb_refiner_forward (refiner.model.Refiner: the hip dropped, the second head denormalised, the
+    hip put back at 0).
+
+    refiner: a refiner.model.LinearModelPG; norm: (data_mean, data_std, labels_mean, labels_std) of
+    its norm.pkl.  Both the network and the refiner are snapshots: refresh() re-reads both.
+    pred(images, boxes, cams): images float32 [N, 3, H, W]; boxes as PosePredictor; cams holds, per
+    image, fl [N, 2], c_p [N, 2] and the root (pelvis) depth `depth` [N] in mm, which must be given
+    as in the H36M protocol (it is not estimated).  Returns a dict of numpy arrays:
+      kps     [N, 16, 4] float64  PosePredictor's output with boxes (image x, y, root-relative z, 1)
+      pose    [N, 16, 3] float64  camera-frame mm, root-relative (MPII order, root = joint 6)
+      refined [N, 16, 3] float32  the refiner's output, hip at 0
+    Constructor refusals: those of PosePredictor, and a network of other than 16 joints."""
+
+    ROOT = 6
+
+    def __init__(self, model, refiner, norm, flip_test=None, shift_heatmap=None, flip_pairs=None):
+        from refiner.model import Refiner
+        net = getattr(model, "module", model)
+        super().__init__(model, flip_test, shift_heatmap, flip_pairs)
+        if net._plan.num_joints != 16:
+            raise ValueError("RefinedPosePredictor refines 16-joint poses in MPII order, the network has %d "
+                             "joints" % net._plan.num_joints)
+        self.refiner = Refiner(refiner, norm, device=self.dev)
+
+    def refresh(self):
+        super().refresh()
+        if getattr(self, "refiner", None) is not None:
+            self.refiner.refresh()
+
+    def _forward(self, ent):
+        super()._forward(ent)
+        N = ent["box"].shape[0]
+        kps = ent["kps"][:, :, :3].contiguous()
+        _ops.pose_to_camera(kps, ent["cam"], N, 16, self.ROOT, ent["pose"])
+        if "ws" not in ent:                 # allocated by the warm-up run, before the capture
+            ent["ws"] = self.refiner.workspace(N)
+        ent["refined"] = self.refiner.refine(ent["pose"], ws=ent["ws"])
+
+    def __call__(self, images, boxes=None, cams=None):
+        if boxes is None or cams is None:
+            raise ValueError("RefinedPosePredictor needs the boxes and the cameras (fl, c_p, depth) of every image")
+        x = torch.as_tensor(images)
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError("expected images [N, 3, H, W], got %s" % (tuple(x.shape),))
+        if x.dtype != torch.float32:
+            raise TypeError("expected float32 images, got %s" % x.dtype)
+        N, _, H, W = x.shape
+        fl = np.asarray(cams["fl"], dtype=np.float64).reshape(N, -1)[:, :2]
+        cp = np.asarray(cams["c_p"], dtype=np.float64).reshape(N, -1)[:, :2]
+        depth = np.asarray(cams["depth"], dtype=np.float64).reshape(N, 1)
+        cam = torch.from_numpy(np.ascontiguousarray(np.concatenate([fl, cp, depth], axis=1)))
+        from ..utils.img_utils import _boxes
+        meta = dict(boxes)
+        meta.setdefault("scale", np.ones(N))
+        meta.setdefault("rot", np.zeros(N))
+        with torch.cuda.device(self.dev):
+            key = (N, H, W)
+            ent = self.graphs.get(key)
+            if ent is None:
+                B = 2 * N if self.flip_test else N
+                ent = {"x": torch.zeros((B, 3, H, W), device=self.dev),
+                       "box": _boxes(meta, N, torch.device("cpu")).to(self.dev),
+                       "cam": cam.to(self.dev),
+                       "pose": torch.empty((N, 16, 3), device=self.dev, dtype=torch.float64)}
+                self._record(key, ent)
+            ent["x"][:N].copy_(x, non_blocking=x.is_cuda)
+            ent["box"].copy_(_boxes(meta, N, torch.device("cpu")))
+            ent["cam"].copy_(cam)
+            ent["graph"].replay()
+            self.logits = ent["logits"]
+            kps = np.ones((N, 16, 4), dtype=np.float64)
+            kps[:, :, :3] = ent["kps"][:, :, :3].cpu().numpy()
+            return {"kps": kps, "pose": ent["pose"].cpu().numpy(), "refined": ent["refined"].cpu().numpy()}

@@ -9,7 +9,8 @@ cam_config (random) and returns {'cam_1': view, 'cam_2': view} of the same frame
 A view is the reference's (img_patch, label, label_weight, meta) in the main process and a
 deferred sample in a DataLoader worker (JointIntegralDataset.sample).  `evaluate` runs the H36M
 protocol through evaluate_h36m (epb_h36m_eval) and, for each k of TEST.PSS_K, appends PSS@k
-(lib/core/pss.py); the DEBUG.DEBUG plots are not built."""
+(lib/core/pss.py), and with TEST.REFINER the four Refined-* entries of the refined poses
+(lib/core/refine.py); the DEBUG.DEBUG plots are not built."""
 import copy
 import logging
 import os
@@ -20,6 +21,7 @@ import numpy as np
 from .JointIntegralDataset import JointsIntegralDataset, H36M_NAMES, MPII_NAMES, load_pickle
 from .h36m_eval import evaluate_h36m
 from ..core.pss import h36m_pss
+from ..core.refine import check_refiner_config, h36m_refined
 from ..utils.data_utils import define_actions
 
 logger = logging.getLogger(__name__)
@@ -131,13 +133,17 @@ class H36M_Integral(JointsIntegralDataset):
             if S else np.zeros((0, 3))
         mpii = bool(self.cfg.DATASET.MPII_ORDER)
         gt = np.stack([np.asarray(g['joints_3d'], dtype=np.float64) for g in gts]) if S else np.zeros((0, 17, 3))
-        name_value, perf, details = evaluate_h36m(preds, gt, get('pelvis'), get('fl'), get('c_p'), mpii_order=mpii)
         test = getattr(self.cfg, 'TEST', None)
+        refiner = check_refiner_config(test, mpii, preds.shape[1])
+        name_value, perf, details = evaluate_h36m(preds, gt, get('pelvis'), get('fl'), get('c_p'), mpii_order=mpii,
+                                                  return_poses=refiner is not None)
         pss_k = list(getattr(test, 'PSS_K', None) or [])
         if pss_k:
             name_value = name_value + h36m_pss(preds, gt, get('pelvis'), get('fl'), get('c_p'), mpii, pss_k,
                                                os.path.join(self.root, 'annot', 'train-fs.pkl'),
                                                getattr(test, 'PSS_CENTROIDS', ''))
+        if refiner is not None:
+            name_value = name_value + h36m_refined(details['poses'], *refiner)
         per_joint_error = details['per_joint'].mean(axis=0).tolist()
         for name, err in zip(MPII_NAMES if mpii else H36M_NAMES, per_joint_error):
             print(name, err)

@@ -20,7 +20,7 @@ _KERNELS_PER_CALL = {
     "epb_softargmax_fwd": 2, "epb_softargmax_flip_fwd": 2, "epb_softargmax_flip_lse_fwd": 2, "epb_bn_bwd_apply": 2, "epb_colsum": 3,
     "epb_split16_batch": 3, "epb_split16": 3, "epb_bn_bwd_apply_split": 2, "epb_conv16_wgrad": 2,
     "epb_bn_bwd_reduce_mx": 2, "epb_bn_bwd_split": 3, "epb_softargmax_bwd_split": 3,
-    "epb_patch_sample": 2, "epb_patch_sample_occ": 2, "epb_jpeg_decode": 14,
+    "epb_patch_sample": 2, "epb_patch_sample_occ": 2, "epb_jpeg_decode": 14, "epb_refiner_forward": 12,
 }
 
 
@@ -440,6 +440,35 @@ def h36m_eval(pred, gt, cam, S, J, root, j14mask, pck_thr, metrics, per_joint, p
     _call("epb_h36m_eval", _p(pred, torch.float64), _p(gt, torch.float64), _p(cam, torch.float64),
           S, J, root, int(j14mask), float(pck_thr), _p(metrics, torch.float64),
           _p(per_joint, torch.float64), _p(pck, torch.int32), _p(poses, torch.float64), _stream())
+
+
+def pose_errors(pred, gt, S, J, submask, metrics, per_joint):
+    _call("epb_pose_errors", _p(pred, torch.float64), _p(gt, torch.float64), S, J, int(submask),
+          _p(metrics, torch.float64), _p(per_joint, torch.float64), _stream())
+
+
+def pose_to_camera(joints, cam, N, J, root, out):
+    _call("epb_pose_to_camera", _p(joints, torch.float64), _p(cam, torch.float64), N, J, root,
+          _p(out, torch.float64), _stream())
+
+
+def refiner_sizes(in_size, linear_size, out_size, N):
+    """(parameter floats, workspace floats) of the refiner kernels (host only)."""
+    npar, nws = ctypes.c_int64(), ctypes.c_int64()
+    _lib.call("epb_refiner_sizes", in_size, linear_size, out_size, N, ctypes.byref(npar), ctypes.byref(nws))
+    return npar.value, nws.value
+
+
+def refiner_prepare(in_size, linear_size, out_size, tensors, eps, params):
+    """tensors: the 68 float32 device tensors in the order of include/epb.h."""
+    ptrs = (ctypes.c_void_p * len(tensors))(*[_p(t) for t in tensors])
+    _call("epb_refiner_prepare", in_size, linear_size, out_size, ptrs, float(eps), _p(params), _stream())
+
+
+def refiner_forward(in_size, linear_size, out_size, params, x, N, normalize_in, denormalize_out, y, ws,
+                    force_form=0):
+    _call("epb_refiner_forward", in_size, linear_size, out_size, _p(params), _p(x), N, int(normalize_in),
+          int(denormalize_out), _p(y), _p(ws), ws.numel(), int(force_form), _stream())
 
 
 def pose_normalize(pose, cam, S, J, root, out):

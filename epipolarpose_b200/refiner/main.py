@@ -89,7 +89,7 @@ def _restore(path, model, optimizer, logger):
     return ckpt["epoch"], ckpt["err"], ckpt["step"], ckpt["lr"]
 
 
-def main(argv=None, train_dl=None, test_dl=None, log_root='refiner/experiments'):
+def main(argv=None, train_dl=None, test_dl=None, log_root='refiner/experiments', data_root='refiner/data'):
     args = parse_args(argv)
     out_dir = os.path.join(log_root, args.exp)
     os.makedirs(out_dir, exist_ok=True)
@@ -106,9 +106,14 @@ def main(argv=None, train_dl=None, test_dl=None, log_root='refiner/experiments')
     if args.load:
         _, best, glob_step, lr_now = _restore(args.load, model, optimizer, logger)
     if train_dl is None or test_dl is None:
-        from .data import Human36M
-        train_dl = torch.utils.data.DataLoader(Human36M(is_train=True), batch_size=64, shuffle=True)
-        test_dl = torch.utils.data.DataLoader(Human36M(is_train=False), batch_size=64, shuffle=False)
+        from .data import Human36M, SyntheticPoses
+        if all(os.path.exists(os.path.join(data_root, f)) for f in ("train.pkl", "valid.pkl")):
+            make = lambda is_train: Human36M(is_train=is_train, root=data_root)
+        else:
+            logger.info("no train.pkl / valid.pkl under %s: using synthetic poses", data_root)
+            make = lambda is_train: SyntheticPoses(is_train=is_train)
+        train_dl = torch.utils.data.DataLoader(make(True), batch_size=64, shuffle=True)
+        test_dl = torch.utils.data.DataLoader(make(False), batch_size=64, shuffle=False)
     if args.mode == 'test':
         return test(model, test_dl)
     if args.mode != 'train':

@@ -501,6 +501,55 @@ int epb_h36m_eval(const double* pred, const double* gt, const double* cam, int S
                   int root, uint32_t j14mask, double pck_thr, double* metrics,
                   double* per_joint, int32_t* pck, double* poses, epb_stream_t stream);
 
+/* Per-sample errors of camera-frame poses, the per-sample body of the refiner's evaluate
+ * (refiner/data.py:78-160 of the reference): no back-projection, no root alignment; the
+ * alignment is compute_similarity_transform(gt, pred, compute_optimal_scale=True)
+ * (lib/utils/prep_h36m.py:108-168), the same code as epb_h36m_eval's.  float64, --fmad=false.
+ *   pred, gt  [S][J][3]  camera-frame joints (mm), J <= 32
+ *   submask              bit j set <=> joint j belongs to the subset (the reference's j14)
+ *   metrics   [S][7]     means over joints of: e, e_align, e (subset), e_align (subset), |dx|, |dy|, |dz|
+ *   per_joint [S][J] (or NULL)  e per joint */
+int epb_pose_errors(const double* pred, const double* gt, int S, int J, uint32_t submask, double* metrics,
+                    double* per_joint, epb_stream_t stream);
+/* Root-relative camera-frame poses of image-space joints: CamBackProj (lib/utils/prep_h36m.py:85-89)
+ * of every joint minus that of the root, bit-identical to the `pred` column epb_h36m_eval writes
+ * (lib/dataset/h36m.py:346-348, pred_to_save['pred']).  float64, --fmad=false.
+ *   joints [N][J][3] (x px, y px, root-relative depth mm), cam [N][5] as epb_h36m_eval,
+ *   out [N][J][3] mm. */
+int epb_pose_to_camera(const double* joints, const double* cam, int N, int J, int root, double* out,
+                       epb_stream_t stream);
+
+/* Eval-mode refiner MLP: LinearModelPG.forward (refiner/model.py:117-143 of the reference,
+ * num_stage 2, bias, BatchNorm, ReLU; dropout the identity), second head.  Widths: in (input),
+ * L (linear_size, a multiple of 4), out (output); each <= 2048.
+ *
+ * epb_refiner_sizes (host only): floats of the parameter buffer, and of the workspace of a
+ * forward over N rows (N * (pad4(out) + 4 L)).
+ *
+ * epb_refiner_prepare: builds the parameter buffer (16-byte aligned) from the module's tensors,
+ * float32 device pointers in this order (68):
+ *   weight, bias of w1, linear_stages.0.w1..w4, w2, w3, linear_stages.1.w1..w4, w4 (layer order);
+ *   gamma, beta, running_mean, running_var of batch_norm1, linear_stages.0.batch_norm1..4,
+ *   batch_norm3, linear_stages.1.batch_norm1..4;
+ *   data_mean, data_std [in], labels_mean, labels_std [out] (norm.pkl; pass 0 / 1 if unused).
+ * Weights keep the [out][in] layout, rows padded to a multiple of 4 with zeros.  Each BatchNorm
+ * becomes scale = gamma / sqrt(var + eps), shift = beta - mean * scale, in float64, rounded once.
+ *
+ * epb_refiner_forward: x [N][in] -> y [N][out] (p2); 12 launches, one per linear layer.
+ *   normalize_in:    x is normalised at the first layer's load, (x - data_mean) / data_std
+ *   denormalize_out: y = p2 * labels_std + labels_mean (float32, the reference's order)
+ *   ws (16-byte aligned) begins with p1 [N][pad4(out)].
+ * Every output is one fp32 FMA chain in k order, so each row's bits do not depend on N, on the
+ * row's position or on the form: force_form 0 picks the GEMV form for N <= 128 and the tiled
+ * form above; 1 / 2 force the GEMV / tiled form (for tests of that identity).  Rows per call:
+ * N <= 262140 in the GEMV form, N <= 4194240 in the tiled form (EPB_EINVAL above). */
+int epb_refiner_sizes(int in, int L, int out, int N, int64_t* param_floats, int64_t* ws_floats);
+int epb_refiner_prepare(int in, int L, int out, const float* const* src, float eps, float* params,
+                        epb_stream_t stream);
+int epb_refiner_forward(int in, int L, int out, const float* params, const float* x, int N,
+                        int normalize_in, int denormalize_out, float* y, float* ws, int64_t ws_floats,
+                        int force_form, epb_stream_t stream);
+
 /* Pose Structure Score (the EpipolarPose paper's PSS@k, Sec. 3.3; the reference release has no
  * PSS code, the definition is lib/core/pss.py's).  float64, --fmad=false, every summation order
  * fixed, so that a numpy restatement reproduces each result bit for bit.
