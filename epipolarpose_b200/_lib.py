@@ -12,6 +12,9 @@ EPB_JPEG_DESC_BYTES = 8192
 EPB_JPEG_PLAN_LEN = 10
 EPB_JPEG_EVENTS = 6
 EPB_JPEG_STATS = 7
+EPB_JPEG_TC_DESC_BYTES = 64
+EPB_JPEG_TC_INFO_BYTES = 1128
+EPB_JPEG_TC_PLAN_LEN = 4
 
 c_int, c_i64, c_f, c_d, c_p = (ctypes.c_int, ctypes.c_int64, ctypes.c_float,
                                ctypes.c_double, ctypes.c_void_p)
@@ -110,6 +113,9 @@ _PROTOS = {
     "epb_jpeg_parse": (c_int, [c_p, c_p, c_int, c_p, c_p, c_p, c_p, c_p]),
     "epb_jpeg_decode": (c_int, [c_p, c_p, c_p, c_int, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_p]),
     "epb_softargmax_flip_lse_fwd": (c_int, [c_p] + [c_int] * 5 + [ctypes.POINTER(c_int), c_int, c_p, c_p, c_p]),
+    "epb_jpeg_transcode_plan": (c_int, [c_p, c_int, c_p, c_p, c_p, c_p]),
+    "epb_jpeg_transcode": (c_int, [c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_i64,
+                                   c_p]),
     "epb_triangulate_robust": (c_int, [c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p, c_p, c_p]),
 }
 

@@ -932,6 +932,421 @@ jpeg_color_kernel(const JpegDesc* __restrict__ descs, const uint8_t* __restrict_
   jpeg_color_pixel(d, pl, x, y, out_base + out_off[b] + (int64_t)y * out_hwp[b * 3 + 2] + 3 * x);
 }
 
+// ------------------------------------------------------------------ 6. lossless transcode
+// The coefficients of stages 2-3 coded again with a restart interval of R MCUs: every interval
+// starts from DC predictors 0 and a byte boundary, so a decoder can start at any RSTn in an exact
+// state.  Every Huffman table of the scan is regenerated from the new symbol counts (Annex K.2);
+// the coefficients, and so every decoder's pixels, stay exactly those of the source.
+constexpr int kTcDcBins = 16;                          // DC categories 0..15
+constexpr int kTcBins = 2 * kTcDcBins + 2 * 256;       // one interval: DC slots 0, 1 and AC slots 2, 3
+constexpr int kTcDhtMax = 4 + 4 * (17 + 256) + 6;      // new DHT segment + DRI segment, at most
+
+struct TcDesc {                // per image, from epb_jpeg_transcode_plan
+  int32_t ri, nint;            // restart interval (MCUs) and number of intervals; 0 when not transcoded
+  int64_t ws_hist, ws_len, ws_off, ws_tab;
+};
+static_assert(sizeof(TcDesc) <= EPB_JPEG_TC_DESC_BYTES, "transcode descriptor size");
+
+struct TcLen {                 // one interval: coded bits (-1: a category no table can code), stuffed bytes
+  int32_t bits, bytes;
+};
+
+struct TcTable {               // encoder form of one regenerated table; size 0: symbol absent
+  uint16_t code[256];
+  uint8_t size[256];
+};
+
+struct TcInfo {                // per image, read back by the host (layout in include/epb.h)
+  int32_t status, ri;
+  int64_t bytes, off, hdr_bytes;
+  uint8_t bits[4][17];         // DHT lists of slots DC 0, DC 1, AC 0, AC 1
+  uint8_t val[4][256];
+};
+static_assert(sizeof(TcInfo) == EPB_JPEG_TC_INFO_BYTES, "transcode info size");
+
+__host__ __device__ inline int tc_cat(int v) {
+  const uint32_t a = (uint32_t)(v < 0 ? -v : v);
+#ifdef __CUDA_ARCH__
+  return a ? 32 - __clz(a) : 0;
+#else
+  return a ? 32 - __builtin_clz(a) : 0;
+#endif
+}
+// the extra bits of value v of category s (F.1.2.1: negative values as v - 1, low s bits)
+__host__ __device__ inline uint32_t tc_extra(int v, int s) {
+  return (uint32_t)(v < 0 ? v + (1 << s) - 1 : v) & ((1u << s) - 1);
+}
+
+// Interval i of an image: MCUs [i R, min((i + 1) R, MCUs)) in the decoder's block order
+// (slot_comp), DC predictors reset to 0, each symbol handed to sink.sym(table slot, symbol,
+// extra-bit count, extra bits): the DC category, then AC run/size with ZRL and EOB.  Returns
+// false on a category above 15, which a Huffman table of the scan cannot code.
+template <class Sink>
+__host__ __device__ inline bool tc_walk(const JpegDesc& d, const int16_t* coef, int ri, int i, Sink& sink) {
+  const int64_t mcus = (int64_t)d.mcux * d.mcuy;
+  const int64_t m0 = (int64_t)i * ri, m1 = m0 + ri < mcus ? m0 + ri : mcus;
+  int pred[3] = {0, 0, 0};
+  for (int64_t m = m0; m < m1; ++m) {
+    for (int slot = 0; slot < d.bpm; ++slot) {
+      const int comp = d.slot_comp[slot];
+      const int16_t* blk = coef + (m * d.bpm + slot) * 64;
+      const int diff = blk[0] - pred[comp];
+      pred[comp] = blk[0];
+      const int cat = tc_cat(diff);
+      if (cat > 15) return false;
+      sink.sym(d.cdc[comp], cat, cat, tc_extra(diff, cat));
+      int run = 0;
+      for (int k = 1; k < 64; ++k) {
+        const int v = blk[zigzag_natural(k)];
+        if (!v) { ++run; continue; }
+        for (; run >= 16; run -= 16) sink.sym(d.cac[comp], 0xF0, 0, 0u);
+        const int s = tc_cat(v);
+        if (s > 15) return false;
+        sink.sym(d.cac[comp], (run << 4) | s, s, tc_extra(v, s));
+        run = 0;
+      }
+      if (run) sink.sym(d.cac[comp], 0x00, 0, 0u);
+    }
+  }
+  return true;
+}
+
+struct TcHist {                // symbol counts of one interval, kTcBins
+  int32_t* h;
+  __host__ __device__ void sym(int slot, int s, int, uint32_t) {
+    ++h[slot < 2 ? slot * kTcDcBins + s : 2 * kTcDcBins + (slot - 2) * 256 + s];
+  }
+};
+
+// Bit writer of one interval: codes MSB first, then 1-bits to the next byte; every 0xFF is
+// followed by a stuffed 0x00.  With out null it only counts; otherwise it stores at most cap
+// bytes and sets over when it would store more.
+struct TcWriter {
+  const TcTable* tab;
+  uint8_t* out;
+  int64_t cap;
+  uint64_t acc = 0;
+  int nacc = 0;
+  int64_t bits = 0, bytes = 0;
+  bool over = false;
+  __host__ __device__ void emit(int v) {
+    if (out) {
+      if (bytes < cap) out[bytes] = (uint8_t)v; else over = true;
+    }
+    ++bytes;
+  }
+  __host__ __device__ void put(uint32_t v, int n) {
+    acc = (acc << n) | v;
+    nacc += n;
+    while (nacc >= 8) {
+      nacc -= 8;
+      const int x = (int)((acc >> nacc) & 255);
+      emit(x);
+      if (x == 0xFF) emit(0);
+    }
+  }
+  __host__ __device__ void sym(int slot, int s, int n, uint32_t v) {
+    put(tab[slot].code[s], tab[slot].size[s]);
+    bits += tab[slot].size[s] + n;
+    if (n) put(v, n);
+  }
+  __host__ __device__ void finish() {
+    if (nacc) put((1u << (8 - nacc)) - 1, 8 - nacc);
+  }
+};
+
+struct TcWork {                // scratch of huff_optimal
+  int64_t freq[257];
+  int16_t sym[257], size[257], next[257];
+  int32_t nbits[258];
+};
+
+// Optimal table of Annex K.2 (figures K.1 to K.4) for the symbols of count > 0 among count[0..n),
+// plus a reserved symbol 256 of count 1 so that no code is all 1-bits.  Tie rule: of equal counts
+// the larger symbol value is taken first (the reserved symbol before every real one).  Lengths
+// are limited to 16 by K.3, and K.3's last step drops the reserved symbol's code.  Writes
+// bits[0..16] (bits[0] = 0) and val (symbols by unlimited code length, then by value); returns
+// the number of symbols.
+__host__ __device__ inline int huff_optimal(const int64_t* count, int n, TcWork& w, uint8_t* bits, uint8_t* val) {
+  int m = 0;
+  for (int s = 0; s < n; ++s)
+    if (count[s] > 0) { w.sym[m] = (int16_t)s; w.freq[m] = count[s]; ++m; }
+  for (int l = 0; l <= 16; ++l) bits[l] = 0;
+  if (m == 0) return 0;
+  w.sym[m] = 256;
+  w.freq[m] = 1;
+  ++m;
+  for (int i = 0; i < m; ++i) { w.size[i] = 0; w.next[i] = -1; }
+  for (;;) {                                   // K.1: merge the two least counts
+    int v1 = -1, v2 = -1;
+    for (int i = m - 1; i >= 0; --i) {         // descending: the first of equal counts is the larger symbol
+      const int64_t f = w.freq[i];
+      if (f <= 0) continue;
+      if (v1 < 0 || f < w.freq[v1]) { v2 = v1; v1 = i; }
+      else if (v2 < 0 || f < w.freq[v2]) v2 = i;
+    }
+    if (v2 < 0) break;
+    w.freq[v1] += w.freq[v2];
+    w.freq[v2] = 0;
+    ++w.size[v1];
+    while (w.next[v1] >= 0) { v1 = w.next[v1]; ++w.size[v1]; }
+    w.next[v1] = (int16_t)v2;
+    ++w.size[v2];
+    while (w.next[v2] >= 0) { v2 = w.next[v2]; ++w.size[v2]; }
+  }
+  for (int l = 0; l < 258; ++l) w.nbits[l] = 0;          // K.2
+  int lmax = 0;
+  for (int i = 0; i < m; ++i) {
+    ++w.nbits[w.size[i]];
+    lmax = w.size[i] > lmax ? w.size[i] : lmax;
+  }
+  for (int i = lmax; i > 16;) {                           // K.3
+    if (w.nbits[i] > 0) {
+      int j = i - 2;
+      while (w.nbits[j] == 0) --j;
+      w.nbits[i] -= 2;
+      w.nbits[i - 1] += 1;
+      w.nbits[j + 1] += 2;
+      w.nbits[j] -= 1;
+    } else {
+      --i;
+    }
+  }
+  int i = 16;
+  while (w.nbits[i] == 0) --i;
+  w.nbits[i] -= 1;
+  for (int l = 1; l <= 16; ++l) bits[l] = (uint8_t)w.nbits[l];
+  int k = 0;                                              // K.4
+  for (int l = 1; l <= lmax; ++l)
+    for (int q = 0; q < m; ++q)
+      if (w.size[q] == l && w.sym[q] != 256) val[k++] = (uint8_t)w.sym[q];
+  return k;
+}
+
+// encoder codes of a table (C.2 / C.3); every other symbol gets size 0
+__host__ __device__ inline void huff_codes(const uint8_t* bits, const uint8_t* val, TcTable& t) {
+  for (int s = 0; s < 256; ++s) { t.code[s] = 0; t.size[s] = 0; }
+  int code = 0, k = 0;
+  for (int l = 1; l <= 16; ++l) {
+    for (int q = 0; q < bits[l]; ++q, ++code, ++k) {
+      t.code[val[k]] = (uint16_t)code;
+      t.size[val[k]] = (uint8_t)l;
+    }
+    code <<= 1;
+  }
+}
+
+// length pass of interval i: coded bits and stuffed bytes, the RSTn after it included
+__host__ __device__ inline TcLen tc_interval_len(const JpegDesc& d, const int16_t* coef, const TcTable* tab, int ri,
+                                                 int nint, int i) {
+  TcWriter w{tab, nullptr, 0};
+  tc_walk(d, coef, ri, i, w);
+  w.finish();
+  TcLen r;
+  r.bits = (int32_t)w.bits;
+  r.bytes = (int32_t)w.bytes + (i + 1 < nint ? 2 : 0);
+  return r;
+}
+
+// write pass of interval i into out[0, len.bytes): its bytes, then RSTn (n = i mod 8) unless it is
+// the last; false when the interval does not come out at len.bytes
+__host__ __device__ inline bool tc_interval_write(const JpegDesc& d, const int16_t* coef, const TcTable* tab, int ri,
+                                                  int nint, int i, TcLen len, uint8_t* out) {
+  const int rst = i + 1 < nint ? 2 : 0;
+  TcWriter w{tab, out, (int64_t)len.bytes - rst};
+  tc_walk(d, coef, ri, i, w);
+  w.finish();
+  if (w.over || w.bytes + rst != len.bytes) return false;
+  if (rst) {
+    out[w.bytes] = 0xFF;
+    out[w.bytes + 1] = (uint8_t)(0xD0 + (i & 7));
+  }
+  return true;
+}
+
+// symbol pass: one thread per interval, its histogram
+__global__ void __launch_bounds__(128)
+jpeg_tc_symbols_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, uint8_t* __restrict__ ws,
+                       const int32_t* __restrict__ status) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const JpegDesc& d = descs[b];
+  const TcDesc& t = tdesc[b];
+  if (d.status != JPEG_OK || status[b] != JPEG_OK || i >= t.nint) return;
+  int32_t* h = reinterpret_cast<int32_t*>(ws + t.ws_hist) + (int64_t)i * kTcBins;
+  for (int k = 0; k < kTcBins; ++k) h[k] = 0;
+  TcHist sink{h};
+  const bool ok = tc_walk(d, reinterpret_cast<const int16_t*>(ws + d.ws_coef), t.ri, i, sink);
+  reinterpret_cast<TcLen*>(ws + t.ws_len)[i].bits = ok ? 0 : -1;
+}
+
+// one block per image: the interval histograms summed in interval order, one table per slot in use
+__global__ void __launch_bounds__(256)
+jpeg_tc_tables_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, uint8_t* __restrict__ ws,
+                      int32_t* __restrict__ status, TcInfo* __restrict__ info) {
+  const int b = blockIdx.x;
+  const JpegDesc& d = descs[b];
+  const TcDesc& t = tdesc[b];
+  if (d.status != JPEG_OK || status[b] != JPEG_OK) return;
+  __shared__ int64_t cnt[kTcBins];
+  __shared__ TcWork work[4];
+  const TcLen* len = reinterpret_cast<const TcLen*>(ws + t.ws_len);
+  int bad = 0;
+  for (int q = threadIdx.x; q < t.nint; q += blockDim.x) bad |= len[q].bits < 0;
+  if (__syncthreads_or(bad)) {
+    if (threadIdx.x == 0) status[b] = JPEG_UNSUPPORTED;
+    return;
+  }
+  const int32_t* h = reinterpret_cast<const int32_t*>(ws + t.ws_hist);
+  for (int k = threadIdx.x; k < kTcBins; k += blockDim.x) {
+    int64_t s = 0;
+    for (int q = 0; q < t.nint; ++q) s += h[(int64_t)q * kTcBins + k];
+    cnt[k] = s;
+  }
+  __syncthreads();
+  const int slot = threadIdx.x >> 5;
+  TcInfo& o = info[b];
+  TcTable* tab = reinterpret_cast<TcTable*>(ws + t.ws_tab);
+  if (slot < 4 && (threadIdx.x & 31) == 0) {           // one lane per table: the four run side by side
+    const int64_t* c = slot < 2 ? cnt + slot * kTcDcBins : cnt + 2 * kTcDcBins + (slot - 2) * 256;
+    huff_optimal(c, slot < 2 ? kTcDcBins : 256, work[slot], o.bits[slot], o.val[slot]);
+    huff_codes(o.bits[slot], o.val[slot], tab[slot]);
+  }
+}
+
+// length pass: one thread per interval
+__global__ void __launch_bounds__(128)
+jpeg_tc_length_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, uint8_t* __restrict__ ws,
+                      const int32_t* __restrict__ status) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const JpegDesc& d = descs[b];
+  const TcDesc& t = tdesc[b];
+  if (d.status != JPEG_OK || status[b] != JPEG_OK || i >= t.nint) return;
+  reinterpret_cast<TcLen*>(ws + t.ws_len)[i] =
+      tc_interval_len(d, reinterpret_cast<const int16_t*>(ws + d.ws_coef), reinterpret_cast<const TcTable*>(ws + t.ws_tab),
+                      t.ri, t.nint, i);
+}
+
+// one block per image: exclusive scan of the stuffed interval lengths -> byte offsets, and the total
+__global__ void __launch_bounds__(512)
+jpeg_tc_scan_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, uint8_t* __restrict__ ws,
+                    const int32_t* __restrict__ status, TcInfo* __restrict__ info) {
+  const int b = blockIdx.x;
+  const JpegDesc& d = descs[b];
+  const TcDesc& t = tdesc[b];
+  if (d.status != JPEG_OK || status[b] != JPEG_OK) return;
+  const TcLen* len = reinterpret_cast<const TcLen*>(ws + t.ws_len);
+  int64_t* off = reinterpret_cast<int64_t*>(ws + t.ws_off);
+  int64_t base = 0;
+  for (int q0 = 0; q0 < t.nint; q0 += blockDim.x) {
+    const int q = q0 + threadIdx.x;
+    const uint32_t v = q < t.nint ? (uint32_t)len[q].bytes : 0u;
+    uint32_t tot;
+    const uint32_t pre = block_excl_scan(v, &tot);
+    if (q < t.nint) off[q] = base + pre;
+    base += tot;
+  }
+  if (threadIdx.x == 0) info[b].bytes = base;
+}
+
+// one block: every image's final status and restart interval, then its output offset, a 64-bit
+// running sum over the images in order (one thread: B is at most 65535)
+__global__ void __launch_bounds__(512)
+jpeg_tc_finish_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, const int32_t* __restrict__ status,
+                      TcInfo* __restrict__ info, int B) {
+  for (int b = threadIdx.x; b < B; b += blockDim.x) {
+    const int s = descs[b].status != JPEG_OK ? descs[b].status : status[b];
+    info[b].status = s;
+    info[b].ri = s == JPEG_OK ? tdesc[b].ri : 0;
+    if (s != JPEG_OK) info[b].bytes = 0;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    int64_t base = 0;
+    for (int b = 0; b < B; ++b) {
+      info[b].off = base;
+      base += info[b].bytes;
+    }
+  }
+}
+
+// write pass: one thread per interval, into out_base at info.off + its offset, inside out_bytes.
+// An interval whose offsets fail the checks, or that does not come out at its counted length,
+// sets *failed (the host reads it back and fails the call).
+__global__ void __launch_bounds__(128)
+jpeg_tc_write_kernel(const JpegDesc* __restrict__ descs, const TcDesc* __restrict__ tdesc, const uint8_t* __restrict__ ws,
+                     const int32_t* __restrict__ status, const TcInfo* __restrict__ info, uint8_t* __restrict__ out_base,
+                     int64_t out_bytes, int32_t* __restrict__ failed) {
+  const int b = blockIdx.y, i = blockIdx.x * blockDim.x + threadIdx.x;
+  const JpegDesc& d = descs[b];
+  const TcDesc& t = tdesc[b];
+  if (d.status != JPEG_OK || status[b] != JPEG_OK || i >= t.nint) return;
+  const TcLen len = reinterpret_cast<const TcLen*>(ws + t.ws_len)[i];
+  const int64_t rel = reinterpret_cast<const int64_t*>(ws + t.ws_off)[i], img = info[b].off;
+  if (rel < 0 || len.bytes < 0 || rel + len.bytes > info[b].bytes || img < 0 || img + info[b].bytes > out_bytes ||
+      !tc_interval_write(d, reinterpret_cast<const int16_t*>(ws + d.ws_coef),
+                         reinterpret_cast<const TcTable*>(ws + t.ws_tab), t.ri, t.nint, i, len, out_base + img + rel))
+    *failed = 1;
+}
+
+// R = 0 (auto): the largest R whose mean interval, entropy bits / MCUs * R, is at most 3/4 of
+// kJpegSubBits.  The entropy bits are those of the bytes from SOS to the end of the blob.
+inline int tc_auto_interval(const JpegDesc& d) {
+  const int64_t mcus = (int64_t)d.mcux * d.mcuy, bits = d.ent_len * 8 > 0 ? d.ent_len * 8 : 1;
+  const int64_t r = (int64_t)kJpegSubBits * 3 / 4 * mcus / bits;
+  return (int)(r < 1 ? 1 : r > 65535 ? 65535 : r);
+}
+
+// The transcoded file's header: SOI; every segment of the source before SOS except DHT and DRI,
+// verbatim and in order; one DHT with the regenerated tables under the source's table ids (the
+// SOS selectors are kept); DRI(ri); the source's SOS segment.  b must have parsed OK.
+// Returns the bytes written, or -1 when cap is short.
+inline int64_t jpeg_tc_header(const uint8_t* b, int ri, const uint8_t (*bits)[17],
+                              const uint8_t (*val)[256], uint8_t* out, int64_t cap) {
+  int64_t n = 0, i = 2;
+  auto put = [&](const uint8_t* p, int64_t k) -> bool {
+    if (n + k > cap) return false;
+    memcpy(out + n, p, (size_t)k);
+    n += k;
+    return true;
+  };
+  const uint8_t soi[2] = {0xFF, 0xD8};
+  if (!put(soi, 2)) return -1;
+  for (;;) {
+    while (b[i] == 0xFF) ++i;
+    const int m = b[i++];
+    const int len = rd16(b + i);
+    const uint8_t mk[2] = {0xFF, (uint8_t)m};
+    if (m == 0xDA) {
+      const uint8_t* s = b + i + 2;
+      int td[2] = {-1, -1}, ta[2] = {-1, -1};           // table id of each slot, first use first (as the parser)
+      for (int q = 0; q < s[0]; ++q) {
+        const int x = s[2 + 2 * q] >> 4, y = s[2 + 2 * q] & 15;
+        if (td[0] != x && td[1] != x) td[td[0] < 0 ? 0 : 1] = x;
+        if (ta[0] != y && ta[1] != y) ta[ta[0] < 0 ? 0 : 1] = y;
+      }
+      uint8_t dht[kTcDhtMax];
+      int k = 4;
+      for (int slot = 0; slot < 4; ++slot) {
+        const int id = slot < 2 ? td[slot] : ta[slot - 2];
+        if (id < 0) continue;
+        int cnt = 0;
+        dht[k++] = (uint8_t)((slot < 2 ? 0x00 : 0x10) | id);
+        for (int l = 1; l <= 16; ++l) { dht[k++] = bits[slot][l]; cnt += bits[slot][l]; }
+        for (int q = 0; q < cnt; ++q) dht[k++] = val[slot][q];
+      }
+      dht[0] = 0xFF;
+      dht[1] = 0xC4;
+      dht[2] = (uint8_t)((k - 2) >> 8);
+      dht[3] = (uint8_t)(k - 2);
+      const uint8_t dri[6] = {0xFF, 0xDD, 0x00, 0x04, (uint8_t)(ri >> 8), (uint8_t)ri};
+      if (!put(dht, k) || !put(dri, 6) || !put(mk, 2) || !put(b + i, len)) return -1;
+      return n;
+    }
+    if (m != 0xC4 && m != 0xDD && (!put(mk, 2) || !put(b + i, len))) return -1;
+    i += len;
+  }
+}
+
 }  // namespace
 
 extern "C" __attribute__((visibility("default"))) int epb_jpeg_parse(
@@ -960,18 +1375,14 @@ extern "C" __attribute__((visibility("default"))) int epb_jpeg_parse(
   return EPB_OK;
 }
 
-extern "C" __attribute__((visibility("default"))) int epb_jpeg_decode(
-    const uint8_t* blob_base, const int64_t* blob_off, const void* desc, int B, const int64_t* plan_host, void* ws,
-    int64_t ws_bytes, uint8_t* out_base, const int64_t* out_off, const int32_t* out_hwp, int32_t* status,
-    int32_t* stats, void* const* events_host, epb_stream_t stream) {
-  EPB_CHECK_ARG(B >= 0 && B <= 65535 && plan_host);
-  if (B == 0 || plan_host[7] == 0) return EPB_OK;
-  EPB_CHECK_ARG(blob_base && blob_off && desc && ws && out_base && out_off && out_hwp && status);
-  EPB_CHECK_ARG(ws_bytes >= plan_host[0]);
-  EPB_CHECK_ARG(plan_host[2] < (1LL << 31) && plan_host[4] < (1LL << 37) && plan_host[5] <= 65535);
-  const JpegDesc* d = static_cast<const JpegDesc*>(desc);
-  uint8_t* w = static_cast<uint8_t*>(ws);
-  cudaStream_t st = as_stream(stream);
+namespace {
+
+// Stages 2 and 3 of every image whose parse status is OK (event marks 0..3): the quantised
+// coefficients, natural order with absolute DC, at ws + ws_coef; status[b] OK or MALFORMED.
+// Shared by epb_jpeg_decode and epb_jpeg_transcode.
+int jpeg_launch_coefs(const uint8_t* blob_base, const int64_t* blob_off, const JpegDesc* d, int B,
+                      const int64_t* plan_host, uint8_t* w, int32_t* status, int32_t* stats,
+                      void* const* events_host, cudaStream_t st) {
   auto mark = [&](int i) -> int {
     if (events_host) EPB_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(events_host[i]), st));
     return EPB_OK;
@@ -1004,7 +1415,29 @@ extern "C" __attribute__((visibility("default"))) int epb_jpeg_decode(
     EPB_CUDA(cudaMemsetAsync(w + plan_host[8], 0, (size_t)(plan_host[9] - plan_host[8]), st));
   jpeg_phase_c_kernel<<<gsub, 128, 0, st>>>(d, w, status);
   EPB_LAUNCH_CHECK();
-  if ((rc = mark(3))) return rc;
+  return mark(3);
+}
+
+}  // namespace
+
+extern "C" __attribute__((visibility("default"))) int epb_jpeg_decode(
+    const uint8_t* blob_base, const int64_t* blob_off, const void* desc, int B, const int64_t* plan_host, void* ws,
+    int64_t ws_bytes, uint8_t* out_base, const int64_t* out_off, const int32_t* out_hwp, int32_t* status,
+    int32_t* stats, void* const* events_host, epb_stream_t stream) {
+  EPB_CHECK_ARG(B >= 0 && B <= 65535 && plan_host);
+  if (B == 0 || plan_host[7] == 0) return EPB_OK;
+  EPB_CHECK_ARG(blob_base && blob_off && desc && ws && out_base && out_off && out_hwp && status);
+  EPB_CHECK_ARG(ws_bytes >= plan_host[0]);
+  EPB_CHECK_ARG(plan_host[2] < (1LL << 31) && plan_host[4] < (1LL << 37) && plan_host[5] <= 65535);
+  const JpegDesc* d = static_cast<const JpegDesc*>(desc);
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  cudaStream_t st = as_stream(stream);
+  auto mark = [&](int i) -> int {
+    if (events_host) EPB_CUDA(cudaEventRecord(static_cast<cudaEvent_t>(events_host[i]), st));
+    return EPB_OK;
+  };
+  int rc;
+  if ((rc = jpeg_launch_coefs(blob_base, blob_off, d, B, plan_host, w, status, stats, events_host, st))) return rc;
   const dim3 gblk((unsigned)((plan_host[4] + 127) / 128), B);
   jpeg_idct_kernel<<<gblk, 128, 0, st>>>(d, w, status);
   EPB_LAUNCH_CHECK();
@@ -1013,4 +1446,101 @@ extern "C" __attribute__((visibility("default"))) int epb_jpeg_decode(
   jpeg_color_kernel<<<gpix, 128, 0, st>>>(d, w, status, out_base, out_off, out_hwp);
   EPB_LAUNCH_CHECK();
   return mark(5);
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_jpeg_transcode_plan(
+    const void* desc_host, int B, const int32_t* interval_host, const int64_t* plan_host, void* tdesc_host,
+    int64_t* tplan_host) {
+  EPB_CHECK_ARG(B >= 0 && B <= 65535 && plan_host && tplan_host && (B == 0 || (desc_host && interval_host && tdesc_host)));
+  const JpegDesc* d = static_cast<const JpegDesc*>(desc_host);
+  TcDesc* t = static_cast<TcDesc*>(tdesc_host);
+  int64_t o = align16(plan_host[0]);
+  tplan_host[2] = o;
+  o = align16(o + (int64_t)sizeof(TcInfo) * B) + 16;      // info records, then the write pass's failure word
+  int64_t mx = 0;
+  for (int b = 0; b < B; ++b) {
+    EPB_CHECK_ARG(interval_host[b] >= 0 && interval_host[b] <= 65535);
+    memset(&t[b], 0, sizeof(TcDesc));
+    if (d[b].status != JPEG_OK) continue;
+    const int64_t mcus = (int64_t)d[b].mcux * d[b].mcuy;
+    t[b].ri = interval_host[b] ? interval_host[b] : tc_auto_interval(d[b]);
+    const int64_t nint = (mcus + t[b].ri - 1) / t[b].ri;
+    // every stuffed byte count, per interval and per image, must fit 32 bits: at most 31 bits per
+    // symbol, 64 symbols per block, each byte stuffed, plus an RSTn per interval
+    EPB_CHECK_ARG(d[b].nblocks * 64 * 31 / 8 * 2 + 2 * nint + 16 < (1LL << 31));
+    t[b].nint = (int32_t)nint;
+    t[b].ws_hist = o; o = align16(o + nint * kTcBins * 4);
+    t[b].ws_len = o;  o = align16(o + nint * (int64_t)sizeof(TcLen));
+    t[b].ws_off = o;  o = align16(o + nint * 8);
+    t[b].ws_tab = o;  o = align16(o + 4 * (int64_t)sizeof(TcTable));
+    mx = nint > mx ? nint : mx;
+  }
+  tplan_host[0] = o;
+  tplan_host[1] = mx;
+  tplan_host[3] = kTcDhtMax;
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_jpeg_transcode(
+    const uint8_t* blob_base, const int64_t* blob_off, const void* desc, const void* tdesc, int B,
+    const int64_t* plan_host, const int64_t* tplan_host, void* ws, int64_t ws_bytes, int32_t* status,
+    const uint8_t* const* blobs_host, void* info_host, uint8_t* hdr_host, const int64_t* hdr_off_host,
+    uint8_t* out_base, int64_t out_bytes, epb_stream_t stream) {
+  EPB_CHECK_ARG(B >= 0 && B <= 65535 && plan_host && tplan_host);
+  if (B == 0) return EPB_OK;
+  EPB_CHECK_ARG(blob_base && blob_off && desc && tdesc && ws && status && info_host);
+  EPB_CHECK_ARG(ws_bytes >= tplan_host[0] && tplan_host[0] >= plan_host[0]);
+  EPB_CHECK_ARG(plan_host[2] < (1LL << 31) && plan_host[5] <= 65535 && tplan_host[1] < (1LL << 31));
+  const JpegDesc* d = static_cast<const JpegDesc*>(desc);
+  const TcDesc* t = static_cast<const TcDesc*>(tdesc);
+  uint8_t* w = static_cast<uint8_t*>(ws);
+  TcInfo* info = reinterpret_cast<TcInfo*>(w + tplan_host[2]);
+  TcInfo* ih = static_cast<TcInfo*>(info_host);
+  cudaStream_t st = as_stream(stream);
+  const dim3 gint((unsigned)((tplan_host[1] + 127) / 128), B);
+  if (out_base) {                            // second call: the entropy data at the offsets read back
+    for (int b = 0; b < B; ++b)
+      EPB_CHECK_ARG(ih[b].status != JPEG_OK || (ih[b].off >= 0 && ih[b].bytes >= 0 && ih[b].off + ih[b].bytes <= out_bytes));
+    if (tplan_host[1] == 0) return EPB_OK;
+    int32_t* failed = reinterpret_cast<int32_t*>(w + align16(tplan_host[2] + (int64_t)sizeof(TcInfo) * B));
+    int32_t failed_host = 0;
+    EPB_CUDA(cudaMemsetAsync(failed, 0, 4, st));
+    jpeg_tc_write_kernel<<<gint, 128, 0, st>>>(d, t, w, status, info, out_base, out_bytes, failed);
+    EPB_LAUNCH_CHECK();
+    EPB_CUDA(cudaMemcpyAsync(&failed_host, failed, 4, cudaMemcpyDeviceToHost, st));
+    EPB_CUDA(cudaStreamSynchronize(st));
+    if (failed_host) {
+      epb_set_error("epb_jpeg_transcode: an interval's offsets or length disagree with the first call's (was the "
+                    "workspace reused by another call, or the output smaller than the sizes read back?)");
+      return EPB_EINVAL;
+    }
+    return EPB_OK;
+  }
+  EPB_CHECK_ARG(blobs_host && hdr_host && hdr_off_host);
+  EPB_CUDA(cudaMemsetAsync(info, 0, sizeof(TcInfo) * B, st));
+  int rc;
+  if (plan_host[7] &&
+      (rc = jpeg_launch_coefs(blob_base, blob_off, d, B, plan_host, w, status, nullptr, nullptr, st)))
+    return rc;
+  if (tplan_host[1]) {
+    jpeg_tc_symbols_kernel<<<gint, 128, 0, st>>>(d, t, w, status);
+    EPB_LAUNCH_CHECK();
+    jpeg_tc_tables_kernel<<<B, 256, 0, st>>>(d, t, w, status, info);
+    EPB_LAUNCH_CHECK();
+    jpeg_tc_length_kernel<<<gint, 128, 0, st>>>(d, t, w, status);
+    EPB_LAUNCH_CHECK();
+    jpeg_tc_scan_kernel<<<B, 512, 0, st>>>(d, t, w, status, info);
+    EPB_LAUNCH_CHECK();
+  }
+  jpeg_tc_finish_kernel<<<1, 512, 0, st>>>(d, t, status, info, B);
+  EPB_LAUNCH_CHECK();
+  EPB_CUDA(cudaMemcpyAsync(ih, info, sizeof(TcInfo) * B, cudaMemcpyDeviceToHost, st));
+  EPB_CUDA(cudaStreamSynchronize(st));
+  for (int b = 0; b < B; ++b) {
+    if (ih[b].status != JPEG_OK) continue;
+    ih[b].hdr_bytes = jpeg_tc_header(blobs_host[b], ih[b].ri, ih[b].bits, ih[b].val, hdr_host + hdr_off_host[b],
+                                     hdr_off_host[b + 1] - hdr_off_host[b]);
+    EPB_CHECK_ARG(ih[b].hdr_bytes >= 0);
+  }
+  return EPB_OK;
 }

@@ -340,6 +340,96 @@ def decode_jpeg_batch_device(blobs, stats=None, events=None):
     return frames
 
 
+JPEG_TC_MISMATCH = 3          # transcode status: the verify decode differed from the source's
+
+
+def transcode_jpeg_batch_device(blobs, interval='auto', verify=True):
+    """B JPEG files (bytes or 1-D uint8 arrays) -> (list of B bytes, status int32 [B]): each file
+    losslessly re-coded on the device with a restart interval of `interval` MCUs ('auto': per image
+    the largest whose mean interval is at most 768 bits, so that the device decoder starts most
+    1024-bit subsequences at a restart marker) and regenerated Huffman tables.  The quantised
+    coefficients are kept, so every decoder gives the source's pixels.  The header keeps every
+    segment before SOS except DHT and DRI; bytes after the source's EOI are dropped.
+    Status 0: transcoded.  Blobs the device does not decode (1 unsupported, 2 malformed) come back
+    unchanged.  verify: decode the outputs and the sources on the device and compare the frames;
+    a difference returns the source unchanged with status JPEG_TC_MISMATCH (3)."""
+    ops = _backend[0]
+    dev = _dev()
+    bufs = [np.frombuffer(b, dtype=np.uint8) if isinstance(b, (bytes, bytearray, memoryview))
+            else np.ascontiguousarray(np.asarray(b, dtype=np.uint8).reshape(-1)) for b in blobs]
+    B = len(bufs)
+    if interval == 'auto':
+        r = 0
+    else:
+        r = int(interval)
+        if not 1 <= r <= 65535:
+            raise ValueError("interval must be 'auto' or 1..65535 MCUs, got %r" % (interval,))
+    if B == 0:
+        return [], np.zeros(0, np.int32)
+    desc, status, _, _, plan = ops.jpeg_parse(bufs)
+    tdesc, tplan = ops.jpeg_transcode_plan(desc, B, np.full(B, r, np.int32), plan)
+    blob_off = np.zeros(B, dtype=np.int64)
+    pos = 0
+    for i, b in enumerate(bufs):
+        blob_off[i] = pos
+        pos += (b.size + 16 + 15) // 16 * 16
+    parts = [("desc", desc.reshape(-1)), ("tdesc", tdesc.reshape(-1)), ("blob_off", blob_off.view(np.uint8)),
+             ("status", status.view(np.uint8))]
+    where, p = {}, pos
+    for name, a in parts:
+        where[name] = (p, a.size)
+        p = (p + a.size + 15) // 16 * 16
+    stage = torch.empty(p, dtype=torch.uint8).pin_memory()
+    sn = stage.numpy()
+    for i, b in enumerate(bufs):
+        sn[blob_off[i]:blob_off[i] + b.size] = b
+    for name, a in parts:
+        sn[where[name][0]:where[name][0] + a.size] = a
+    d_stage = stage.to(dev, non_blocking=True)
+
+    def view(name, dtype):
+        o, n = where[name]
+        return d_stage[o:o + n].view(dtype)
+    args = (d_stage, view("blob_off", torch.int64), view("desc", torch.uint8), view("tdesc", torch.uint8), B, plan,
+            tplan)
+    ws = torch.empty(int(tplan[0]), dtype=torch.uint8, device=dev)
+    hdr_off = np.zeros(B + 1, dtype=np.int64)
+    hdr_off[1:] = np.cumsum([b.size + int(tplan[3]) for b in bufs])
+    hdr = np.zeros(int(hdr_off[-1]), dtype=np.uint8)
+    info = ops.jpeg_transcode(*args, ws, view("status", torch.int32), bufs, hdr, hdr_off)
+    ok = info["status"] == 0
+    ent = torch.empty(max(int((info["bytes"] * ok).sum()), 16), dtype=torch.uint8, device=dev)
+    ops.jpeg_transcode_write(*args, ws, view("status", torch.int32), info, ent)
+    ent_h = ent.cpu().numpy()
+    out, st = [], info["status"].astype(np.int32)
+    for i, b in enumerate(bufs):
+        if not ok[i]:
+            out.append(b.tobytes())
+            continue
+        h0, o = int(hdr_off[i]), int(info["off"][i])
+        out.append(hdr[h0:h0 + int(info["hdr_bytes"][i])].tobytes() + ent_h[o:o + int(info["bytes"][i])].tobytes() +
+                   b"\xff\xd9")
+    if verify and ok.any():
+        idx = [i for i in range(B) if ok[i]]
+        src = decode_jpeg_batch_device([bufs[i] for i in idx])
+        try:
+            both = decode_jpeg_batch_device([out[i] for i in idx])
+            new = [(both, k) for k in range(len(idx))]
+        except IOError:                     # an output no decoder reads: check them one by one
+            new = []
+            for i in idx:
+                try:
+                    new.append((decode_jpeg_batch_device([out[i]]), 0))
+                except IOError:
+                    new.append((None, 0))
+        for k, i in enumerate(idx):
+            f, j = new[k]
+            if src.status[k] != 0 or f is None or f.status[j] != 0 or not torch.equal(src.frame(k), f.frame(j)):
+                out[i] = bufs[i].tobytes()
+                st[i] = JPEG_TC_MISMATCH
+    return out, st
+
+
 def read_jpeg_batch_device(paths):
     """decode_jpeg_batch_device of the files at `paths`."""
     blobs = []

@@ -430,6 +430,46 @@ def jpeg_decode(blob_base, blob_off, desc, B, plan, ws, out_base, out_off, out_h
           _p(out_hwp, torch.int32), _p(status, torch.int32), _p(stats, torch.int32), ev, _stream())
 
 
+def _tc_info_dtype():
+    import numpy as np
+    return np.dtype([("status", np.int32), ("ri", np.int32), ("bytes", np.int64), ("off", np.int64),
+                     ("hdr_bytes", np.int64), ("bits", np.uint8, (4, 17)), ("val", np.uint8, (4, 256))],
+                    align=True)
+
+
+def jpeg_transcode_plan(desc, B, interval, plan):
+    """desc / plan: host arrays of jpeg_parse; interval: int32 [B], R in MCUs or 0 for auto ->
+    (tdesc uint8 [B, EPB_JPEG_TC_DESC_BYTES], tplan int64 [EPB_JPEG_TC_PLAN_LEN]), host."""
+    import numpy as np
+    interval = np.ascontiguousarray(interval, dtype=np.int32)
+    tdesc = np.zeros((max(B, 1), _lib.EPB_JPEG_TC_DESC_BYTES), dtype=np.uint8)
+    tplan = np.zeros(_lib.EPB_JPEG_TC_PLAN_LEN, dtype=np.int64)
+    _lib.call("epb_jpeg_transcode_plan", desc.ctypes.data, B, interval.ctypes.data,
+              np.ascontiguousarray(plan, dtype=np.int64).ctypes.data, tdesc.ctypes.data, tplan.ctypes.data)
+    return tdesc[:B], tplan
+
+
+def jpeg_transcode(blob_base, blob_off, desc, tdesc, B, plan, tplan, ws, status, blobs_host, hdr, hdr_off):
+    """First call of epb_jpeg_transcode (out_base NULL): -> the info records (numpy structured, [B]);
+    headers are written into the host uint8 array hdr at hdr_off (int64 [B + 1])."""
+    import numpy as np
+    dt = _tc_info_dtype()
+    assert dt.itemsize == _lib.EPB_JPEG_TC_INFO_BYTES
+    info = np.zeros(max(B, 1), dtype=dt)
+    ptrs = (ctypes.c_void_p * max(B, 1))(*[b.ctypes.data for b in blobs_host])
+    _call("epb_jpeg_transcode", _p(blob_base, torch.uint8), _p(blob_off, torch.int64), _p(desc, torch.uint8),
+          _p(tdesc, torch.uint8), B, plan.ctypes.data, tplan.ctypes.data, _p(ws, torch.uint8), ws.numel(),
+          _p(status, torch.int32), ptrs, info.ctypes.data, hdr.ctypes.data, hdr_off.ctypes.data, None, 0, _stream())
+    return info[:B]
+
+
+def jpeg_transcode_write(blob_base, blob_off, desc, tdesc, B, plan, tplan, ws, status, info, out):
+    """Second call of epb_jpeg_transcode: every OK image's entropy data into the device uint8 out."""
+    _call("epb_jpeg_transcode", _p(blob_base, torch.uint8), _p(blob_off, torch.int64), _p(desc, torch.uint8),
+          _p(tdesc, torch.uint8), B, plan.ctypes.data, tplan.ctypes.data, _p(ws, torch.uint8), ws.numel(),
+          _p(status, torch.int32), None, info.ctypes.data, None, None, _p(out, torch.uint8), out.numel(), _stream())
+
+
 def patch_joints(joints, box, trans, B, J, patch_w, patch_h, rect_3d_w, depth_in_image, label):
     _call("epb_patch_joints", _p(joints, torch.float64), _p(box, torch.float64), _p(trans, torch.float64),
           B, J, float(patch_w), float(patch_h), float(rect_3d_w), int(depth_in_image),

@@ -672,6 +672,37 @@ int epb_jpeg_decode(const uint8_t* blob_base, const int64_t* blob_off, const voi
                     const int64_t* out_off, const int32_t* out_hwp, int32_t* status, int32_t* stats,
                     void* const* events_host, epb_stream_t stream);
 
+/* Lossless transcode to short restart intervals.  The quantised coefficients are those of
+ * epb_jpeg_decode's stages; only the entropy coding changes: restart interval R (DRI), every
+ * Huffman table regenerated from the new symbol counts (JPEG Annex K.2, codes of at most 16
+ * bits), the rest of the header kept.  Any decoder gives the source's pixels. */
+#define EPB_JPEG_TC_DESC_BYTES 64   /* one transcode descriptor per image                        */
+#define EPB_JPEG_TC_INFO_BYTES 1128 /* per image: int32 status, int32 R, int64 entropy bytes,
+                                       int64 entropy offset, int64 header bytes,
+                                       uint8 bits[4][17], uint8 val[4][256] (slots DC 0, DC 1,
+                                       AC 0, AC 1)                                             */
+#define EPB_JPEG_TC_PLAN_LEN 4
+/* Host only.  interval_host [B]: R in MCUs (1..65535), or 0 for the largest R whose mean
+ * interval (entropy bytes from SOS to the end of the blob x 8 / MCUs x R) is at most 768 bits.
+ * tdesc_host [B][EPB_JPEG_TC_DESC_BYTES] (the device copy is what epb_jpeg_transcode reads);
+ * tplan_host: [0] workspace bytes (includes epb_jpeg_parse's), [1] most intervals of an image,
+ * [2] info offset in the workspace, [3] bytes the header may grow by (new DHT and DRI). */
+int epb_jpeg_transcode_plan(const void* desc_host, int B, const int32_t* interval_host, const int64_t* plan_host,
+                            void* tdesc_host, int64_t* tplan_host);
+/* Two calls with the same arguments and workspace.  With out_base NULL: decodes the coefficients,
+ * counts the symbols, builds the tables and lays the entropy data out; synchronises the stream
+ * and fills info_host [B][EPB_JPEG_TC_INFO_BYTES] (status OK, UNSUPPORTED for a category no table
+ * can code, or the parse / decode status; offsets of the OK images packed in image order) and,
+ * for every OK image, its header (SOI up to and including SOS) at hdr_host + hdr_off_host[b],
+ * at most hdr_off_host[b + 1] - hdr_off_host[b] bytes.  With out_base: writes each OK image's
+ * entropy data (intervals, RSTn between them; no EOI) at out_base + off, all within out_bytes;
+ * synchronises the stream and fails if any interval's offsets or length disagree with the first call's.
+ * The file is header + entropy data + EOI.  Images not OK are never touched. */
+int epb_jpeg_transcode(const uint8_t* blob_base, const int64_t* blob_off, const void* desc, const void* tdesc,
+                       int B, const int64_t* plan_host, const int64_t* tplan_host, void* ws, int64_t ws_bytes,
+                       int32_t* status, const uint8_t* const* blobs_host, void* info_host, uint8_t* hdr_host,
+                       const int64_t* hdr_off_host, uint8_t* out_base, int64_t out_bytes, epb_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * Optimiser (torch.optim.Adam call site lib/utils/utils.py:56-60; betas
  * (0.9,0.999), eps 1e-8, no weight decay) over one flat parameter buffer.
