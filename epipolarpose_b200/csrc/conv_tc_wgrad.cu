@@ -31,6 +31,11 @@ constexpr int kGroups = 2;       // producer groups of 4 warps (one tile each, r
 constexpr int kProd = 32 * kProdWarps;
 constexpr int kThreadsW = 32 * kConsWarps + kProd;
 constexpr int kMaxSlots = 16;
+// Longest pixel run one CTA accumulates in registers, in KPIX blocks, for 3xTF32.  wgmma adds
+// into its fp32 accumulator rounding toward zero, so a run of K pixels drifts toward zero by up
+// to ~0.75 * 2^-24 * passes * K / 8 of the result: 184 blocks (5888 pixels) keep that below
+// 1e-4 with three passes; one pass may run three times as long.
+constexpr int kMaxRunBlocks3 = 184;
 
 template <int BNW, int NS>
 struct WCfg {
@@ -366,13 +371,16 @@ int launch_wgrad(const epb_conv_geom* g, const float* in, const float* dout, con
   const int nb = (total_slots + groups - 1) / groups;          // balanced group size
   const int groups2 = (total_slots + nb - 1) / nb;
   const int64_t tiles = (int64_t)co_tiles * groups2;
-  // Split the pixel range so that the grid fills whole waves of one CTA per SM (a
-  // 2.16-wave grid idles most SMs in its last round).  Cost model per split count:
-  // rounds x (pixel blocks per CTA + fixed prologue/epilogue cost worth ~6 blocks).
+  // Split the pixel range so that no CTA's run exceeds the accumulation cap (kMaxRunBlocks3)
+  // and the grid fills whole waves of one CTA per SM (a 2.16-wave grid idles most SMs in its
+  // last round).  Cost model per split count: rounds x (pixel blocks per CTA + fixed
+  // prologue/epilogue cost worth ~6 blocks), over up to three waves past the fewest splits.
   const int64_t max_splits = (M + 8 * KPIX - 1) / (8 * KPIX);   // >= 8 pixel blocks per CTA
-  int64_t splits = 1;
+  const int64_t run_cap = (int64_t)kMaxRunBlocks3 * 3 / NS * KPIX;
+  const int64_t min_splits = (M + run_cap - 1) / run_cap;
+  int64_t splits = min_splits;
   int64_t best = -1;
-  for (int64_t sp = 1; sp <= max_splits && sp * tiles <= 3 * kNumSMs + tiles; ++sp) {
+  for (int64_t sp = min_splits; sp <= max_splits && (sp - min_splits) * tiles <= 3 * kNumSMs; ++sp) {
     const int64_t rounds = (sp * tiles + kNumSMs - 1) / kNumSMs;
     const int64_t blocks = ((M + sp - 1) / sp + KPIX - 1) / KPIX;
     const int64_t cost = rounds * (blocks + 6);

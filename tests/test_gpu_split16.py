@@ -414,10 +414,15 @@ C4_LAYERS = [
 
 @pytest.mark.parametrize("layer", C4_LAYERS, ids=[c[0] for c in C4_LAYERS])
 def test_conv16_bench_layer_shapes_vs_torch_float64(dev, layer):
+    _check_conv16_layer(dev, layer, 128, 2e-4)
+
+
+def _check_conv16_layer(dev, layer, N, wgrad_bar):
+    """conv16 fprop (with statistics), dgrad and wgrad of one layer over N images against torch
+    float64 on the values the planes hold; returns the three errors"""
     import torch.nn.functional as F
     from epipolarpose_b200 import net, ops
     name, kind, cin, cout, k, s, p, hw = layer
-    N = 128
     conv = net.Conv("t", kind, cin, cout, k, s, p, 0)
     Ho, Wo = conv.out_hw(hw, hw)
     T = k * k
@@ -453,7 +458,7 @@ def test_conv16_bench_layer_shapes_vs_torch_float64(dev, layer):
             gm.in_relu, gm.accumulate = 0, 0
             ops.conv16_fprop(gm, x, x_sc, wf, wf_sc, out, None, stats)
     r = ref.detach().permute(0, 2, 3, 1)
-    e = float((out.double() - r).abs().max() / r.abs().max())
+    e_f = e = float((out.double() - r).abs().max() / r.abs().max())
     assert e <= 5e-5, "fprop %.3e" % e
     # per-channel sums: fp32 partial sums over up to 3584 rows per CTA, then float64 atomics
     assert float((stats[:cout] - r.sum((0, 1, 2))).abs().max() / r.abs().sum((0, 1, 2)).max()) <= 5e-5
@@ -464,7 +469,7 @@ def test_conv16_bench_layer_shapes_vs_torch_float64(dev, layer):
             gm.in_relu, gm.accumulate = 0, 0
             ops.conv16_fprop(gm, dz, dz_sc, wd, wd_sc, din, None, None)
     r = xa.grad.permute(0, 2, 3, 1)
-    e = float((din.double() - r).abs().max() / r.abs().max())
+    e_d = e = float((din.double() - r).abs().max() / r.abs().max())
     assert e <= 5e-5, "dgrad %.3e" % e
     # wgrad (packed [cout][T][cin])
     dw = torch.zeros(cout * T * cin, device=dev)
@@ -476,4 +481,5 @@ def test_conv16_bench_layer_shapes_vs_torch_float64(dev, layer):
     gw = wt.grad
     r = (gw.permute(0, 2, 3, 1) if kind == "conv" else gw.permute(1, 2, 3, 0)).reshape(cout, T, cin)
     e = float((dw.view(cout, T, cin).double() - r).abs().max() / r.abs().max())
-    assert e <= 2e-4, "wgrad %.3e" % e       # fp32 accumulation over up to 524288 pixels (split in <= 74 runs)
+    assert e <= wgrad_bar, "wgrad %.3e (bar %.2e)" % (e, wgrad_bar)   # C4: fp32 runs over up to 524288 / 74 pixels
+    return e_f, e_d, e

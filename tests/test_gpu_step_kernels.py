@@ -380,7 +380,10 @@ def test_fused_adam_vs_float64_on_model_buffer(dev):
     in the flat layout: epb_adam_step_dev is the path taken.  Steps 1, 2 and 1000 (step_dev set
     to 999 first), update / m / v per element against the float64 contract, and the update
     against torch.optim.Adam on the same fp32 state."""
-    m, opt = _r50(dev)
+    _check_fused_adam(dev, *_r50(dev))
+
+
+def _check_fused_adam(dev, m, opt):
     st_key = "flat0"
     opt.state.pop(st_key, None)                             # from step 1, whatever ran before
     buf = opt._flat[0]["buf"]
@@ -675,9 +678,12 @@ def test_split16_batch_bit_exact_on_model_jobs(dev):
     synthetic jobs in the same batch (all zeros, amax in the last partial block, amax a power of
     two, 1 / 3 / 2049 elements, 2^24 + 5 elements): bit-exact with the CPU emulation, planes as
     int16 and both scale words; s = pow2_scale(amax), max|hi| <= 2^14, no +-65504."""
+    _check_split16_batch(dev, *_r50(dev))
+
+
+def _check_split16_batch(dev, m, opt):
     from epipolarpose_b200 import ops
     from tests import emul_ops
-    m, opt = _r50(dev)
     if "flat0" not in opt.state:
         _flat_grads(opt, dev, 31)
         opt.step()
@@ -720,9 +726,12 @@ def test_pack_weight_batch_bit_exact_on_model_jobs(dev):
     """pack_weight_batch on the engine's model-scale jobs (R50/J16/D64): the fprop / dgrad operand
     pack of every layer and the per-stage unpack of the weight gradients, bit-exact with the CPU
     emulation (a permutation: no arithmetic)."""
+    _check_pack_weight_batch(dev, _r50(dev)[0])
+
+
+def _check_pack_weight_batch(dev, m):
     from epipolarpose_b200 import ops
     from tests import emul_ops
-    m, _ = _r50(dev)
     eng = m._engine()
     eng.dev = dev
     params = dict(m.named_parameters())
@@ -757,12 +766,15 @@ def test_pack_weight_batch_bit_exact_on_model_jobs(dev):
 def test_im2col_split_bit_exact_at_stem_bench_size(dev):
     """im2col_split over all 128 images of 256 x 256 (7 x 7 / 2, pad 3): bit-exact with the CPU
     emulation on the first, last and three middle images."""
+    _check_im2col_split(dev, _r50(dev)[0]._engine().stem_kpad, 128, 256)
+
+
+def _check_im2col_split(dev, kpad, N, H):
+    """im2col_split of N images of H x H (7 x 7 / 2, pad 3), bit-exact on five images"""
     from epipolarpose_b200 import ops, net16
     from tests import emul_ops
-    m, _ = _r50(dev)
-    eng = m._engine()
-    N, H, W, kpad = 128, 256, 256, eng.stem_kpad
-    Ho = Wo = 128
+    W = H
+    Ho = Wo = H // 2
     g = torch.Generator(device=dev).manual_seed(51)
     img = torch.randn(N, 3, H, W, device=dev, generator=g)
     img[5, :, 0, :] = 4094.0 / net16.IMG_SCALE              # the static scale's largest magnitude
@@ -770,7 +782,7 @@ def test_im2col_split_bit_exact_at_stem_bench_size(dev):
     sc = torch.tensor([net16.IMG_SCALE, 1.0 / net16.IMG_SCALE, 65504.0 / net16.IMG_SCALE, 0.0], device=dev)
     ops.im2col_split(img, col, sc, N, 3, H, W, 7, 7, 2, 3, Ho, Wo, kpad)
     torch.cuda.synchronize()
-    pick = [0, 5, 63, 64, N - 1]
+    pick = [0, 5, N // 2 - 1, N // 2, N - 1]
     cimg = img[pick].cpu()
     ccol = torch.empty(2, len(pick), Ho, Wo, kpad, dtype=torch.float16)
     emul_ops.im2col_split(cimg, ccol, sc.cpu(), len(pick), 3, H, W, 7, 7, 2, 3, Ho, Wo, kpad)
@@ -785,9 +797,14 @@ def test_maxpool_bwd_vs_float64_at_stem_bench_size(dev):
     bn_relu_maxpool_split on dyadic inputs (exact fma, many ties), fp32 dy.  maxpool_bwd against a
     float64 scatter within 3u sum|g|, bit-equal with an fp32 restatement adding in (kh, kw)
     order; where argidx differs from torch.max_pool2d's index the window holds a tie."""
+    _check_maxpool_bwd(dev, 128, 128)
+
+
+def _check_maxpool_bwd(dev, N, H):
+    """maxpool_bwd of the stem's pool over N images of H x H x 64"""
     from epipolarpose_b200 import ops
-    N, H, W, C = 128, 128, 128, 64
-    Ho = Wo = 64
+    W, C = H, 64
+    Ho = Wo = H // 2
     g = torch.Generator(device=dev).manual_seed(61)
     z = torch.round(torch.randn(N, H, W, C, device=dev, generator=g) * 64) / 64
     scale = torch.round((torch.rand(C, device=dev, generator=g) + 0.5) * 256) / 256
@@ -857,8 +874,12 @@ def test_softargmax_fwd_vs_float64_at_bench_shape(dev, kind):
     the merge-depth bar, lse[0] the exact maximum, lse[1] * sum exp(v - m) - 1 within its bar.
     randn3: logits x 3 as in the backward test; peaks60: one logit of 60 per (image, joint);
     constant: every logit 0.7 (the uniform distribution)."""
+    _check_softargmax_fwd(dev, kind, 128, 16, 64, 64, 64)
+
+
+def _check_softargmax_fwd(dev, kind, N, J, D, H, W):
+    """epb_softargmax_fwd (NHWC) at one shape against float64 within the merge-depth bar"""
     from epipolarpose_b200 import ops
-    N, J, D, H, W = 128, 16, 64, 64, 64
     C = J * D
     g = torch.Generator(device=dev).manual_seed(71)
     if kind == "constant":
@@ -925,8 +946,12 @@ def _jointloss64(x, t, w, kind, norm, div):
 def test_jointloss_vs_float64_at_bench_shape(dev, kind, norm):
     """epb_jointloss_fwd_bwd at N = 128, J = 16 (6144 elements), weights with zeros, |d| on both
     sides of 1 and exactly 1 (dyadic x, t: d exact without norm): loss and dx against float64."""
+    _check_jointloss(dev, kind, norm, 128, 16)
+
+
+def _check_jointloss(dev, kind, norm, N, J):
+    """epb_jointloss_fwd_bwd over n = N J 3 elements against float64 within the module's bar"""
     from epipolarpose_b200 import ops
-    N, J = 128, 16
     n = N * J * 3
     g = torch.Generator(device=dev).manual_seed(81 + kind + 2 * norm)
     t = torch.round((torch.rand(n, device=dev, generator=g) - 0.5) * 1024) / 1024

@@ -151,13 +151,18 @@ _KNAME = re.compile(r"conv_(fprop|wgrad)_(?:tc_kernel(?:<(\d+), ?(\d+)>|ILi(\d+)
 def _ran(fn):
     """Runs fn under torch.profiler; returns the conv kernels that ran, as 'fprop_tc<128,3>',
     'wgrad_simt', ...  fn writes scratch buffers only: a short profiling session now and then
-    delivers no device activity at all, and is then repeated (up to three sessions)."""
+    delivers no device activity at all, and is then repeated (up to eight sessions).  Each
+    session starts on an idle device and stays open a few milliseconds after fn's kernels have
+    finished, so that their activity records are inside its window when it stops."""
+    import time
     from torch.profiler import ProfilerActivity, profile
     tags = set()
-    for _ in range(3):
+    for _ in range(8):
+        torch.cuda.synchronize()
         with profile(activities=[ProfilerActivity.CUDA]) as prof:
             fn()
             torch.cuda.synchronize()
+            time.sleep(0.005)
         for ev in prof.events():
             m = _KNAME.search(ev.name)
             if m:
