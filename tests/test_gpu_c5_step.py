@@ -524,8 +524,12 @@ def test_c5_softargmax_fwd_vs_float64(dev, kind):
 def test_c5_softargmax_bwd_fp32_vs_float64(dev):
     """epb_softargmax_bwd (fp32 NHWC, the path C5's head takes) at N = 64, J = 17, D = 96,
     96 x 96: every element of the logit gradient against float64 p (s - s_bar) within its bar."""
+    _check_softargmax_bwd_fp32(dev, N5, J5, D5, HM5, HM5)
+
+
+def _check_softargmax_bwd_fp32(dev, N, J, D, H, W):
+    """epb_softargmax_bwd (fp32 NHWC) at one shape against float64 within _sabwd_ref_bar"""
     from epipolarpose_b200 import ops
-    N, J, D, H, W = N5, J5, D5, HM5, HM5
     C = J * D
     g = torch.Generator(device=dev).manual_seed(93)
     logits = torch.randn(N, H, W, C, device=dev, generator=g) * 3
@@ -545,7 +549,7 @@ def test_c5_softargmax_bwd_fp32_vs_float64(dev):
         worst = max(worst, float(err.max()))
         ratio = max(ratio, float((err / (e + 1e-300)).max()))
         del ref, e, err
-    print("  C5 softargmax bwd fp32: max err %.3e, worst err / bar %.3f" % (worst, ratio))
+    print("  softargmax bwd fp32 N %d J %d D %d %dx%d: max err %.3e, worst err / bar %.3f" % (N, J, D, H, W, worst, ratio))
     assert ratio <= 1.0
 
 
@@ -555,8 +559,12 @@ def test_c5_colsum_vs_float64(dev, M):
     """epb_colsum over M x 1632 (the bias gradient of C5's final layer; M5 - 23 leaves a partial
     last CTA of 41 rows) against float64 column sums within the module's bar; a second run
     within one fp32 ulp."""
+    _check_colsum(dev, M, J5 * D5)
+
+
+def _check_colsum(dev, M, C):
+    """epb_colsum over M x C against float64 column sums within _colsum_bar's terms"""
     from epipolarpose_b200 import ops
-    C = J5 * D5
     g = torch.Generator(device=dev).manual_seed(95)
     x = torch.randn(M, C, device=dev, generator=g) * 1e-3
     x[:, :8] += 1e-3                                            # columns with a consistent sign
@@ -570,12 +578,13 @@ def test_c5_colsum_vs_float64(dev, M):
         xd = x[r0:r0 + (1 << 16)].double()
         ref += xd.sum(0)
         sab += xd.abs().sum(0)
-    ctas = -(-M // 64)
-    bar = 64 * U * sab + (1 + ctas) * 2.0 ** -53 * sab + U * ref.abs()
+    rpi = max(256 // (C // 4), 1)                               # bn.cu make_rowmap
+    ctas = -(-M // (64 * rpi))
+    bar = 64 * U * sab + (rpi + ctas) * 2.0 ** -53 * sab + U * ref.abs()
     err = (out.double() - ref).abs()
     ulp = (out.double().abs() * 2.0 ** -23).clamp_min(2.0 ** -149)
-    print("  C5 colsum M %d: max err %.3e, worst err / bar %.3f, second run identical %s"
-          % (M, float(err.max()), float((err / bar).max()), bool(torch.equal(out, out2))))
+    print("  colsum M %d C %d: max err %.3e, worst err / bar %.3f, second run identical %s"
+          % (M, C, float(err.max()), float((err / bar).max()), bool(torch.equal(out, out2))))
     assert bool((err <= bar).all())
     assert bool(((out.double() - out2.double()).abs() <= ulp).all())
 

@@ -1,0 +1,1008 @@
+"""The tf32x3 training step (net.Engine at precision 3: the 3xTF32 wgmma convolutions and the fp32
+bn.cu BatchNorm chain; MODEL.PRECISION's default, bench.py --precision tf32x3, and the engine
+get_pose_net falls back to for plans net16 refuses) against float64 kernel by kernel at the bench's
+sizes (R50, J = 16, D = 64, 256 x 256, N = 128: 32 tuples x 4 views), and a coverage gate: every
+C-ABI entry one tf32x3 step calls must name the tests that hold it to float64 at those sizes
+(COVERAGE_TF32X3).
+
+Every reference is torch float64 on the device, computed from the exact fp32 values the kernel
+read, in image or row chunks where memory needs it.  Bars (u = 2^-24):
+
+  * Convolutions (fprop, dgrad, wgrad at every distinct R50 conv of the step, with the step's
+    operand modes): the bars of test_gpu_tf32.  fprop / dgrad: _tc_bar(FPROP_BAR, K, 3), K the
+    longest taps x Cin of the call's geometries; wgrad: _tc_bar(WGRAD_BAR, R, 3), R the pixel
+    run of one CTA from the TF32 wgrad planner (`_tf32_wgrad_plan` over each geometry's
+    N Hp Wp pixels), since wgmma accumulates toward zero.  Statistics: STATS_SELF_BAR against
+    the float64 sums of the kernel's own output, the fprop bar against the reference's sums.
+    Every conv kernel that runs must be a three-pass instantiation `<*, 3>`.
+  * bn_bwd_reduce + bn_bwd_apply.  Each thread adds kRowsPerThread = 64 rows in fp32, the CTA's
+    row slots and all CTAs add in double, so with d = 64 + 2, |d dbeta| <= d u sum|g| and
+    |d dgamma| <= (d + 1) u sum|g xhat| + sum|g| e_xhat, where e_xhat = 4u (|xhat| + |mean|
+    invstd) is the error of the fp32 xhat formed from the fp32 mean and invstd (the same terms
+    as test_gpu_bn_chain's backward).  dgamma and dbeta then round once to fp32.  Not from
+    max|dgamma|: dgamma cancels.  k0 = gamma invstd, k1 = sum g / M, k2 = sum g xhat / M round
+    to fp32, and dx = k0 (g - k1 - xhat k2) takes four more roundings: |d dx| <= |gamma invstd|
+    (4u (|g| + |k1| + |xhat k2|) + bar_b / M + |xhat| bar_g / M + |k2| e_xhat) + 2u |dx|.
+    g is dy masked by y_out > 0 (the last BatchNorm of a block and every downsample BatchNorm)
+    or by the BatchNorm's own ReLU, fma(z, scale, shift) > 0 (every other BatchNorm): the
+    float64 sign of z scale + shift is that fma's sign, so the reference masks exactly alike.
+  * bn_act: y = relu(fma(x, s, b) + q), q = fma(r, rs, rb), r or 0: three roundings on the
+    terms, so |d y| <= 4u (|x s| + |b| + |r rs| + |rb|) (|r| for an identity residual); where
+    the float64 value is below minus that bar, y must be exactly 0.
+  * bn_relu_maxpool: the fp32 activations relu(fma(z, s, b)) are recomputed exactly (`_fma32`),
+    the pool restated with the kernel's rule (the first strictly greater value in (kh, kw)
+    order) must give y and argidx bit for bit, and y is within one rounding, u y64, of the
+    float64 pool (the maximum is 1-Lipschitz).
+  * add_masked, im2col, nchw_to_nhwc: data movement and one fp32 add, bit-exact with torch.
+  * Soft-argmax backward (fp32 NHWC) and colsum at C4's shape: the bars of test_gpu_c5_step.
+
+CPU tests below run the gate through the emulated ABI and show against numpy emulations of the
+kernels' arithmetic that each new bar holds for the kernel's order and rejects a plausible
+mistake: M - 1 in k1 / k2, a reduce that ignores y_out, a reduce that drops the last partial CTA,
+bn_act without the residual's affine, a pool that keeps the last maximum or skips the ReLU, and a
+3xTF32 wgrad that loses a correction pass at the longest C4 run."""
+import math
+import re
+
+import numpy as np
+import pytest
+import torch
+
+from tests.test_gpu_c5_step import (KPIX, RUN_BLOCKS3, _check_colsum, _check_softargmax_bwd_fp32,
+                                    _tf32_wgrad_plan)
+from tests.test_gpu_step_kernels import _bench_meta, _cfg, _entry_names, _missing_coverage, _record_calls
+from tests.test_gpu_tf32 import (FPROP_BAR, STATS_SELF_BAR, WGRAD_BAR, _act64, _emul_mma, _fwd64, _geoms,
+                                 _guarded, _layer, _ran, _tc_bar, _tf32_np, _trunc_np)
+
+gpu = pytest.mark.gpu
+
+U = 2.0 ** -24
+EPS = 1e-5
+NB, HWB, JB, DB, HMB = 128, 256, 16, 64, 64      # one GPU's bench batch: 32 tuples x 4 views
+ROWS_PER_THREAD = 64                             # bn.cu kRowsPerThread
+
+S = "test_gpu_tf32x3_step.py::"
+SK = "test_gpu_step_kernels.py::"
+COVERAGE_TF32X3 = {
+    "epb_nchw_to_nhwc": [S + "test_tf32x3_nchw_to_nhwc_bit_exact"],
+    "epb_im2col": [S + "test_tf32x3_im2col_bit_exact_at_stem"],
+    "epb_conv_fprop": [S + "test_tf32x3_conv_layers_vs_float64"],
+    "epb_conv_wgrad": [S + "test_tf32x3_conv_layers_vs_float64", S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
+    "epb_bn_finalize": [S + "test_tf32x3_bn_finalize_vs_float64", SK + "test_bn_finalize_vs_float64_at_bench_M"],
+    "epb_bn_relu_maxpool": [S + "test_tf32x3_bn_relu_maxpool_vs_float64"],
+    "epb_bn_act": [S + "test_tf32x3_bn_act_vs_float64"],
+    "epb_bn_bwd_reduce": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
+    "epb_bn_bwd_apply": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
+    "epb_add_masked": [S + "test_tf32x3_add_masked_bit_exact"],
+    "epb_maxpool_bwd": [SK + "test_maxpool_bwd_vs_float64_at_stem_bench_size"],
+    "epb_softargmax_fwd": [SK + "test_softargmax_fwd_vs_float64_at_bench_shape"],
+    "epb_softargmax_bwd": [S + "test_tf32x3_softargmax_bwd_fp32_vs_float64"],
+    "epb_colsum": [S + "test_tf32x3_colsum_vs_float64"],
+    "epb_jointloss_fwd_bwd": [SK + "test_jointloss_vs_float64_at_bench_shape"],
+    "epb_pack_weight_batch": [S + "test_tf32x3_pack_weight_batch_bit_exact_on_model_jobs",
+                              S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
+    "epb_adam_step_dev": [S + "test_tf32x3_fused_adam_vs_float64_on_model_buffer"],
+    "epb_patch_to_image": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_triangulate": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_project_labels": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+}
+# the fp32 engine's own entries: the f16x3 step calls none of them
+FP32_ENGINE = {"epb_nchw_to_nhwc", "epb_im2col", "epb_conv_fprop", "epb_conv_wgrad", "epb_bn_finalize",
+               "epb_bn_relu_maxpool", "epb_bn_act", "epb_bn_bwd_reduce", "epb_bn_bwd_apply", "epb_add_masked",
+               "epb_softargmax_bwd", "epb_colsum"}
+_THREE_PASS = re.compile(r"^(fprop|wgrad)_tc<\d+,3>$")
+
+
+def _all_three_pass(tags):
+    """every conv kernel tag _ran reported is a 3xTF32 tensor-core instantiation"""
+    return bool(tags) and all(_THREE_PASS.match(t) for t in tags)
+
+
+# every distinct conv of R50 at 256 x 256 (trunk at 64 / 32 / 16 / 8, deconvs 8 -> 64, the final
+# 1 x 1 with bias), the stem as a 1 x 1 conv over its 160-column patch matrix; (name, kind, cin,
+# cout, k, stride, pad, input hw, operand, dgrad).  operand "in": a materialised tensor (patch
+# matrix, pool or block output); "act": the producer's BatchNorm + ReLU applied on load.
+# dgrad "write", "acc" (a downsample adds into the block's input gradient) or None (the stem).
+C4_LAYERS = [
+    ("stem_col_160_64", "conv", 160, 64, 1, 1, 0, 128, "in", None),
+    ("l1_1x1_64_64", "conv", 64, 64, 1, 1, 0, 64, "in", "write"),
+    ("l1_3x3_64", "conv", 64, 64, 3, 1, 1, 64, "act", "write"),
+    ("l1_1x1_64_256", "conv", 64, 256, 1, 1, 0, 64, "act", "write"),
+    ("l1_down_64_256", "conv", 64, 256, 1, 1, 0, 64, "in", "acc"),
+    ("l1_1x1_256_64", "conv", 256, 64, 1, 1, 0, 64, "in", "write"),
+    ("l2_1x1_256_128", "conv", 256, 128, 1, 1, 0, 64, "in", "write"),
+    ("l2_3x3_s2_128", "conv", 128, 128, 3, 2, 1, 64, "act", "write"),
+    ("l2_1x1_128_512", "conv", 128, 512, 1, 1, 0, 32, "act", "write"),
+    ("l2_down_s2_256_512", "conv", 256, 512, 1, 2, 0, 64, "in", "acc"),
+    ("l2_1x1_512_128", "conv", 512, 128, 1, 1, 0, 32, "in", "write"),
+    ("l2_3x3_128", "conv", 128, 128, 3, 1, 1, 32, "act", "write"),
+    ("l3_1x1_512_256", "conv", 512, 256, 1, 1, 0, 32, "in", "write"),
+    ("l3_3x3_s2_256", "conv", 256, 256, 3, 2, 1, 32, "act", "write"),
+    ("l3_1x1_256_1024", "conv", 256, 1024, 1, 1, 0, 16, "act", "write"),
+    ("l3_down_s2_512_1024", "conv", 512, 1024, 1, 2, 0, 32, "in", "acc"),
+    ("l3_1x1_1024_256", "conv", 1024, 256, 1, 1, 0, 16, "in", "write"),
+    ("l3_3x3_256", "conv", 256, 256, 3, 1, 1, 16, "act", "write"),
+    ("l4_1x1_1024_512", "conv", 1024, 512, 1, 1, 0, 16, "in", "write"),
+    ("l4_3x3_s2_512", "conv", 512, 512, 3, 2, 1, 16, "act", "write"),
+    ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 8, "act", "write"),
+    ("l4_down_s2_1024_2048", "conv", 1024, 2048, 1, 2, 0, 16, "in", "acc"),
+    ("l4_1x1_2048_512", "conv", 2048, 512, 1, 1, 0, 8, "in", "write"),
+    ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 8, "act", "write"),
+    ("deconv0_2048_256", "deconv", 2048, 256, 4, 2, 1, 8, "in", "write"),
+    ("deconv1_256", "deconv", 256, 256, 4, 2, 1, 16, "act", "write"),
+    ("deconv2_256", "deconv", 256, 256, 4, 2, 1, 32, "act", "write"),
+    ("final_256_1024", "conv", 256, JB * DB, 1, 1, 0, 64, "act", "write"),
+]
+
+
+def _wgrad_runs(layer, N=NB):
+    """(pixels N Hp Wp, Cin, Cout, taps) of each wgrad geometry of a C4_LAYERS row: one for a
+    convolution, one per output phase (2 x 2, 4 taps each) for the 4 x 4 / 2 deconvolutions"""
+    _, kind, cin, cout, k, s, p, hw, _, _ = layer
+    if kind == "conv":
+        ho = (hw + 2 * p - k) // s + 1
+        return [(N * ho * ho, cin, cout, k * k)]
+    return [(N * hw * hw, cin, cout, 4)] * 4
+
+
+def _wgrad_run(layer):
+    """the longest pixel run of one CTA over the layer's wgrad geometries"""
+    return max(_tf32_wgrad_plan(M, ci, co, T, 3)[0] for M, ci, co, T in _wgrad_runs(layer))
+
+
+# ------------------------------------------------------------------ coverage gate, CPU
+def test_coverage_tf32x3_gate_has_teeth():
+    """Deleting any row, or pointing one at a test that does not exist, fails the gate; the kernel
+    tag check rejects a single-pass or CUDA-core conv among three-pass ones."""
+    rec = sorted(COVERAGE_TF32X3)
+    assert _missing_coverage(rec, COVERAGE_TF32X3) == ([], [])
+    for k in rec:
+        t = dict(COVERAGE_TF32X3)
+        del t[k]
+        assert _missing_coverage(rec, t)[0] == [k]
+    for k in rec:
+        t = dict(COVERAGE_TF32X3)
+        t[k] = [S + "test_no_such_test"]
+        assert _missing_coverage(rec, t)[1]
+    good = {"fprop_tc<64,3>", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
+    assert _all_three_pass(good)
+    for bad in ("fprop_tc<128,1>", "wgrad_tc<64,1>", "wgrad_simt", "fprop_simt"):
+        assert not _all_three_pass(good | {bad})
+    assert not _all_three_pass(set())
+
+
+def test_coverage_tf32x3_gate_cpu_emulated_step():
+    """One tf32x3 training step (R18, J = 16, D = 64, 2 tuples x 4 views of 64 x 64) through the
+    emulated ABI: GraphedTrainStep.eager_step, SmoothL1JointLocationLoss, FusedAdam, given labels
+    (no CPU geometry).  The model runs net.Engine at precision 3 and the step records the fp32
+    engine's entries; every entry has a row."""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    import lib.utils.utils as Ut
+    from epipolarpose_b200 import net, ops
+    from tests import emul_ops
+    rec, depth, saved = set(), [0], {}
+    for k, e in _entry_names(ops).items():
+        if not hasattr(emul_ops, k):
+            continue
+        f = saved[k] = getattr(emul_ops, k)
+
+        def wrap(*a, _f=f, _e=e, **kw):
+            if depth[0] == 0:
+                rec.update(_e)
+            depth[0] += 1
+            try:
+                return _f(*a, **kw)
+            finally:
+                depth[0] -= 1
+        setattr(emul_ops, k, wrap)
+    il._backend[0], Ut._backend[0] = emul_ops, emul_ops
+    try:
+        J, D, HW, B = JB, DB, 64, 8
+        torch.manual_seed(0)
+        m = models.pose3d_resnet.get_pose_net(_cfg(18, J, D, HW), False, ops=emul_ops, precision="tf32x3").train()
+        eng = m._engine()
+        assert type(eng) is net.Engine and eng.precision == 3 and eng.wgrad_precision == 3
+        opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+        step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
+        g = torch.Generator().manual_seed(1)
+        loss = step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
+                               torch.ones(B, J * 3), None)
+        assert math.isfinite(float(loss))
+    finally:
+        for k, f in saved.items():
+            setattr(emul_ops, k, f)
+        il._backend[0] = Ut._backend[0] = ops
+    print("emulated tf32x3 step calls: %s" % sorted(rec))
+    assert FP32_ENGINE <= rec, sorted(FP32_ENGINE - rec)
+    assert not any(e.endswith("_split") or "conv16" in e for e in rec), sorted(rec)
+    missing, dangling = _missing_coverage(rec, COVERAGE_TF32X3)
+    assert not missing, "entries without a float64 test at bench size: %s" % missing
+    assert not dangling, dangling
+
+
+def test_c4_layer_table_wgrad_runs():
+    """The restated planner over C4_LAYERS at N = 128: every run within the three-pass cap, and
+    the bar of the longest run under 1e-4."""
+    runs = [(c[0], _wgrad_run(c)) for c in C4_LAYERS]
+    for name, r in runs:
+        assert 0 < r <= RUN_BLOCKS3 * KPIX and r % KPIX == 0, (name, r)
+    R = max(r for _, r in runs)
+    print("longest C4 wgrad run: %d pixels (%s), bar %.2e" % (R, [n for n, r in runs if r == R], _tc_bar(WGRAD_BAR, R, 3)))
+    assert _tc_bar(WGRAD_BAR, R, 3) <= 1e-4
+
+
+# ------------------------------------------------------------------ bars shared by the CPU and GPU tests
+def _bn_stats64(x):
+    """float64 batch mean and invstd of x [M, C] (the fp32 eps, as bn_finalize adds it)"""
+    xd = x.double()
+    mu = xd.mean(0)
+    var = (xd - mu).pow(2).mean(0)
+    return mu, 1 / torch.sqrt(var + float(np.float32(EPS)))
+
+
+def _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv):
+    """float64 BatchNorm backward of g = dy * keep on x [M, C] with batch statistics (mu, inv),
+    and the module's bars: (dbeta, dgamma, dx, bar_b, bar_g, bar_dx)"""
+    M = x.shape[0]
+    g = dy.double() * keep
+    xh = (x.double() - mu) * inv
+    sg, sgx = g.sum(0), (g * xh).sum(0)
+    d = ROWS_PER_THREAD + 2
+    ag = g.abs()
+    e_xh = 4 * U * (xh.abs() + mu.abs() * inv)
+    bar_b = d * U * ag.sum(0)
+    bar_g = (d + 1) * U * (ag * xh.abs()).sum(0) + (ag * e_xh).sum(0)
+    k1, k2 = sg / M, sgx / M
+    a = gamma.double() * inv
+    dx = a * (g - k1 - xh * k2)
+    bar = a.abs() * (4 * U * (ag + k1.abs() + (xh * k2).abs()) + bar_b / M + xh.abs() * (bar_g / M)
+                     + k2.abs() * e_xh) + 2 * U * dx.abs()
+    return sg, sgx, dx, bar_b, bar_g, bar
+
+
+def _bn_bwd_ratios(dbeta, dgamma, dx, ref):
+    """worst err / bar of dbeta, dgamma (each after its one fp32 rounding) and dx"""
+    sg, sgx, dx64, bar_b, bar_g, bar = ref
+    eb = ((dbeta.double() - sg).abs() - U * sg.abs()).clamp_min(0) / (bar_b + 1e-300)   # a fully masked
+    eg = ((dgamma.double() - sgx).abs() - U * sgx.abs()).clamp_min(0) / (bar_g + 1e-300)  # channel: 0 / 0
+    ex = (dx.double() - dx64).abs() / (bar + 1e-300)
+    return float(eb.max()), float(eg.max()), float(ex.max())
+
+
+def _fma_np(x, s, b):
+    return (x.astype(np.float64) * s + b).astype(np.float32)
+
+
+def _emul_bn_bwd(dy, x, y_out, scale, shift, mean, invstd, gamma, relu, mistake=None):
+    """bn_bwd_reduce_kernel, bn_bwd_coef_kernel and bn_bwd_apply_kernel in numpy fp32 for
+    C4 <= 256 (one channel chunk, rpi = 256 / C4 row slots).  mistake: "m_minus_1" (M - 1 in k1
+    and k2), "ignore_y_out" (the ReLU mask of z in place of y_out > 0), "drop_last_cta" (the
+    reduce loses its last, partial CTA)"""
+    f = np.float32
+    M, C = x.shape
+    rpi = max(256 // (C // 4), 1)
+    per = rpi * ROWS_PER_THREAD
+    ctas = -(-M // per)
+    if y_out is not None and mistake != "ignore_y_out":
+        keep = y_out > 0
+    elif relu or mistake == "ignore_y_out":
+        keep = _fma_np(x, scale, shift) > 0
+    else:
+        keep = np.ones_like(x, dtype=bool)
+    g = np.where(keep, dy, f(0)).astype(f)
+    xm = (x - mean).astype(f)
+    t = ((g * xm).astype(f) * invstd).astype(f)
+    pad = lambda a: np.concatenate([a, np.zeros((ctas * per - M, C), f)]).reshape(ctas, ROWS_PER_THREAD, rpi, C)
+    gp, tp = pad(g), pad(t)
+    a0 = np.zeros((ctas, rpi, C), f)
+    a1 = np.zeros((ctas, rpi, C), f)
+    for k in range(ROWS_PER_THREAD):                   # row r0 + k rpi + slot, in fp32
+        a0 = (a0 + gp[:, k]).astype(f)
+        a1 = (a1 + tp[:, k]).astype(f)
+    if mistake == "drop_last_cta":
+        a0, a1 = a0[:-1], a1[:-1]
+    sg = a0.astype(np.float64).sum((0, 1))
+    sgx = a1.astype(np.float64).sum((0, 1))
+    Md = M - 1 if mistake == "m_minus_1" else M
+    k0 = (gamma.astype(np.float64) * invstd).astype(f)
+    k1, k2 = (sg / Md).astype(f), (sgx / Md).astype(f)
+    inner = ((g - k1).astype(f) - ((xm * invstd).astype(f) * k2).astype(f)).astype(f)
+    return (k0 * inner).astype(f), sgx.astype(f), sg.astype(f)
+
+
+def _bn_bwd_case_np(M, C, seed, relu):
+    """z with per-channel means, dy with per-channel means (gradients rarely centre), y_out"""
+    rng = np.random.default_rng(seed)
+    f = np.float32
+    x = (rng.standard_normal((M, C)) * rng.uniform(0.2, 2.2, C) + rng.standard_normal(C) * 2).astype(f)
+    dy = ((rng.standard_normal((M, C)) + rng.standard_normal(C) * 0.5) * 1e-4).astype(f)
+    gamma = rng.uniform(0.5, 1.5, C).astype(f)
+    beta = (rng.standard_normal(C) * 0.1).astype(f)
+    mu, inv = _bn_stats64(torch.from_numpy(x))
+    scale = (gamma * inv.numpy()).astype(f)
+    shift = (beta - mu.numpy() * gamma * inv.numpy()).astype(f)
+    y_out = None if relu else np.maximum(rng.standard_normal((M, C)), 0).astype(f)
+    return x, dy, y_out, scale, shift, mu, inv, gamma
+
+
+@pytest.mark.parametrize("mistake", ["m_minus_1", "ignore_y_out", "drop_last_cta"])
+def test_bn_bwd_bars_hold_for_the_kernel_order_and_reject(mistake):
+    """The fp32 emulation of the reduce / coef / apply kernels meets the dbeta, dgamma and dx bars
+    in both mask forms; the named mistake misses one of them.  M - 1 and y_out at M = 8192 (the
+    smallest M of the step, where k1 and k2 move most), the dropped CTA at a ragged M = 8169."""
+    M, C = (8192 - 23, 64) if mistake == "drop_last_cta" else (8192, 64)
+    worst_ok, worst_bad = 0.0, 0.0
+    for relu in ((0,) if mistake == "ignore_y_out" else (0, 1)):
+        x, dy, y_out, scale, shift, mu, inv, gamma = _bn_bwd_case_np(M, C, 5 + relu, relu)
+        mean, invstd = mu.float().numpy(), inv.float().numpy()
+        keep = torch.from_numpy(y_out > 0 if y_out is not None else _fma_np(x, scale, shift) > 0)
+        ref = _bn_bwd_ref_bar(torch.from_numpy(x), torch.from_numpy(dy), keep, torch.from_numpy(gamma), mu, inv)
+        T = torch.from_numpy
+        dx, dg, db = _emul_bn_bwd(dy, x, y_out, scale, shift, mean, invstd, gamma, relu)
+        worst_ok = max(worst_ok, *_bn_bwd_ratios(T(db), T(dg), T(dx), ref))
+        dx, dg, db = _emul_bn_bwd(dy, x, y_out, scale, shift, mean, invstd, gamma, relu, mistake)
+        worst_bad = max(worst_bad, *_bn_bwd_ratios(T(db), T(dg), T(dx), ref))
+    print("emulated BatchNorm backward: worst err / bar %.3f; %s: %.3g" % (worst_ok, mistake, worst_bad))
+    assert worst_ok <= 1.0
+    assert worst_bad > 2.0
+
+
+def _bn_act_ref_bar(x, s, b, r, rs, rb):
+    """float64 x s + b (+ r rs + rb, or + r) and the bar 4u on its terms"""
+    xd = x.double()
+    t = xd * s.double() + b.double()
+    terms = (xd * s.double()).abs() + b.double().abs()
+    if r is not None:
+        rd = r.double()
+        if rs is not None:
+            t = t + rd * rs.double() + rb.double()
+            terms = terms + (rd * rs.double()).abs() + rb.double().abs()
+        else:
+            t = t + rd
+            terms = terms + rd.abs()
+    return t, 4 * U * terms
+
+
+def _bn_act_check(y, t, bar):
+    """(worst |y - relu(t)| / bar, elements below -bar that are not exactly 0, negative y)"""
+    err = (y.double() - t.clamp_min(0)).abs()
+    dead = t < -bar
+    return (float((err / (bar + 1e-300)).max()), int((dead & (y != 0)).sum()), int((y < 0).sum()))
+
+
+def test_bn_act_bar_rejects_a_residual_without_its_affine():
+    """The fp32 emulation of bn_act (residual with the downsample BatchNorm's affine) meets the
+    bar with its exact zeros; adding the raw residual misses it."""
+    rng = np.random.default_rng(9)
+    f = np.float32
+    M, C = 4096, 64
+    x = (rng.standard_normal((M, C)) * 2 + 0.3).astype(f)
+    r = (rng.standard_normal((M, C)) * 1.5 - 0.2).astype(f)
+    s, b = rng.uniform(0.2, 1.5, C).astype(f), (rng.standard_normal(C) * 0.5).astype(f)
+    rs, rb = rng.uniform(0.2, 1.5, C).astype(f), (rng.standard_normal(C) * 0.5).astype(f)
+    ok = np.maximum((_fma_np(x, s, b) + _fma_np(r, rs, rb)).astype(f), 0)
+    bad = np.maximum((_fma_np(x, s, b) + r).astype(f), 0)
+    T = torch.from_numpy
+    t, bar = _bn_act_ref_bar(T(x), T(s), T(b), T(r), T(rs), T(rb))
+    r_ok, r_bad = _bn_act_check(T(ok), t, bar), _bn_act_check(T(bad), t, bar)
+    print("emulated bn_act: %s; residual without its affine: %s" % (r_ok, r_bad))
+    assert r_ok[0] <= 1.0 and r_ok[1:] == (0, 0)
+    assert r_bad[0] > 10.0 and r_bad[1] > 0
+
+
+def _fma32(x, s, b):
+    """fp32 fma(x, s, b) as the kernel rounds it, broadcast over the last axis: x s is exact in
+    double, and the TwoSum error of the double sum settles the one case in which rounding that
+    sum to fp32 differs from rounding the exact value (a double on an fp32 midpoint)"""
+    p = x.double() * s.double()
+    bd = b.double().expand_as(p)
+    s64 = p + bd
+    a = s64 - bd
+    e = (p - a) + (bd - (s64 - a))
+    del p, bd, a
+    f = s64.float()
+    f64 = f.double()
+    up = torch.nextafter(f, torch.tensor(float("inf"), device=f.device))
+    dn = torch.nextafter(f, torch.tensor(float("-inf"), device=f.device))
+    f = torch.where((s64 == (f64 + up.double()) / 2) & (e > 0), up, f)
+    f = torch.where((s64 == (f64 + dn.double()) / 2) & (e < 0), dn, f)
+    return f
+
+
+def _pool_restated(z, s, b, last=False, relu=True):
+    """bn_relu_maxpool_kernel in torch on the exact fp32 activations: (y, argidx) from the first
+    strictly greater value in (kh, kw) order (last: the last of equal maxima), and the float64
+    pool y64 of relu(z s + b)"""
+    n, H, W, C = z.shape
+    Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+    a32 = _fma32(z, s, b)
+    a64 = z.double() * s.double() + b.double()
+    if relu:
+        a32, a64 = a32.clamp_min(0), a64.clamp_min(0)
+    p32 = torch.full((n, H + 2, W + 2, C), float("-inf"), device=z.device)
+    p64 = torch.full((n, H + 2, W + 2, C), float("-inf"), device=z.device, dtype=torch.float64)
+    p32[:, 1:-1, 1:-1], p64[:, 1:-1, 1:-1] = a32, a64
+    del a32, a64
+    best = torch.full((n, Ho, Wo, C), float("-inf"), device=z.device)
+    y64 = torch.full((n, Ho, Wo, C), float("-inf"), device=z.device, dtype=torch.float64)
+    arg = torch.zeros((n, Ho, Wo, C), device=z.device, dtype=torch.uint8)
+    for kh in range(3):
+        for kw in range(3):
+            v = p32[:, kh:kh + 2 * Ho:2, kw:kw + 2 * Wo:2]
+            take = (v >= best) & (v > float("-inf")) if last else v > best
+            best = torch.where(take, v, best)
+            arg = torch.where(take, torch.full_like(arg, kh * 3 + kw), arg)
+            y64 = torch.maximum(y64, p64[:, kh:kh + 2 * Ho:2, kw:kw + 2 * Wo:2])
+    return best, arg, y64
+
+
+def _pool_errors(y, arg, z, s, b):
+    """(y bit-equal to the restated pool, argidx equal, worst |y - y64| / (u y64), windows whose
+    maximum is a ReLU zero)"""
+    yk, ak, y64 = _pool_restated(z, s, b)
+    err = (y.double() - y64).abs()
+    ratio = float((err / (U * y64)).nan_to_num(0.0, posinf=float("inf")).max()) if bool((err > 0).any()) else 0.0
+    return (torch.equal(y.view(torch.int32), yk.view(torch.int32)), torch.equal(arg, ak), ratio,
+            int((y64 == 0).sum()))
+
+
+def test_pool_restatement_rejects_the_last_maximum_and_a_missing_relu():
+    """A numpy emulation of bn_relu_maxpool on dyadic inputs (many equal maxima) and on random
+    fp32 inputs matches the restatement bit for bit within u y64; keeping the last of equal
+    maxima fails the argidx check, skipping the ReLU fails the value check."""
+    rng = np.random.default_rng(13)
+    f = np.float32
+    n, H, W, C = 2, 17, 16, 8
+    for dyadic in (True, False):
+        z = rng.standard_normal((n, H, W, C))
+        z = (np.round(z * 8) / 8 if dyadic else z).astype(f)
+        s = (np.round(rng.uniform(0.5, 1.5, C) * 16) / 16 if dyadic else rng.uniform(0.5, 1.5, C)).astype(f)
+        b = (np.round(rng.standard_normal(C) * 0.3 * 16) / 16 if dyadic else rng.standard_normal(C) * 0.3).astype(f)
+        T = torch.from_numpy
+        Ho, Wo = (H - 1) // 2 + 1, (W - 1) // 2 + 1
+        act = _fma_np(z, s, b)
+
+        def emul(last, relu):
+            a = np.maximum(act, 0) if relu else act
+            y = np.full((n, Ho, Wo, C), -np.inf, f)
+            ai = np.zeros((n, Ho, Wo, C), np.uint8)
+            for oh in range(Ho):
+                for ow in range(Wo):
+                    for kh in range(3):
+                        for kw in range(3):
+                            ih, iw = 2 * oh - 1 + kh, 2 * ow - 1 + kw
+                            if 0 <= ih < H and 0 <= iw < W:
+                                v = a[:, ih, iw]
+                                t = v >= y[:, oh, ow] if last else v > y[:, oh, ow]
+                                y[:, oh, ow] = np.where(t, v, y[:, oh, ow])
+                                ai[:, oh, ow] = np.where(t, kh * 3 + kw, ai[:, oh, ow])
+            return T(y), T(ai)
+        same, arg_ok, ratio, zeros = _pool_errors(*emul(False, True), T(z), T(s), T(b))
+        assert same and arg_ok and ratio <= 1.0, (dyadic, same, arg_ok, ratio)
+        if dyadic:
+            assert zeros > 0
+            assert not _pool_errors(*emul(True, True), T(z), T(s), T(b))[1]
+        y_nr, a_nr = emul(False, False)
+        r = _pool_errors(y_nr, a_nr, T(z), T(s), T(b))
+        assert not r[0] and r[2] > 1.0
+        print("pool emulation (%s): bit-equal, %d ReLU-zero maxima; without ReLU: err / bar %.3g"
+              % ("dyadic" if dyadic else "random", zeros, r[2]))
+
+
+def test_tf32_wgrad_bar_rejects_a_lost_correction_pass_at_the_longest_c4_run():
+    """The wgrad product at the longest pixel run of C4_LAYERS (R from the planner), with the
+    toward-zero accumulation of test_gpu_tf32: 3xTF32 meets _tc_bar(WGRAD_BAR, R, 3); dropping
+    the dout lo pass or the activation lo pass misses it."""
+    R = max(_wgrad_run(c) for c in C4_LAYERS)
+    rng = np.random.default_rng(17)
+    co, ci = 128, 64
+    a = (rng.standard_normal((co, R)) * 1e-3).astype(np.float32)         # dz^T
+    b = np.maximum(rng.standard_normal((R, ci)), 0).astype(np.float32)    # relu(BN(z)) of the producer
+    ah, bh = _tf32_np(a), _tf32_np(b)
+    al, bl = _trunc_np(a - ah), _trunc_np(b - bh)
+    ref = a.astype(np.float64) @ b.astype(np.float64)
+    e = lambda x: float(np.max(np.abs(x - ref)) / np.max(np.abs(ref)))
+    full = e(_emul_mma([(al, bh), (ah, bl), (ah, bh)], R, True))
+    no_alo = e(_emul_mma([(ah, bl), (ah, bh)], R, True))
+    no_blo = e(_emul_mma([(al, bh), (ah, bh)], R, True))
+    bar = _tc_bar(WGRAD_BAR, R, 3)
+    print("R = %d: 3xTF32 %.2e, dout lo lost %.2e, activation lo lost %.2e, bar %.2e" % (R, full, no_alo, no_blo, bar))
+    assert full <= bar
+    assert min(no_alo, no_blo) > bar
+
+
+# ------------------------------------------------------------------ GPU fixtures
+@pytest.fixture(scope="module")
+def dev():
+    from epipolarpose_b200 import ops
+    ops.device_check()
+    return torch.device("cuda:0")
+
+
+_MODEL = {}
+
+
+@pytest.fixture(scope="module", autouse=True)
+def _release_device_memory():
+    """After the module, drop its cached model and hand the allocator's reserve back to the
+    device for the tests after it; report the module's peak allocation."""
+    if torch.cuda.is_available() and torch.cuda.is_initialized():
+        torch.cuda.reset_peak_memory_stats()
+    yield
+    _MODEL.clear()
+    if torch.cuda.is_initialized():
+        import gc
+        gc.collect()
+        print("\n  tf32x3 step module: peak device allocation %.1f GB" % (torch.cuda.max_memory_allocated() / 2 ** 30))
+        torch.cuda.empty_cache()
+
+
+def _r50(dev):
+    """the bench model (R50, J = 16, D = 64, 256 x 256) on net.Engine at precision 3, with
+    FusedAdam over its parameters"""
+    if "m" not in _MODEL:
+        import lib.models as models
+        import lib.utils.utils as Ut
+        from epipolarpose_b200 import net
+        torch.manual_seed(0)
+        m = models.pose3d_resnet.get_pose_net(_cfg(50, JB, DB, HWB), False, precision="tf32x3").to(dev).train()
+        assert type(m._engine()) is net.Engine and m._engine().precision == 3
+        _MODEL["m"] = m
+        _MODEL["opt"] = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    return _MODEL["m"], _MODEL["opt"]
+
+
+# ------------------------------------------------------------------ 1. coverage gate, GPU half
+@gpu
+def test_coverage_tf32x3_gate_step(dev):
+    """One tf32x3 bench-composition step at a reduced batch (R50, J = 16, D = 64, 2 tuples x 4
+    views of 256 x 256): GraphedTrainStep(online=True, method="iterative").eager_step, SmoothL1,
+    FusedAdam, under the profiler.  Every entry it calls has a row in COVERAGE_TF32X3 naming
+    existing tests, and every conv kernel that ran is a three-pass instantiation."""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    import lib.utils.img_utils as iu
+    import lib.utils.utils as Ut
+    tuples = 2
+    B = 4 * tuples
+    torch.manual_seed(0)
+    m = models.pose3d_resnet.get_pose_net(_cfg(50, JB, DB, HWB), False, precision="tf32x3").to(dev).train()
+    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(JB).to(dev), opt, online=True, method="iterative")
+    meta = iu.pack_meta({k: v.to(dev) for k, v in _bench_meta(tuples).items()}, B, dev)
+    x = torch.randn(B, 3, HWB, HWB, device=dev)
+    losses = []
+    with _record_calls() as names:
+        tags = _ran(lambda: losses.append(float(step.eager_step(x, None, None, meta))))
+        torch.cuda.synchronize()
+    assert losses and all(math.isfinite(v) for v in losses)
+    print("  tf32x3 step calls %d entries; conv kernels %s" % (len(names), sorted(tags)))
+    for e in sorted(names):
+        print("    %-28s -> %s" % (e, ", ".join(COVERAGE_TF32X3.get(e, ["(none)"]))))
+    assert FP32_ENGINE <= names, sorted(FP32_ENGINE - names)
+    assert "epb_adam_step_dev" in names and "epb_triangulate" in names
+    assert _all_three_pass(tags), "a conv of the tf32x3 step ran below three passes: %s" % sorted(tags)
+    assert any(t.startswith("fprop") for t in tags) and any(t.startswith("wgrad") for t in tags), tags
+    missing, dangling = _missing_coverage(names, COVERAGE_TF32X3)
+    assert not missing, "entries without a float64 test at bench size: %s" % missing
+    assert not dangling, dangling
+
+
+# ------------------------------------------------------------------ 2. convolutions at N = 128
+@gpu
+@pytest.mark.parametrize("layer", C4_LAYERS, ids=[c[0] for c in C4_LAYERS])
+def test_tf32x3_conv_layers_vs_float64(dev, layer):
+    """fprop (statistics into a zeroed buffer, or the bias for the final layer), dgrad (written,
+    or added into the block's input gradient for a downsample) and wgrad (into a zeroed dW) at
+    N = 128 with the step's operand mode, each against torch float64 within its bar; every
+    output followed by a guard band, every kernel a three-pass instantiation."""
+    import torch.nn.functional as F
+    from epipolarpose_b200 import ops
+    name, kind, cin, cout, k, s, p, hw, operand, dmode = layer
+    N = NB
+    final = name.startswith("final")
+    conv, Ho, Wo, x, sc, sh, w, gout = _layer(dev, kind, cin, cout, k, s, p, 0, N, hw, hw, 17)
+    ci, co, T = conv.cin_p, conv.cout_p, k * k
+    act = operand == "act"
+    aff = (sc, sh) if act else (None, None)
+    wf, wd = conv.pack(ops, w)
+    tags, errs = set(), {}
+    # ---- fprop
+    bias = torch.randn(co, device=dev, generator=torch.Generator(device=dev).manual_seed(5)) * 0.5 if final else None
+    geoms = conv.fprop_geoms(ops, N, hw, hw, 3)
+    gms = _geoms(geoms, int(act), 0)
+    out, guard = _guarded((N, Ho, Wo, co), dev, 0.0 if any(gm is None for gm in geoms) else float("nan"))
+    guard.fill_(1234.5)
+    stats = sguard = None
+    if not final:
+        sbuf = torch.zeros(2 * co + 64, device=dev, dtype=torch.float64)
+        stats, sguard = sbuf[:2 * co], sbuf[2 * co:]
+
+    def fwd(o, st):
+        for gm in gms:
+            ops.conv_fprop(gm, x, wf, o, aff[0], aff[1], bias, st)
+    tags |= _ran(lambda: fwd(out.clone(), None if stats is None else stats.clone()))
+    fwd(out, stats)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "fprop guard band overwritten"
+    a64 = _act64(x, *aff, act)
+    with torch.no_grad():
+        ref = _fwd64(conv, a64, w.double())
+        if bias is not None:
+            ref += bias.double()[None, :, None, None]
+        ref = ref.permute(0, 2, 3, 1)
+        bar_f = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in gms), 3)
+        errs["fprop"] = float((out.double() - ref).abs().max() / ref.abs().max())   # NaN fails
+        if stats is not None:
+            assert bool((sguard == 0).all()), "statistics guard band overwritten"
+            o = out.double().reshape(-1, co)
+            s1, s2 = stats[:co], stats[co:]
+            errs["st_self"] = max(float(((s1 - o.sum(0)).abs() / o.abs().sum(0).clamp_min(1e-300)).max()),
+                                  float(((s2 - (o * o).sum(0)).abs() / (o * o).sum(0).clamp_min(1e-300)).max()))
+            del o
+            r = ref.reshape(-1, co)
+            r2 = (r * r).sum(0)
+            errs["st_ref"] = max(float(((s1 - r.sum(0)).abs() / r.abs().sum(0).clamp_min(1e-300)).max()),
+                                 float((s2 - r2).abs().max() / r2.abs().max()))
+            del r, r2
+    del out, ref
+    # ---- dgrad
+    bar_d = None
+    if dmode is not None:
+        dgeoms = conv.dgrad_geoms(ops, N, hw, hw, 3)
+        acc = int(dmode == "acc")
+        dgms = _geoms(dgeoms, 0, acc)
+        with torch.no_grad():
+            g64, w64 = gout.permute(0, 3, 1, 2).double(), w.double()
+            if kind == "conv":
+                ref = torch.nn.grad.conv2d_input((N, ci, hw, hw), w64, g64, s, p)
+            else:
+                ref = F.conv2d(g64, w64, None, s, p)
+            del g64
+            ref = ref.permute(0, 2, 3, 1)
+        din, guard = _guarded((N, hw, hw, ci), dev, 0.0 if (acc or any(gm is None for gm in dgeoms)) else float("nan"))
+        guard.fill_(1234.5)
+        init = None
+        if acc:
+            init = torch.randn(din.shape, device=dev, generator=torch.Generator(device=dev).manual_seed(9))
+            init *= float(ref.abs().max()) / 3
+            din.copy_(init)
+
+        def bwd(o):
+            for gm in dgms:
+                ops.conv_fprop(gm, gout, wd, o, None, None, None, None)
+        tags |= _ran(lambda: bwd(din.clone()))
+        bwd(din)
+        torch.cuda.synchronize()
+        assert bool((guard == 1234.5).all()), "dgrad guard band overwritten"
+        base = init.double() if init is not None else 0.0
+        errs["dgrad"] = float((din.double() - (base + ref)).abs().max() / ref.abs().max())
+        bar_d = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in dgms), 3)
+        del din, ref, init
+    # ---- wgrad
+    runs = sorted((gm.N * gm.Hp * gm.Wp, gm.Cin, gm.Cout, gm.T) for gm in gms)
+    assert runs == sorted((M, _pad4(a), _pad4(b), t) for M, a, b, t in _wgrad_runs(layer)), runs
+    R = _wgrad_run(layer)
+    bar_w = _tc_bar(WGRAD_BAR, R, 3)
+    w64 = w.double().requires_grad_(True)
+    _fwd64(conv, a64, w64).backward(gout.permute(0, 3, 1, 2).double())
+    del a64
+    gw = w64.grad
+    ref = (gw.permute(0, 2, 3, 1) if kind == "conv" else gw.permute(1, 2, 3, 0)).reshape(co, T, ci)
+    del w64, gw
+    dw, guard = _guarded((co * T * ci,), dev, 0.0)
+    guard.fill_(1234.5)
+
+    def wgr(o):
+        for gm in gms:
+            ops.conv_wgrad(gm, x, gout, o, aff[0], aff[1])
+    tags |= _ran(lambda: wgr(torch.zeros_like(dw)))
+    wgr(dw)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "dW guard band overwritten"
+    errs["wgrad"] = float((dw.view(co, T, ci).double() - ref).abs().max() / ref.abs().max())
+    print("  %-22s %-36s fprop %.2e (bar %.2e)%s%s wgrad %.2e (run %d, bar %.2e)" % (
+        name, ",".join(sorted(tags)), errs["fprop"], bar_f,
+        " stats %.1e / %.1e" % (errs["st_self"], errs["st_ref"]) if "st_self" in errs else "",
+        " dgrad %.2e (bar %.2e)" % (errs["dgrad"], bar_d) if bar_d else "", errs["wgrad"], R, bar_w))
+    assert _all_three_pass(tags), tags
+    assert errs["fprop"] <= bar_f, errs
+    if "st_self" in errs:
+        assert errs["st_self"] <= STATS_SELF_BAR and errs["st_ref"] <= bar_f, errs
+    if bar_d is not None:
+        assert errs["dgrad"] <= bar_d, errs
+    assert errs["wgrad"] <= bar_w, errs
+
+
+def _pad4(c):
+    return (c + 3) // 4 * 4
+
+
+@gpu
+def test_tf32x3_stem_wgrad_through_flat_buffer(dev):
+    """The stem's weight gradient as the engine forms it: images -> nchw_to_nhwc -> im2col (the
+    patch matrix, K padded 147 -> 160), Engine._conv_wgrad(stem_col, col, dz, ..., None) into the
+    step's flat buffer, then the stage's batched unpack.  Columns 147 .. 159 of the [64][160]
+    gradient are exactly zero, and both it and the unpacked [64, 3, 7, 7] gradient match float64
+    within _tc_bar(WGRAD_BAR, R, 3)."""
+    from epipolarpose_b200 import net, ops
+    m, _ = _r50(dev)
+    eng = m._engine()
+    eng.dev = dev
+    N, H = NB, HWB
+    H1 = H // 2
+    kpad = eng.stem_kpad
+    g = torch.Generator(device=dev).manual_seed(23)
+    img = torch.randn(N, 3, H, H, device=dev, generator=g)
+    x = torch.empty(N, H, H, 4, device=dev)
+    ops.nchw_to_nhwc(img, x, N, 3, H, H, 4)
+    del img
+    col = torch.empty(N, H1, H1, kpad, device=dev)
+    ops.im2col(x, col, N, H, H, 4, 3, 7, 7, 2, 3, H1, H1, kpad)
+    del x
+    dz = torch.randn(N, H1, H1, 64, device=dev, generator=g) * 1e-3
+    grads = {k: torch.full_like(v, float("nan")) for k, v in m.named_parameters()}
+    gs = eng._grad_state(grads)
+    gs["flat"].zero_()
+    eng._gs, eng._side = gs, None
+    try:
+        eng._conv_wgrad(eng.stem_col, col, dz, N, H1, H1, None)
+        ops.pack_weight_batch(gs["batches"][net.stage_of("conv1")])
+    finally:
+        eng._gs = None
+    torch.cuda.synchronize()
+    flat = gs["dwp"]["conv1"].view(64, kpad)
+    ref = torch.zeros(64, kpad, device=dev, dtype=torch.float64)
+    step = 1 << 18
+    cf, df = col.view(-1, kpad), dz.view(-1, 64)
+    for r0 in range(0, cf.shape[0], step):
+        ref += df[r0:r0 + step].double().t() @ cf[r0:r0 + step].double()
+    R = _tf32_wgrad_plan(N * H1 * H1, kpad, 64, 1, 3)[0]
+    bar = _tc_bar(WGRAD_BAR, R, 3)
+    scale = float(ref.abs().max())
+    e_flat = float((flat.double() - ref).abs().max()) / scale
+    w = grads["conv1.weight"]
+    ref_w = ref[:, :147].view(64, 7, 7, 3).permute(0, 3, 1, 2)        # [64][(r s c)] -> [64, 3, 7, 7]
+    e_w = float((w.double() - ref_w).abs().max()) / scale               # NaN (not written) fails
+    print("  stem wgrad through the flat buffer: run %d, [64][160] %.2e, unpacked %.2e, bar %.2e"
+          % (R, e_flat, e_w, bar))
+    assert bool((flat[:, 147:] == 0).all()), "K-pad columns of the stem gradient are not zero"
+    assert e_flat <= bar and e_w <= bar
+
+
+# ------------------------------------------------------------------ 3. the fp32 BatchNorm chain
+# (M, C, mask) of every BatchNorm backward of the step: "y_out" for the last BatchNorm of a block
+# and the downsample BatchNorms, "relu" for the stem, the inner BatchNorms and the deconvs'
+BN_BWD = [(2097152, 64, "relu"), (524288, 64, "relu"), (524288, 128, "relu"), (524288, 256, "y_out"),
+          (524288, 256, "relu"), (131072, 128, "relu"), (131072, 256, "relu"), (131072, 512, "y_out"),
+          (32768, 256, "relu"), (32768, 512, "relu"), (32768, 1024, "y_out"), (8192, 512, "relu"),
+          (8192, 2048, "y_out")]
+# make_rowmap beyond the step: a ragged M (not a multiple of rpi x 64 rows), C4 not dividing 256,
+# C4 above 256 with a partial second channel chunk
+BN_EDGE = [(524288 - 23, 256, "y_out"), (131072 - 23, 96, "relu"), (131072 - 23, 160, "y_out"),
+           (32768 - 23, 1152, "relu")]
+
+
+def _check_bn_bwd(dev, M, C, mode):
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(M + C)
+    x = torch.randn(M, C, device=dev, generator=g) * (torch.rand(C, device=dev, generator=g) * 2 + 0.2) \
+        + torch.randn(C, device=dev, generator=g) * 2
+    x[:, 0] = 0.37                                           # var 0: invstd = 1 / sqrt(eps)
+    dy = (torch.randn(M, C, device=dev, generator=g) + torch.randn(C, device=dev, generator=g) * 0.5) * 1e-4
+    dy[M // 2, 1] = 3.0                                      # one huge element
+    gamma = torch.rand(C, device=dev, generator=g) + 0.5
+    beta = torch.randn(C, device=dev, generator=g) * 0.1
+    mu, inv = _bn_stats64(x)
+    mean, invstd = mu.float(), inv.float()
+    scale, shift = (gamma.double() * inv).float(), (beta.double() - mu * gamma.double() * inv).float()
+    y_out = None
+    if mode == "relu":
+        scale[2], shift[2] = 0.0, -1.0                       # a fully masked channel
+        keep = (x.double() * scale.double() + shift.double()) > 0
+    else:
+        y_out = torch.relu(torch.randn(M, C, device=dev, generator=g))
+        y_out[:, 2] = 0
+        keep = y_out > 0
+    relu = int(mode == "relu")
+    sums = torch.zeros(2 * C, device=dev, dtype=torch.float64)
+    dx, dg, db = torch.empty(M, C, device=dev), torch.empty(C, device=dev), torch.empty(C, device=dev)
+    ops.bn_bwd_reduce(dy, x, y_out, scale, shift, mean, invstd, relu, M, C, sums)
+    ops.bn_bwd_apply(dy, x, y_out, scale, shift, mean, invstd, gamma, relu, sums, M, C, dx, dg, db)
+    torch.cuda.synchronize()
+    del y_out
+    ref = _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv)
+    rb, rg, rx = _bn_bwd_ratios(db, dg, dx, ref)
+    print("  bn bwd %7d x %-4d %-5s worst err / bar: dbeta %.3f dgamma %.3f dx %.3f (max dx err %.2e)"
+          % (M, C, mode, rb, rg, rx, float((dx.double() - ref[2]).abs().max())))
+    assert rb <= 1.0 and rg <= 1.0 and rx <= 1.0
+
+
+@gpu
+@pytest.mark.parametrize("M,C,mode", BN_BWD, ids=["%dx%d-%s" % c for c in BN_BWD])
+def test_tf32x3_bn_bwd_vs_float64(dev, M, C, mode):
+    """bn_bwd_reduce + bn_bwd_apply at every (M, C) and mask form of the step: dbeta, dgamma per
+    channel and dx per element against float64, with a constant channel (invstd = 316), one
+    huge gradient element and a fully masked channel beside ordinary ones."""
+    _check_bn_bwd(dev, M, C, mode)
+
+
+@gpu
+@pytest.mark.parametrize("M,C,mode", BN_EDGE, ids=["%dx%d-%s" % c for c in BN_EDGE])
+def test_tf32x3_bn_bwd_edge_shapes(dev, M, C, mode):
+    _check_bn_bwd(dev, M, C, mode)
+
+
+BN_ACT = [(524288, 256), (131072, 512), (32768, 1024), (8192, 2048)]
+
+
+@gpu
+@pytest.mark.parametrize("res", ["affine", "identity", "relu"])
+@pytest.mark.parametrize("M,C", BN_ACT, ids=["%dx%d" % c for c in BN_ACT])
+def test_tf32x3_bn_act_vs_float64(dev, M, C, res):
+    """bn_act at every block output: the residual with the downsample BatchNorm's affine, the
+    identity residual, and ReLU alone; within 4u of the terms, exact zeros below -bar."""
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(M + C + len(res))
+    x = torch.randn(M, C, device=dev, generator=g) * 3 + 0.5
+    s, b = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
+    r = rs = rb = None
+    if res != "relu":
+        r = torch.randn(M, C, device=dev, generator=g) * 2
+        if res == "identity":
+            r = torch.relu(r)                                     # a block output
+        else:
+            rs, rb = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
+    y, guard = _guarded((M, C), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.bn_act(x, s, b, r, rs, rb, 1, y, M, C)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    worst, bad0, neg = 0.0, 0, 0
+    step = max((1 << 24) // C, 1)
+    for r0 in range(0, M, step):
+        sl = slice(r0, r0 + step)
+        t, bar = _bn_act_ref_bar(x[sl], s, b, None if r is None else r[sl], rs, rb)
+        w_, z_, n_ = _bn_act_check(y[sl], t, bar)
+        worst, bad0, neg = max(worst, w_), bad0 + z_, neg + n_
+        del t, bar
+    print("  bn_act %6d x %-4d %-8s worst err / bar %.3f" % (M, C, res, worst))
+    assert worst <= 1.0 and bad0 == 0 and neg == 0, (worst, bad0, neg)
+
+
+@gpu
+def test_tf32x3_bn_relu_maxpool_vs_float64(dev):
+    """The stem's pool at 128 x 128 x 128 x 64 -> 64 x 64: y and argidx bit-equal with the
+    restated kernel (first strictly greater value in (kh, kw) order over the exact fp32
+    activations; ties at ReLU zeros are common), y within u y64 of the float64 pool."""
+    from epipolarpose_b200 import ops
+    N, H, C = NB, HWB // 2, 64
+    Ho = H // 2
+    g = torch.Generator(device=dev).manual_seed(29)
+    z = torch.randn(N, H, H, C, device=dev, generator=g) * 2 + 0.1
+    s = torch.rand(C, device=dev, generator=g) + 0.3
+    b = torch.randn(C, device=dev, generator=g) * 0.5 - 0.6
+    b[:4] = -20.0                                             # channels that are all ReLU zeros
+    y = torch.full((N, Ho, Ho, C), float("nan"), device=dev)
+    arg = torch.full((N, Ho, Ho, C), 255, device=dev, dtype=torch.uint8)
+    ops.bn_relu_maxpool(z, s, b, y, arg, N, H, H, C)
+    torch.cuda.synchronize()
+    same = arg_ok = True
+    worst, zeros = 0.0, 0
+    for n0 in range(0, N, 16):
+        sl = slice(n0, n0 + 16)
+        e_same, e_arg, ratio, nz = _pool_errors(y[sl], arg[sl], z[sl], s, b)
+        same, arg_ok = same and e_same, arg_ok and e_arg
+        worst, zeros = max(worst, ratio), zeros + nz
+    print("  bn_relu_maxpool: bit-equal %s, argidx %s, worst err / (u y64) %.3f, %d ReLU-zero maxima"
+          % (same, arg_ok, worst, zeros))
+    assert same and arg_ok and worst <= 1.0
+    assert zeros > 0
+
+
+ADD_MASKED = [(524288, 256), (131072, 512), (32768, 1024), (8192, 2048)]
+
+
+@gpu
+@pytest.mark.parametrize("M,C", ADD_MASKED, ids=["%dx%d" % c for c in ADD_MASKED])
+def test_tf32x3_add_masked_bit_exact(dev, M, C):
+    """add_masked (a block's input gradient: dgrad + where(block output > 0, incoming, 0)) at
+    every identity block's output size, bit-exact with torch, a guard band untouched."""
+    from epipolarpose_b200 import ops
+    n = M * C
+    g = torch.Generator(device=dev).manual_seed(C)
+    a = torch.randn(n, device=dev, generator=g)
+    b = torch.randn(n, device=dev, generator=g)
+    mask = torch.relu(torch.randn(n, device=dev, generator=g))
+    mask[::7] = -0.0
+    a[::11] = -0.0
+    out, guard = _guarded((n,), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.add_masked(a, b, mask, out, n)
+    torch.cuda.synchronize()
+    ref = a + torch.where(mask > 0, b, torch.zeros_like(b))
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    assert torch.equal(out.view(torch.int32), ref.view(torch.int32))
+    print("  add_masked %d elements bit-exact" % n)
+
+
+@gpu
+def test_tf32x3_im2col_bit_exact_at_stem(dev):
+    """im2col of all 128 images of 256 x 256 (7 x 7 / 2, pad 3, NHWC pitch 4 with a poisoned pad
+    channel) against F.unfold, bit for bit; the K-pad columns 147 .. 159 exactly zero."""
+    import torch.nn.functional as F
+    from epipolarpose_b200 import ops
+    N, H, kpad = NB, HWB, 160
+    H1 = H // 2
+    g = torch.Generator(device=dev).manual_seed(31)
+    x = torch.randn(N, H, H, 4, device=dev, generator=g)
+    x[..., 3] = 1e30                                          # the pad channel is never read
+    col = torch.full((N, H1, H1, kpad), float("nan"), device=dev)
+    ops.im2col(x, col, N, H, H, 4, 3, 7, 7, 2, 3, H1, H1, kpad)
+    torch.cuda.synchronize()
+    for n0 in range(0, N, 16):
+        u = F.unfold(x[n0:n0 + 16, ..., :3].permute(0, 3, 1, 2), 7, padding=3, stride=2)   # [n, (c r s), L]
+        u = u.view(-1, 3, 49, H1 * H1).permute(0, 3, 2, 1).reshape(-1, H1, H1, 147)         # [n, L, (r s c)]
+        c = col[n0:n0 + 16]
+        assert torch.equal(c[..., :147].contiguous().view(torch.int32), u.contiguous().view(torch.int32)), n0
+        assert bool((c[..., 147:].view(torch.int32) == 0).all()), "K-pad columns not zero"
+    print("  im2col: %d images bit-exact, K pad %d" % (N, kpad))
+
+
+@gpu
+def test_tf32x3_nchw_to_nhwc_bit_exact(dev):
+    """nchw_to_nhwc of the bench batch (128 x 3 x 256 x 256 -> pitch 4), bit-exact, the pad
+    channel +0, a guard band untouched."""
+    from epipolarpose_b200 import ops
+    N, H = NB, HWB
+    g = torch.Generator(device=dev).manual_seed(37)
+    src = torch.randn(N, 3, H, H, device=dev, generator=g)
+    dst, guard = _guarded((N, H, H, 4), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.nchw_to_nhwc(src, dst, N, 3, H, H, 4)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    assert torch.equal(dst[..., :3].contiguous().view(torch.int32), src.permute(0, 2, 3, 1).contiguous().view(torch.int32))
+    assert bool((dst[..., 3].view(torch.int32) == 0).all())
+
+
+@gpu
+@pytest.mark.parametrize("M", [131072, 32768, 8192])
+def test_tf32x3_bn_finalize_vs_float64(dev, M):
+    """bn_finalize at the step's other M (the bench test covers 524288 and 2097152)"""
+    from tests.test_gpu_step_kernels import test_bn_finalize_vs_float64_at_bench_M
+    test_bn_finalize_vs_float64_at_bench_M(dev, M)
+
+
+# ------------------------------------------------------------------ 4. the fp32 head at C4's shape
+@gpu
+def test_tf32x3_softargmax_bwd_fp32_vs_float64(dev):
+    """epb_softargmax_bwd (fp32 NHWC) at N = 128, J = 16, D = 64, 64 x 64"""
+    _check_softargmax_bwd_fp32(dev, NB, JB, DB, HMB, HMB)
+
+
+@gpu
+@pytest.mark.parametrize("M", [NB * HMB * HMB, NB * HMB * HMB - 23], ids=["524288", "524265"])
+def test_tf32x3_colsum_vs_float64(dev, M):
+    """epb_colsum over M x 1024 (the final layer's bias gradient; 524265 leaves a partial last CTA)"""
+    _check_colsum(dev, M, JB * DB)
+
+
+# ------------------------------------------------------------------ 5. weights and optimiser on the fp32 engine
+@gpu
+def test_tf32x3_pack_weight_batch_bit_exact_on_model_jobs(dev):
+    """pack_weight_batch on net.Engine's own jobs for R50 / J16 / D64 (every layer's fprop and
+    dgrad operands, the stem's [64][160] patch-matrix operand, the per-stage unpacks of the
+    packed weight gradients), bit-exact with the CPU emulation"""
+    from tests.test_gpu_step_kernels import _check_pack_weight_batch
+    _check_pack_weight_batch(dev, _r50(dev)[0])
+
+
+@gpu
+def test_tf32x3_fused_adam_vs_float64_on_model_buffer(dev):
+    """FusedAdam over the tf32x3 model's flat parameter buffer: steps 1, 2 and 1000"""
+    from tests.test_gpu_step_kernels import _check_fused_adam
+    _check_fused_adam(dev, *_r50(dev))
