@@ -883,6 +883,31 @@ __global__ void pose_to_camera_kernel(const double* __restrict__ joints, const d
   pose_to_camera_sample(joints + (int64_t)s * J * 3, cam + (int64_t)s * 5, J, root, out + (int64_t)s * J * 3);
 }
 
+// --------------------------------------------------------------- pseudo-label records
+// One thread per (frame, camera), cam_pseudo_record (camera.cuh) over its J joints.  X holds S
+// poses per frame: S = 1 serves every camera, S = V one pose per camera.  Every offset is derived
+// from the sizes the entry validated; nothing read from X or status indexes memory.
+__global__ void pseudo_records_kernel(const double* __restrict__ X, const int32_t* __restrict__ status,
+                                      const double* __restrict__ cam, int T, int S, int V, int J, int root,
+                                      double* __restrict__ jt, double* __restrict__ vis,
+                                      double* __restrict__ pelvis, int32_t* __restrict__ ok) {
+  const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (int64_t)T * V) return;
+  const int64_t t = i / V, v = i % V;
+  const int64_t s = t * S + (S == 1 ? 0 : v);
+  ok[i] = cam_pseudo_record(X + s * J * 3, status + s * J, cam + i * 16, J, root, jt + i * J * 3, vis + i * J * 3,
+                            pelvis + i * 3);
+}
+
+// The size checks of epb_pseudo_records, on the host before any launch.
+int pseudo_records_sizes(int T, int S, int V, int J, int root) {
+  EPB_CHECK_ARG(T >= 0 && S >= 0 && V >= 0 && J >= 0);
+  EPB_CHECK_ARG(V >= 2 && V <= 8 && (S == 1 || S == V));
+  EPB_CHECK_ARG(root >= 0 && root < J);
+  EPB_CHECK_ARG((int64_t)T * V * J <= 0x7fffffff);
+  return EPB_OK;
+}
+
 // --------------------------------------------------------------- relative pose (no extrinsics)
 // Self-supervision without camera extrinsics: the geometry of a view pair comes from its own
 // predicted 2-D joints.  The reference leaves only the pieces (lib/utils/cameras.py:133-143,
@@ -1570,6 +1595,21 @@ extern "C" __attribute__((visibility("default"))) int epb_pose_to_camera(
   EPB_CHECK_ARG(N >= 0 && J > 0 && root >= 0 && root < J);
   if (N == 0) return EPB_OK;
   pose_to_camera_kernel<<<(N + 63) / 64, 64, 0, as_stream(stream)>>>(joints, cam, N, J, root, out);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_pseudo_records(
+    const double* X, const int32_t* status, const double* cam, int T, int S, int V, int J, int root, double* joints_3d,
+    double* vis, double* pelvis, int32_t* ok, epb_stream_t stream) {
+  EPB_CHECK_ARG(X && status && cam && joints_3d && vis && pelvis && ok);
+  const int rc = pseudo_records_sizes(T, S, V, J, root);
+  if (rc != EPB_OK) return rc;
+  if (T == 0) return EPB_OK;
+  const int threads = 128;
+  const int64_t n = (int64_t)T * V;
+  pseudo_records_kernel<<<(unsigned)((n + threads - 1) / threads), threads, 0, as_stream(stream)>>>(
+      X, status, cam, T, S, V, J, root, joints_3d, vis, pelvis, ok);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

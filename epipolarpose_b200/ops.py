@@ -492,6 +492,12 @@ def pose_to_camera(joints, cam, N, J, root, out):
           _p(out, torch.float64), _stream())
 
 
+def pseudo_records(X, status, cam, T, S, V, J, root, joints_3d, vis, pelvis, ok):
+    _call("epb_pseudo_records", _p(X, torch.float64), _p(status, torch.int32), _p(cam, torch.float64), T, S, V,
+          J, root, _p(joints_3d, torch.float64), _p(vis, torch.float64), _p(pelvis, torch.float64),
+          _p(ok, torch.int32), _stream())
+
+
 def refiner_sizes(in_size, linear_size, out_size, N):
     """(parameter floats, workspace floats) of the refiner kernels (host only)."""
     npar, nws = ctypes.c_int64(), ctypes.c_int64()

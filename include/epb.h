@@ -518,6 +518,25 @@ int epb_pose_errors(const double* pred, const double* gt, int S, int J, uint32_t
  *   out [N][J][3] mm. */
 int epb_pose_to_camera(const double* joints, const double* cam, int N, int J, int root, double* out,
                        epb_stream_t stream);
+/* Annotation records of triangulated world joints: from_worldjt_to_imagejt (lib/utils/prep_h36m.py:
+ * 176-204 of the reference, without the 3-D rectangle) per (frame, camera, joint).  float64,
+ * --fmad=false.
+ *   X      [T][S][J][3]  world joints; S = 1: one pose per frame, used for every camera; S = V: one
+ *                        pose per camera
+ *   status [T][S][J]     int32, 1 = triangulated (as the triangulators write it)
+ *   cam    [T][V][16]    R(9) T(3) f(2) c(2), the epb_project_labels layout; X_cam = R (X - T)
+ *   root                 root joint
+ * Outputs:
+ *   joints_3d [T][V][J][3]  CamProj x, y (px), camera-frame depth minus the root's (mm)
+ *   vis       [T][V][J][3]  1 where ok, the joint's status is 1, its depth is > 0 and its row is
+ *                           finite, else 0 (and the joints_3d row is 0)
+ *   pelvis    [T][V][3]     camera-frame root (mm); 0 where ok is 0
+ *   ok        [T][V]        int32, 1 = the root has status 1 and lies, finite, in front of the camera
+ * Nothing non-finite is ever written.  EPB_EINVAL: a negative size, V outside 2..8, S not 1 or V,
+ * root outside [0, J), T*V*J > 2^31-1.  T = 0 launches nothing. */
+int epb_pseudo_records(const double* X, const int32_t* status, const double* cam, int T, int S, int V, int J,
+                       int root, double* joints_3d, double* vis, double* pelvis, int32_t* ok,
+                       epb_stream_t stream);
 
 /* Eval-mode refiner MLP: LinearModelPG.forward (refiner/model.py:117-143 of the reference,
  * num_stage 2, bias, BatchNorm, ReLU; dropout the identity), second head.  Widths: in (input),
