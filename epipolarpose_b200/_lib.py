@@ -117,7 +117,8 @@ _PROTOS = {
     "epb_jpeg_transcode": (c_int, [c_p, c_p, c_p, c_p, c_int, c_p, c_p, c_p, c_i64, c_p, c_p, c_p, c_p, c_p, c_p, c_i64,
                                    c_p]),
     "epb_triangulate_robust": (c_int, [c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p, c_p, c_p]),
-    "epb_pseudo_records": (c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_p]),
+    "epb_tuple_labels": (c_int, [c_p] * 5 + [c_int] * 3 + [c_d] * 4 + [c_p] * 7),
+    "epb_pseudo_records":(c_int, [c_p, c_p, c_p, c_int, c_int, c_int, c_int, c_int, c_p, c_p, c_p, c_p, c_p]),
 }
 
 EXPORTS = tuple(_PROTOS)

@@ -586,7 +586,7 @@ __global__ void triangulate_nview_kernel(const double* __restrict__ u, int strid
 
 // img_utils.py:72-105 with its float32 roundings.  Returns the 2x3 transform
 // mapping src->dst (inv=0: image->patch) or dst->src (inv=1: patch->image).
-__device__ void patch_affine(const double* box, double patch_w, double patch_h, int inv,
+__host__ __device__ void patch_affine(const double* box, double patch_w, double patch_h, int inv,
                              double (&M)[2][3]) {
   const double c_x = box[0], c_y = box[1], scale = box[4], rot = box[5];
   const double src_w = box[2] * scale, src_h = box[3] * scale;
@@ -621,6 +621,23 @@ __device__ void patch_affine(const double* box, double patch_w, double patch_h, 
   }
 }
 
+// One soft-argmax coordinate c [3] (normalised) of a sample with box [6] -> image point k [4] =
+// (x px, y px, z mm, 1).  Shared by patch_to_image_kernel and the tuple-label entry.
+__host__ __device__ inline void patch_to_image_point(const float* c, const double* box, double patch_w,
+                                                     double patch_h, double rect3d_w, double* k) {
+  // integral_loss.py:196-201
+  const double px = ((double)c[0] + 0.5) * patch_w;
+  const double py = ((double)c[1] + 0.5) * patch_h;
+  const double pz = (double)c[2] * patch_w;
+  double M[2][3];
+  patch_affine(box, patch_w, patch_h, 1, M);
+  // img_utils.py:108-111 np.dot(trans, [x, y, 1])
+  k[0] = (M[0][0] * px + M[0][1] * py) + M[0][2];
+  k[1] = (M[1][0] * px + M[1][1] * py) + M[1][2];
+  k[2] = pz / patch_w * rect3d_w;  // img_utils.py:154
+  k[3] = 1.0;
+}
+
 __global__ void patch_to_image_kernel(const float* __restrict__ coords,
                                       const double* __restrict__ box, int B, int J,
                                       double patch_w, double patch_h, double rect3d_w,
@@ -628,29 +645,16 @@ __global__ void patch_to_image_kernel(const float* __restrict__ coords,
   const int idx = blockIdx.x * blockDim.x + threadIdx.x;
   if (idx >= B * J) return;
   const int b = idx / J;
-  // integral_loss.py:196-201
-  const double px = ((double)coords[idx * 3 + 0] + 0.5) * patch_w;
-  const double py = ((double)coords[idx * 3 + 1] + 0.5) * patch_h;
-  const double pz = (double)coords[idx * 3 + 2] * patch_w;
-  double M[2][3];
-  patch_affine(box + b * 6, patch_w, patch_h, 1, M);
-  // img_utils.py:108-111 np.dot(trans, [x, y, 1])
-  kps[(int64_t)idx * 4 + 0] = (M[0][0] * px + M[0][1] * py) + M[0][2];
-  kps[(int64_t)idx * 4 + 1] = (M[1][0] * px + M[1][1] * py) + M[1][2];
-  kps[(int64_t)idx * 4 + 2] = pz / patch_w * rect3d_w;  // img_utils.py:154
-  kps[(int64_t)idx * 4 + 3] = 1.0;
+  patch_to_image_point(coords + idx * 3, box + b * 6, patch_w, patch_h, rect3d_w, kps + (int64_t)idx * 4);
 }
 
-__global__ void project_labels_kernel(const double* __restrict__ X, const double* __restrict__ cam,
-                                      const double* __restrict__ box, int B, int J,
-                                      double patch_w, double patch_h, double rect3d_w,
-                                      float* __restrict__ label, float* __restrict__ weight) {
-  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
-  if (idx >= B * J) return;
-  const int b = idx / J;
-  const double* c = cam + b * 16;   // R(9) T(3) f(2) c(2)
-  const double* x = X + (int64_t)idx * 3;
-  const double* x0 = X + (int64_t)b * J * 3;  // root joint 0 (prep_h36m.py:181)
+// The label of one joint x [3] (world) in one view: root x0 [3] (joint 0, prep_h36m.py:181), c [16]
+// = R(9) T(3) f(2) c(2), box [6].  Writes the label [3] and returns the camera-frame depths of the
+// joint (cz) and of the root (pelvis_z).  Shared by project_labels_kernel and the tuple-label entry.
+__host__ __device__ inline void project_label_point(const double* x, const double* x0, const double* c,
+                                                    const double* box, double patch_w, double patch_h,
+                                                    double rect3d_w, float* label, double& cz_out,
+                                                    double& pelvis_z_out) {
   // prep_h36m.py:186 np.dot(rot, keypoints - trans)
   const double dx = x[0] - c[9], dy = x[1] - c[10], dz = x[2] - c[11];
   const double cx = (c[0] * dx + c[1] * dy) + c[2] * dz;
@@ -663,14 +667,28 @@ __global__ void project_labels_kernel(const double* __restrict__ X, const double
   double v = cy / cz * c[13] + c[15];
   double z = cz - pelvis_z;  // :199
   double M[2][3];
-  patch_affine(box + b * 6, patch_w, patch_h, 0, M);
+  patch_affine(box, patch_w, patch_h, 0, M);
   const double pu = (M[0][0] * u + M[0][1] * v) + M[0][2];   // img_utils.py:235
   const double pv = (M[1][0] * u + M[1][1] * v) + M[1][2];
-  z = z / (rect3d_w * box[b * 6 + 4]) * patch_w;               // :236
+  z = z / (rect3d_w * box[4]) * patch_w;                       // :236
   // integral_loss.py:171-173
-  label[idx * 3 + 0] = (float)(pu / patch_w - 0.5);
-  label[idx * 3 + 1] = (float)(pv / patch_h - 0.5);
-  label[idx * 3 + 2] = (float)(z / patch_w);
+  label[0] = (float)(pu / patch_w - 0.5);
+  label[1] = (float)(pv / patch_h - 0.5);
+  label[2] = (float)(z / patch_w);
+  cz_out = cz;
+  pelvis_z_out = pelvis_z;
+}
+
+__global__ void project_labels_kernel(const double* __restrict__ X, const double* __restrict__ cam,
+                                      const double* __restrict__ box, int B, int J,
+                                      double patch_w, double patch_h, double rect3d_w,
+                                      float* __restrict__ label, float* __restrict__ weight) {
+  const int idx = blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= B * J) return;
+  const int b = idx / J;
+  double cz, pz;
+  project_label_point(X + (int64_t)idx * 3, X + (int64_t)b * J * 3, cam + b * 16, box + b * 6, patch_w,
+                      patch_h, rect3d_w, label + idx * 3, cz, pz);
   weight[idx * 3 + 0] = 1.f;
   weight[idx * 3 + 1] = 1.f;
   weight[idx * 3 + 2] = 1.f;
@@ -1445,6 +1463,84 @@ triangulate_robust_kernel(const double* __restrict__ u, int stride_u, const doub
                status + idx);
 }
 
+// --------------------------------------------------------------- tuple labels (online training)
+// A view-major training batch: T tuples of V views, row v*T + t is view v of tuple t.
+// 1. tuple_point: one (tuple t, joint j).  The lanes stage the V views in u [V*2], P [V*12], w [V]
+//    (lane l: views l, l + n, ..; entries l, l + n, .. of P): the image point of row v*T + t with the
+//    arithmetic of patch_to_image_kernel, its projection matrix, and its weight lse_ws[1] (the peak
+//    softmax probability of the joint) or 1.  Then robust_point, as in triangulate_robust_kernel.
+template <class Red>
+__host__ __device__ void tuple_point(const Red& red, const float* coords, const float* lse_ws, const double* box,
+                                     const double* P, int64_t T, int V, int J, int64_t t, int j, double patch_w,
+                                     double patch_h, double rect3d_w, double thr, double* u, double* Pv,
+                                     double* w, double* X, int32_t* inl, double* resid, int32_t* status) {
+  for (int k = red.lane; k < V * 12; k += red.n) {
+    const int v = k / 12;
+    Pv[k] = P[(v * T + t) * 12 + (k - v * 12)];
+  }
+  for (int v = red.lane; v < V; v += red.n) {
+    const int64_t o = (v * T + t) * J + j;
+    double kp[4];
+    patch_to_image_point(coords + o * 3, box + (v * T + t) * 6, patch_w, patch_h, rect3d_w, kp);
+    u[2 * v + 0] = kp[0];
+    u[2 * v + 1] = kp[1];
+    w[v] = lse_ws ? (double)lse_ws[o * 2 + 1] : 1.0;
+  }
+#ifdef __CUDA_ARCH__
+  __syncwarp();
+#endif
+  robust_point(red, u, Pv, w, V, thr, X, inl, resid, status);
+}
+
+// 2. tuple_label: one (row, joint).  X, status [T][J].  Label and weight 1 when the joint and the root
+//    (joint 0) of the tuple were triangulated and both lie at a positive, finite depth in this view
+//    (and the label is finite); label 0 and weight 0 otherwise.
+__host__ __device__ inline void tuple_label(const double* X, const int32_t* status, const double* cam,
+                                            const double* box, int64_t T, int J, int64_t row, int j, double patch_w,
+                                            double patch_h, double rect3d_w, float* label, float* weight) {
+  const int64_t t = row % T;
+  const double* xt = X + t * J * 3;
+  float lab[3];
+  double cz, pz;
+  project_label_point(xt + (int64_t)j * 3, xt, cam + row * 16, box + row * 6, patch_w, patch_h, rect3d_w, lab,
+                      cz, pz);
+  const bool ok = status[t * J + j] == 1 && status[t * J] == 1 && cz > 0.0 && cz < INFINITY && pz > 0.0 &&
+                  pz < INFINITY && isfinite(lab[0]) && isfinite(lab[1]) && isfinite(lab[2]);
+  for (int k = 0; k < 3; ++k) {
+    label[k] = ok ? lab[k] : 0.f;
+    weight[k] = ok ? 1.f : 0.f;
+  }
+}
+
+__global__ void __launch_bounds__(kRobustWarps * 32)
+tuple_triangulate_kernel(const float* __restrict__ coords, const float* __restrict__ lse_ws,
+                         const double* __restrict__ box, const double* __restrict__ P, int T, int V, int J,
+                         double patch_w, double patch_h, double rect3d_w, double thr, double* __restrict__ X,
+                         int32_t* __restrict__ inl, double* __restrict__ resid, int32_t* __restrict__ status) {
+  __shared__ double sP[kRobustWarps][RB_MAXV * 12], sU[kRobustWarps][RB_MAXV * 2],
+      sW[kRobustWarps][RB_MAXV];
+  const int wid = threadIdx.x >> 5;
+  const int64_t idx = (int64_t)blockIdx.x * kRobustWarps + wid;
+  if (idx >= (int64_t)T * J) return;                       // warp-uniform
+  RbWarp red;
+  red.lane = threadIdx.x & 31;
+  const int64_t t = idx / J;
+  const int j = (int)(idx - t * J);
+  tuple_point(red, coords, lse_ws, box, P, T, V, J, t, j, patch_w, patch_h, rect3d_w, thr, sU[wid], sP[wid],
+              sW[wid], X + idx * 3, inl + idx, resid + idx, status + idx);
+}
+
+__global__ void tuple_label_kernel(const double* __restrict__ X, const int32_t* __restrict__ status,
+                                   const double* __restrict__ cam, const double* __restrict__ box, int T, int V,
+                                   int J, double patch_w, double patch_h, double rect3d_w,
+                                   float* __restrict__ label, float* __restrict__ weight) {
+  const int64_t idx = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+  if (idx >= (int64_t)V * T * J) return;
+  const int64_t row = idx / J;
+  tuple_label(X, status, cam, box, T, J, row, (int)(idx - row * J), patch_w, patch_h, rect3d_w, label + idx * 3,
+              weight + idx * 3);
+}
+
 // --------------------------------------------------------------- argmax
 // inference.py:24-39: one warp per (n,j) map; (value, index) reduction with
 // smallest-index tie-break == numpy argmax first-occurrence.  NaN: numpy
@@ -1639,6 +1735,27 @@ extern "C" __attribute__((visibility("default"))) int epb_triangulate_robust(
   triangulate_robust_kernel<<<(unsigned)((n + kRobustWarps - 1) / kRobustWarps), kRobustWarps * 32, 0,
                               as_stream(stream)>>>(u, stride_u, P, w, NT, V, J, threshold_px, X,
                                                    inliers, resid, status);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_tuple_labels(
+    const float* coords, const float* lse_ws, const double* box, const double* P, const double* cam, int T,
+    int V, int J, double patch_w, double patch_h, double rect3d_w, double threshold_px, float* label,
+    float* weight, double* X, int32_t* inliers, double* resid, int32_t* status, epb_stream_t stream) {
+  EPB_CHECK_ARG(coords && box && P && cam && label && weight && X && inliers && resid && status);
+  EPB_CHECK_ARG(T >= 0 && J >= 0 && V >= 2 && V <= RB_MAXV);
+  EPB_CHECK_ARG(isfinite(threshold_px) && threshold_px > 0.0);
+  EPB_CHECK_ARG((int64_t)V * T * J <= 0x7fffffff);
+  if ((int64_t)T * J == 0) return EPB_OK;
+  cudaStream_t st = as_stream(stream);
+  const int64_t n = (int64_t)T * J;
+  tuple_triangulate_kernel<<<(unsigned)((n + kRobustWarps - 1) / kRobustWarps), kRobustWarps * 32, 0, st>>>(
+      coords, lse_ws, box, P, T, V, J, patch_w, patch_h, rect3d_w, threshold_px, X, inliers, resid, status);
+  EPB_LAUNCH_CHECK();
+  const int64_t m = (int64_t)V * T * J;
+  tuple_label_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(X, status, cam, box, T, V, J, patch_w, patch_h,
+                                                                  rect3d_w, label, weight);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

@@ -9,7 +9,10 @@ ValueError exactly like reference :167,184.
 Extra keys (superset, all default-off): TRAIN.ONLINE_TRIANGULATION,
 TRAIN.TRIANGULATION_METHOD, TRAIN.ESTIMATE_EXTRINSICS (self-supervision without camera
 extrinsics: each view pair's pose is estimated from its 2-D joints; needs
-TRAIN.ONLINE_TRIANGULATION, ValueError otherwise), TRAIN.CUDA_GRAPH (default on),
+TRAIN.ONLINE_TRIANGULATION, ValueError otherwise), DATASET.TRI_VIEWS (views per DATASET.TRI training
+item, default 2: the reference's pairs), TRAIN.TRIANGULATION_METHOD: robust (online labels from the
+robust triangulation of every view of a tuple) with TRAIN.ROBUST_THRESHOLD_PX (default 15.0; see
+tuple_settings for the combinations refused), TRAIN.CUDA_GRAPH (default on),
 MODEL.PRECISION, DATASET.SYNTHETIC_LEN, TEST.PSS_K (list of k: the H36M evaluation appends
 PSS@k, lib/core/pss.py; default []), TEST.PSS_CENTROIDS (.npz of `k<k>` centroids used instead
 of fitting them on train-fs; default ''), TEST.REFINER (a refiner checkpoint: the H36M evaluation
@@ -62,12 +65,12 @@ _DEFAULTS = dict(
                  HYBRID_JOINTS_TYPE='', SELECT_DATA=False, TRI=False, MPII_ORDER=False,
                  TRAIN_FRAME=32, VAL_FRAME=64, NUM_CAMS=4, DEPTH_RANGE=2000, FLIP=True,
                  SCALE_FACTOR=0.25, ROT_FACTOR=30, OCCLUSION=False, VOC='', BG_AUG=False,
-                 Z_WEIGHT=1., SYNTHETIC_LEN=256),
+                 Z_WEIGHT=1., SYNTHETIC_LEN=256, TRI_VIEWS=2),
     TRAIN=dict(LR_FACTOR=0.1, LR_STEP=[90, 110], LR=0.001, OPTIMIZER='adam', MOMENTUM=0.9,
                WD=0.0001, NESTEROV=False, GAMMA1=0.99, GAMMA2=0.0, BEGIN_EPOCH=0, END_EPOCH=140,
                RESUME=False, CHECKPOINT='', BATCH_SIZE=32, SHUFFLE=True,
                ONLINE_TRIANGULATION=False, TRIANGULATION_METHOD='iterative', ESTIMATE_EXTRINSICS=False,
-               CUDA_GRAPH=True),
+               ROBUST_THRESHOLD_PX=15.0, CUDA_GRAPH=True),
     TEST=dict(BATCH_SIZE=32, FLIP_TEST=False, POST_PROCESS=True, SHIFT_HEATMAP=True,
               USE_GT_BBOX=False, OKS_THRE=0.5, IN_VIS_THRE=0.0, COCO_BBOX_FILE='', BBOX_THRE=1.0,
               MODEL_FILE='', IMAGE_THRE=0.0, NMS_THRE=1.0, PSS_K=[], PSS_CENTROIDS='',
@@ -127,6 +130,33 @@ def check_config(cfg):
     if train.get('ESTIMATE_EXTRINSICS', False) and not train.get('ONLINE_TRIANGULATION', False):
         raise ValueError("TRAIN.ESTIMATE_EXTRINSICS needs TRAIN.ONLINE_TRIANGULATION: the estimated "
                          "camera geometry only feeds the online epipolar labels")
+    tuple_settings(cfg)
+
+
+def tuple_settings(cfg):
+    """(views, method, threshold_px) of online self-supervised training: DATASET.TRI_VIEWS, and
+    TRAIN.TRIANGULATION_METHOD / TRAIN.ROBUST_THRESHOLD_PX when TRAIN.ONLINE_TRIANGULATION is set
+    (method None otherwise).  ValueError for TRI_VIEWS outside 2..min(NUM_CAMS, 8), more than two
+    views with online labels from any method but 'robust' (the pair triangulators take two views),
+    'robust' with TRAIN.ESTIMATE_EXTRINSICS (the relative pose is estimated per view pair), and a
+    threshold that is not a positive number of pixels.  Missing keys take their defaults."""
+    ds, train = getattr(cfg, 'DATASET', None), getattr(cfg, 'TRAIN', None)
+    views = int(getattr(ds, 'TRI_VIEWS', 2))
+    cams = int(getattr(ds, 'NUM_CAMS', 4))
+    if not (views == 2 or 2 < views <= min(cams, 8)):       # 2: the reference's pairs, any NUM_CAMS
+        raise ValueError("DATASET.TRI_VIEWS must be in 2..min(NUM_CAMS, 8) = 2..%d, got %d" % (min(cams, 8), views))
+    online = bool(getattr(train, 'ONLINE_TRIANGULATION', False))
+    method = getattr(train, 'TRIANGULATION_METHOD', 'iterative') if online else None
+    thr = float(getattr(train, 'ROBUST_THRESHOLD_PX', 15.0))
+    if online and views > 2 and method != 'robust':
+        raise ValueError("DATASET.TRI_VIEWS = %d with TRAIN.ONLINE_TRIANGULATION needs TRAIN.TRIANGULATION_METHOD: "
+                         "robust; the pair triangulators (%r) take two views" % (views, method))
+    if method == 'robust' and bool(getattr(train, 'ESTIMATE_EXTRINSICS', False)):
+        raise ValueError("TRAIN.TRIANGULATION_METHOD: robust needs calibrated cameras; TRAIN.ESTIMATE_EXTRINSICS "
+                         "estimates the relative pose of view pairs only")
+    if method == 'robust' and not (np.isfinite(thr) and thr > 0):
+        raise ValueError("TRAIN.ROBUST_THRESHOLD_PX must be a positive number of pixels, got %r" % (thr,))
+    return views, method, thr
 
 
 def gen_config(config_file):

@@ -13,7 +13,9 @@ Differences from the reference body (same observable behaviour):
     re-projection) entirely on the device -- the glue the released reference
     leaves unwired (SURVEY.md section 3.3); with config.TRAIN.ESTIMATE_EXTRINSICS the
     cameras of each view pair are estimated from the predicted 2-D joints (no R, T or
-    projection matrix needed: the reference's "without R/t" mode);
+    projection matrix needed: the reference's "without R/t" mode); with
+    TRAIN.TRIANGULATION_METHOD robust the batch holds whole tuples of DATASET.TRI_VIEWS views and
+    every view's labels come from one robust triangulation of all of them (epb_tuple_labels);
   * the gradient all-reduce for multi-GPU data parallelism happens inside the
     model's backward (one NCCL call on the flat gradient buffer);
   * loader batches of deferred samples (lib/dataset/deferred.py: the h36m / mpii_integral
@@ -35,8 +37,9 @@ from ..utils.img_utils import (self_supervision_device,
                                trans_coords_from_patch_to_org_3d_batch)
 from .integral_loss import get_joint_location_coords_flip, get_result_func, joint_location_result_from_coords
 from ..utils.utils import AverageMeter
-from ..dataset.deferred import assemble_batch, cat_meta, is_deferred
+from ..dataset.deferred import assemble_batch, cat_meta, is_deferred, view_keys
 from .refine import export_refiner_pairs  # noqa: F401  (public here, next to eval_integral)
+from .config import tuple_settings
 
 logger = logging.getLogger(__name__)
 
@@ -45,13 +48,15 @@ def loader_batch(data):
     """(batch_data, label, weight, meta) of a loader batch.  A batch of deferred samples (a
     dataset indexed in DataLoader workers) is assembled on the device; a TRI batch
     {'cam_1', 'cam_2'} becomes one batch [cam_1 ; cam_2], the first-half / second-half pairing
-    of online triangulation (reference img_utils.py:194-199)."""
+    of online triangulation (reference img_utils.py:194-199); a batch {'cam_1', .., 'cam_V'} of
+    whole tuples becomes [cam_1 ; .. ; cam_V], row v*B + t view v of tuple t."""
     if is_deferred(data):
         return assemble_batch(data)
-    if isinstance(data, dict) and 'cam_1' in data and 'cam_2' in data:
-        a, b = data['cam_1'], data['cam_2']
-        return (torch.cat([a[0], b[0]]), torch.cat([a[1], b[1]]), torch.cat([a[2], b[2]]),
-                cat_meta(a[3], b[3]))
+    keys = view_keys(data)
+    if keys:
+        parts = [data[k] for k in keys]
+        return (torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts]), torch.cat([p[2] for p in parts]),
+                cat_meta(*[p[3] for p in parts]))
     return data
 
 
@@ -88,19 +93,33 @@ def _estimate_extrinsics(config):
     return est
 
 
-def online_epipolar_loss(criterion, preds, meta, method="iterative", estimate_extrinsics=False):
+def online_epipolar_loss(criterion, preds, meta, method="iterative", estimate_extrinsics=False, views=2,
+                         threshold_px=15.0):
     """criterion(preds, labels(preds), 1) with the labels produced by the epipolar
     self-supervision path from the SAME soft-argmax coordinates the loss uses
     (labels carry no gradient, reference integral_loss.py:88-91).  estimate_extrinsics:
     the cameras of each view pair are estimated from its own 2-D joints, and pairs whose
-    estimate failed carry weight 0."""
-    from .integral_loss import softmax_integral_tensor, _WeightedLossFn
+    estimate failed carry weight 0.  method 'robust': the batch is whole tuples of `views` views,
+    view-major (row v*T + t is view v of tuple t), and the labels and weights come from the robust
+    triangulation of every view of each tuple (img_utils.tuple_labels_device), each view weighted by
+    the peak probability the same soft-argmax pass left in its workspace."""
+    from .integral_loss import softmax_integral_tensor, softmax_integral_tensor_lse, _WeightedLossFn
     from ..utils.img_utils import (patch_to_image_device, triangulate_device,
                                    labels_from_global_coords_device,
-                                   labels_estimated_extrinsics_device)
+                                   labels_estimated_extrinsics_device, tuple_labels_device)
     J = criterion.num_joints
     W, H = preds.shape[-1], preds.shape[-2]
     D = preds.shape[-3] // J
+    if method == "robust":
+        if estimate_extrinsics:
+            raise ValueError("the robust online labels need calibrated cameras (no estimate_extrinsics)")
+        if preds.shape[0] % views:
+            raise ValueError("a batch of %d rows is not whole tuples of %d views" % (preds.shape[0], views))
+        coords, lse = softmax_integral_tensor_lse(preds, J, W, H, D)
+        with torch.no_grad():
+            label, weight = tuple_labels_device(coords.detach(), lse, meta, views, threshold_px)
+        return _WeightedLossFn.apply(coords, label, weight, criterion._kind, criterion.size_average,
+                                     criterion.norm)
     coords = softmax_integral_tensor(preds, J, True, W, H, D)
     with torch.no_grad():
         kps = patch_to_image_device(coords.detach(), meta)
@@ -122,7 +141,7 @@ class GraphedTrainStep:
     eagerly (sizes workspaces, one-time attributes), the second captures and replays."""
 
     def __init__(self, model, criterion, optimizer, online=False, method="iterative",
-                 estimate_extrinsics=False):
+                 estimate_extrinsics=False, views=2, threshold_px=15.0):
         # scripts/train.py:94 wraps the model in nn.DataParallel(device_ids=[k]); with one
         # device id that wrapper only forwards the call (and its scatter is not capturable)
         if isinstance(model, torch.nn.DataParallel) and len(model.device_ids) == 1:
@@ -132,6 +151,11 @@ class GraphedTrainStep:
         if estimate_extrinsics and not online:
             raise ValueError("estimate_extrinsics needs online=True")
         self.estimate_extrinsics = bool(estimate_extrinsics)
+        if online and method == "robust" and self.estimate_extrinsics:
+            raise ValueError("the robust online labels need calibrated cameras (no estimate_extrinsics)")
+        if online and method != "robust" and views != 2:
+            raise ValueError("%d views per tuple need method='robust'; the pair triangulators take two" % views)
+        self.views, self.threshold_px = int(views), float(threshold_px)
         self.graph = None
         self.key = None
         self.warm_key = None          # shape of the last eager (warm-up) step
@@ -161,7 +185,7 @@ class GraphedTrainStep:
             preds = self.model(x)
         if self.online:
             loss = online_epipolar_loss(self.criterion, preds, {"_packed": geom}, self.method,
-                                        self.estimate_extrinsics)
+                                        self.estimate_extrinsics, self.views, self.threshold_px)
         else:
             loss = self.criterion(preds, label, weight)
         loss.backward()
@@ -237,7 +261,8 @@ class GraphedTrainStep:
         if self.online:
             from ..utils.img_utils import pack_meta
             geom = pack_meta(meta, B, dev, self.estimate_extrinsics)
-        key = (tuple(batch_data.shape), self.online, self.estimate_extrinsics)
+        key = (tuple(batch_data.shape), self.online, self.method, self.views, self.threshold_px,
+               self.estimate_extrinsics)
         self.calls += 1
         if self.graph is not None and key == self.key:
             self._load_input(batch_data)
@@ -304,16 +329,17 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
     losses = AverageMeter()
     model.train()
     online = _online_tri(config)
-    method = getattr(config.TRAIN, 'TRIANGULATION_METHOD', 'iterative') if online else None
     estimate = _estimate_extrinsics(config)
+    views, method, thr = tuple_settings(config)
     pending = []           # (device loss, batch size) not yet folded into `losses`
     use_graph = bool(getattr(config.TRAIN, 'CUDA_GRAPH', True)) and \
         _graph_capable(model, criterion, optimizer)
     stepper = getattr(model, '_epb_graphed_step', None)
     if use_graph and (stepper is None or stepper.optimizer is not optimizer
                       or stepper.criterion is not criterion or stepper.online != online
-                      or stepper.estimate_extrinsics != estimate):
-        stepper = GraphedTrainStep(model, criterion, optimizer, online, method, estimate)
+                      or stepper.estimate_extrinsics != estimate or stepper.method != method
+                      or stepper.views != views or stepper.threshold_px != thr):
+        stepper = GraphedTrainStep(model, criterion, optimizer, online, method, estimate, views, thr)
         model._epb_graphed_step = stepper
     end = time.time()
     it = iter(train_loader)
@@ -346,7 +372,7 @@ def train_integral(config, train_loader, model, criterion, optimizer, epoch):
                 preds = model(batch_data)
             if online:
                 # one soft-argmax pass serves both the epipolar labels and the loss
-                loss = online_epipolar_loss(criterion, preds, meta, method, estimate)
+                loss = online_epipolar_loss(criterion, preds, meta, method, estimate, views, thr)
                 batch_label = batch_label_weight = None
             else:
                 batch_label = batch_label.cuda(non_blocking=True)

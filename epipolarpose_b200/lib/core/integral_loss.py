@@ -57,6 +57,9 @@ def _storage(preds, layout):
 
 
 class _SoftArgmaxFn(torch.autograd.Function):
+    """(coords [N, J*3], lse [N*J*2]): the soft-argmax and its softmax workspace (max, 1 / sum exp(l -
+    max) per joint), which carries no gradient; callers that only want the coordinates take [0]."""
+
     @staticmethod
     def forward(ctx, preds, J, D, H, W):
         ops = _backend[0]
@@ -69,10 +72,12 @@ class _SoftArgmaxFn(torch.autograd.Function):
         ctx.save_for_backward(preds, coords, lse)
         ctx.cfg = (layout, N, J, D, H, W)
         ctx.sink = sink if (sink is not None and layout == 1 and sink.matches(preds)) else None
-        return coords
+        ctx.mark_non_differentiable(lse)
+        ctx.set_materialize_grads(False)          # no zero gradient is made for lse
+        return coords, lse
 
     @staticmethod
-    def backward(ctx, dcoords):
+    def backward(ctx, dcoords, dlse):
         ops = _backend[0]
         preds, coords, lse = ctx.saved_tensors
         layout, N, J, D, H, W = ctx.cfg
@@ -101,7 +106,19 @@ def softmax_integral_tensor(preds, num_joints, output_3d, hm_width, hm_height, h
         raise TypeError("softmax_integral_tensor expects float32 logits")
     assert preds.shape[1] == num_joints * hm_depth and preds.shape[2] == hm_height \
         and preds.shape[3] == hm_width
-    return _SoftArgmaxFn.apply(preds, num_joints, hm_depth, hm_height, hm_width)
+    return _SoftArgmaxFn.apply(preds, num_joints, hm_depth, hm_height, hm_width)[0]
+
+
+def softmax_integral_tensor_lse(preds, num_joints, hm_width, hm_height, hm_depth):
+    """softmax_integral_tensor that also returns what the same pass leaves in its softmax workspace:
+    (coords [N, J*3], lse [N, J, 2] without gradient), lse[..., 1] the peak softmax probability of
+    each joint's volume."""
+    if preds.dtype != torch.float32:
+        raise TypeError("softmax_integral_tensor expects float32 logits")
+    assert preds.shape[1] == num_joints * hm_depth and preds.shape[2] == hm_height \
+        and preds.shape[3] == hm_width
+    coords, lse = _SoftArgmaxFn.apply(preds, num_joints, hm_depth, hm_height, hm_width)
+    return coords, lse.view(preds.shape[0], num_joints, 2)
 
 
 def _like(x, t, name):

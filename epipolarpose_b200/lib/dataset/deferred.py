@@ -92,10 +92,21 @@ def make_deferred(blob, box, joints, joints_vis, flip_pairs, do_augment, occlude
             'meta': meta}
 
 
+def view_keys(batch):
+    """['cam_1', .., 'cam_V'] of a TRI batch (a dict with at least 'cam_1' and 'cam_2'), else []."""
+    if not (isinstance(batch, dict) and 'cam_1' in batch and 'cam_2' in batch):
+        return []
+    keys = []
+    while 'cam_%d' % (len(keys) + 1) in batch:
+        keys.append('cam_%d' % (len(keys) + 1))
+    return keys
+
+
 def is_deferred(batch):
-    """A collated batch of deferred samples, or of TRI pairs {'cam_1', 'cam_2'} of them."""
-    if isinstance(batch, dict) and 'cam_1' in batch and 'cam_2' in batch:
-        return is_deferred(batch['cam_1'])
+    """A collated batch of deferred samples, or of TRI tuples {'cam_1', .., 'cam_V'} of them."""
+    keys = view_keys(batch)
+    if keys:
+        return is_deferred(batch[keys[0]])
     return isinstance(batch, dict) and KEY in batch
 
 
@@ -103,29 +114,32 @@ def _np(v):
     return v.numpy() if isinstance(v, torch.Tensor) else np.asarray(v)
 
 
-def cat_meta(a, b):
-    """Collated meta of two batches -> the meta of [a ; b]."""
+def cat_meta(*metas):
+    """Collated meta of batches a, b, .. -> the meta of [a ; b ; ..]."""
+    a = metas[0]
     out = {}
     for k in a:
-        x, y = a[k], b[k]
+        x = a[k]
         if isinstance(x, torch.Tensor):
-            out[k] = torch.cat([x, y.to(x.device)], dim=0)
+            out[k] = torch.cat([x] + [m[k].to(x.device) for m in metas[1:]], dim=0)
         elif isinstance(x, (list, tuple)):
-            out[k] = list(x) + list(y)
+            out[k] = [e for m in metas for e in m[k]]
         else:
-            out[k] = np.concatenate([_np(x), _np(y)], axis=0)
+            out[k] = np.concatenate([_np(m[k]) for m in metas], axis=0)
     return out
 
 
 def assemble_batch(batch):
     """Collated deferred batch -> device (images f32 [B,3,H,W], label f32 [B,J*3], weight f32
     [B,J*3], meta) -- each sample identical to get_single_patch_sample with that sample's draws,
-    meta carrying the drawn scale / rot.  A TRI batch {'cam_1', 'cam_2'} becomes one batch of 2B,
-    [cam_1 ; cam_2]: sample i pairs with sample i + B (reference img_utils.py:194-199)."""
-    if 'cam_1' in batch and 'cam_2' in batch:
-        x1, l1, w1, m1 = assemble_batch(batch['cam_1'])
-        x2, l2, w2, m2 = assemble_batch(batch['cam_2'])
-        return torch.cat([x1, x2]), torch.cat([l1, l2]), torch.cat([w1, w2]), cat_meta(m1, m2)
+    meta carrying the drawn scale / rot.  A TRI batch {'cam_1', .., 'cam_V'} becomes one batch of VB,
+    [cam_1 ; .. ; cam_V]: row v*B + t is view v of tuple t (for V = 2 the pairing of sample i with
+    sample i + B, reference img_utils.py:194-199)."""
+    keys = view_keys(batch)
+    if keys:
+        parts = [assemble_batch(batch[k]) for k in keys]
+        return (torch.cat([p[0] for p in parts]), torch.cat([p[1] for p in parts]), torch.cat([p[2] for p in parts]),
+                cat_meta(*[p[3] for p in parts]))
     if KEY not in batch:
         raise ValueError("not a batch of deferred samples")
     blobs = list(batch['jpeg'])

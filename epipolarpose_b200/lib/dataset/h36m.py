@@ -4,7 +4,10 @@ The db comes from `<root>/annot/<image_set>.pkl`: a list of records, or a dict o
 lists keyed 1..NUM_CAMS.  The construction-time draws are the reference's, in its order
 (np.random.permutation of the dict form, then random.shuffle), so a seeded run builds the same
 db.  With DATASET.TRI a training item draws a camera (np.random) and one of its neighbours in
-cam_config (random) and returns {'cam_1': view, 'cam_2': view} of the same frame index.
+cam_config (random) and returns {'cam_1': view, 'cam_2': view} of the same frame index; with
+DATASET.TRI_VIEWS = V > 2 it returns {'cam_1': view, .., 'cam_V': view} of the same frame index:
+every camera in camera order when V = NUM_CAMS (no draw), else the sorted
+np.random.choice(NUM_CAMS, V, replace=False).
 
 A view is the reference's (img_patch, label, label_weight, meta) in the main process and a
 deferred sample in a DataLoader worker (JointIntegralDataset.sample).  `evaluate` runs the H36M
@@ -34,10 +37,16 @@ class H36M_Integral(JointsIntegralDataset):
         super().__init__(cfg, root, image_set, is_train)
         self.parent_ids = np.array([0, 0, 1, 2, 0, 4, 5, 0, 8, 8, 9, 8, 11, 12, 8, 14, 15], dtype=np.int64)
         self.cam_config = [[1, 2], [0, 3], [0, 3], [1, 2]]          # camera neighbourhoods (:25)
+        self.tri_views = int(getattr(cfg.DATASET, 'TRI_VIEWS', 2))
         self.db = self._get_train_db() if is_train else self._get_val_db()
         logger.info('=> load {} samples'.format(self.db_length))
 
     def __getitem__(self, idx):
+        if self.is_train and self.cfg.DATASET.TRI and self.tri_views > 2:
+            V = self.tri_views
+            cams = range(self.num_cams) if V == self.num_cams else \
+                sorted(np.random.choice(self.num_cams, V, replace=False))
+            return {'cam_%d' % (k + 1): self.get_data(copy.deepcopy(self.db[int(c)][idx])) for k, c in enumerate(cams)}
         if self.is_train and self.cfg.DATASET.TRI:
             cam_1 = np.random.randint(self.num_cams)
             cam_2 = self.cam_config[cam_1][0] if random.random() <= 0.5 else self.cam_config[cam_1][1]
@@ -108,6 +117,9 @@ class H36M_Integral(JointsIntegralDataset):
                 random.shuffle(gt_db)
                 self.db_length = len(gt_db)
         else:
+            if self.cfg.DATASET.TRI and self.tri_views > 2:
+                raise ValueError("DATASET.TRI_VIEWS = %d needs a dict-form annotation pickle (one frame-aligned "
+                                 "list per camera); %s.pkl is a list of records" % (self.tri_views, self.image_set))
             gt_db = list(anno)
             random.shuffle(gt_db)
             self.db_length = len(gt_db)

@@ -12,7 +12,9 @@ P = K.[R | -R.T].
 Sample order: index = tuple*NUM_CAMS + view.  `pair_batch_sampler` lays a
 batch out as [views 0 and 3 of each tuple | views 1 and 2] so that the
 first-half/second-half pairing of reference img_utils.py:194-199 triangulates
-(0,1) and (3,2), both legal neighbours in reference h36m.py:25.
+(0,1) and (3,2), both legal neighbours in reference h36m.py:25.  `tuple_batch_sampler` lays
+out whole tuples view-major (row v*T + t is view v of tuple t), the layout of the robust online
+labels.
 
 `flip_pairs` (read by the flip test of validate_integral): the MPII pairs for 16 joints, the
 H36M-17 pairs for 17 (reference prep_h36m.py:71,68), none for any other joint count."""
@@ -95,6 +97,17 @@ class SyntheticH36M(Dataset):
             ts = range(b, b + tuples_per_batch)
             yield [t * 4 + 0 for t in ts] + [t * 4 + 3 for t in ts] + \
                   [t * 4 + 1 for t in ts] + [t * 4 + 2 for t in ts]
+
+    def tuple_batch_sampler(self, tuples_per_batch, views=None):
+        """Index batches of whole view tuples in the view-major layout of online triangulation
+        with TRAIN.TRIANGULATION_METHOD robust: row v*T + t is view v of tuple t (T =
+        tuples_per_batch, views 0..views-1 of each tuple, default all NUM_CAMS)."""
+        V = self.num_cams if views is None else int(views)
+        if not 2 <= V <= self.num_cams:
+            raise ValueError("views must be in 2..%d, got %d" % (self.num_cams, V))
+        n_tuples = len(self.db) // self.num_cams
+        for b in range(0, n_tuples - tuples_per_batch + 1, tuples_per_batch):
+            yield [t * self.num_cams + v for v in range(V) for t in range(b, b + tuples_per_batch)]
 
     def evaluate(self, preds, save_path=None, debug=False):
         """H36M protocol (reference lib/dataset/h36m.py:168-378) of the predictions against the

@@ -4,7 +4,8 @@ hot-path part of the reference lib/utils/img_utils.py:
   triangulate (:193-209), get_batch_labels_from_global_coords (:212-243).
 Everything downstream of the network output runs on the device in float64
 kernels (epb_patch_to_image -> epb_triangulate -> epb_project_labels); the
-reference's per-sample / per-joint Python loops disappear.  `meta` follows the
+reference's per-sample / per-joint Python loops disappear.  `tuple_labels_device` (not in the
+reference) labels whole camera tuples from one robust V-view triangulation (epb_tuple_labels).  `meta` follows the
 dataset contract of reference lib/dataset/h36m.py:73-86 (collated: tensors or
 lists of length B).  numpy in / numpy out like the reference;
 `self_supervision_device` returns CUDA tensors for the training loop.
@@ -136,6 +137,43 @@ def labels_estimated_extrinsics_device(kps, meta, method="iterative", patch_w=25
     ops.project_labels(X, cam, pm["box"], B, J, patch_w, patch_h, rect_3d_w, label, weight)
     ok = torch.cat([status, status], dim=0).reshape(B, 1) != 0
     return torch.where(ok, label, 0.0), weight * ok
+
+
+def tuple_labels_device(coords, lse, meta, views, threshold_px=_tri.DEFAULT_THRESHOLD_PX, patch_w=256.,
+                        patch_h=256., rect_3d_w=2000., full=False):
+    """Online labels of whole camera tuples (epb_tuple_labels, see include/epb.h): coords [B, J*3]
+    float32 soft-argmax output of a view-major batch (B = views * T, row v*T + t is view v of tuple
+    t), lse the soft-argmax's workspace ([B, J, 2] or [B*J*2]; its peak probability weights each view
+    in the robust refit) or None (weights 1) -> (label, weight) float32 [B, J*3]: the robust V-view
+    triangulation of each (tuple, joint) projected into every view of the tuple; weight 0 (and label
+    0) where the joint or the tuple's root failed or lies behind the camera.  full=True also returns
+    X [T,J,3], status [T,J], inliers [T,J] (bit v: view v) and resid [T,J] (px).  Static shapes, no
+    host synchronisation: capturable in a CUDA graph."""
+    ops = _backend[0]
+    B, J = coords.shape[0], coords.shape[1] // 3
+    V = int(views)
+    if not 2 <= V <= 8:
+        raise ValueError("tuple labels take 2..8 views per tuple, got %d" % V)
+    if B % V:
+        raise ValueError("a batch of %d rows is not whole tuples of %d views" % (B, V))
+    if not (np.isfinite(threshold_px) and threshold_px > 0):
+        raise ValueError("threshold_px must be a positive number of pixels, got %r" % (threshold_px,))
+    if lse is not None and lse.numel() != B * J * 2:
+        raise ValueError("lse must hold B*J*2 = %d values, got %d" % (B * J * 2, lse.numel()))
+    T, dev = B // V, coords.device
+    pm = pack_meta(meta, B, dev)
+    label = torch.empty((B, J * 3), device=dev, dtype=torch.float32)
+    weight = torch.empty((B, J * 3), device=dev, dtype=torch.float32)
+    X = torch.empty((T, J, 3), device=dev, dtype=torch.float64)
+    status = torch.empty((T, J), device=dev, dtype=torch.int32)
+    inliers = torch.empty((T, J), device=dev, dtype=torch.int32)
+    resid = torch.empty((T, J), device=dev, dtype=torch.float64)
+    ops.tuple_labels(coords.detach().contiguous(), None if lse is None else lse.detach().reshape(-1).contiguous(),
+                     pm["box"], pm["P"].reshape(B, 12).contiguous(), pm["cam"], T, V, J, patch_w, patch_h,
+                     rect_3d_w, threshold_px, label, weight, X, inliers, resid, status)
+    if full:
+        return label, weight, X, status, inliers, resid
+    return label, weight
 
 
 def self_supervision_device(preds, meta, method="iterative", estimate_extrinsics=False):

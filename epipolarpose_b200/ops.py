@@ -21,6 +21,7 @@ _KERNELS_PER_CALL = {
     "epb_split16_batch": 3, "epb_split16": 3, "epb_bn_bwd_apply_split": 2, "epb_conv16_wgrad": 2,
     "epb_bn_bwd_reduce_mx": 2, "epb_bn_bwd_split": 3, "epb_softargmax_bwd_split": 3,
     "epb_patch_sample": 2, "epb_patch_sample_occ": 2, "epb_jpeg_decode": 14, "epb_refiner_forward": 12,
+    "epb_tuple_labels": 2,
 }
 
 
@@ -559,6 +560,14 @@ def triangulate_robust(u, stride_u, P, w, NT, V, J, threshold_px, X, inliers, re
     _call("epb_triangulate_robust", _p(u, torch.float64), stride_u, _p(P, torch.float64),
           _p(w, torch.float64), NT, V, J, float(threshold_px), _p(X, torch.float64),
           _p(inliers, torch.int32), _p(resid, torch.float64), _p(status, torch.int32), _stream())
+
+
+def tuple_labels(coords, lse_ws, box, P, cam, T, V, J, patch_w, patch_h, rect3d_w, threshold_px, label, weight,
+                 X, inliers, resid, status):
+    _call("epb_tuple_labels", _p(coords), _p(lse_ws), _p(box, torch.float64), _p(P, torch.float64),
+          _p(cam, torch.float64), T, V, J, float(patch_w), float(patch_h), float(rect3d_w), float(threshold_px),
+          _p(label), _p(weight), _p(X, torch.float64), _p(inliers, torch.int32), _p(resid, torch.float64),
+          _p(status, torch.int32), _stream())
 
 
 def relative_pose(u, stride_u, intr, box, B, J, rect3d_w, Pa, Pb, cam, inliers, status, diag=None):

@@ -484,6 +484,29 @@ int epb_project_labels(const double* X, const double* cam, const double* box,
                        int B, int J, double patch_w, double patch_h,
                        double rect3d_w, float* label, float* weight,
                        epb_stream_t stream);
+/* Online self-supervised labels of whole camera tuples (not in the reference, which pairs two
+ * views): the training soft-argmax output of a view-major batch of T tuples of V views (row v*T + t
+ * is view v of tuple t; for V = 2 the reference's [cam_1 ; cam_2]) -> the labels and weights the
+ * joint loss consumes.  Per row, the image points with the arithmetic of epb_patch_to_image; per
+ * (tuple, joint), epb_triangulate_robust over the V views; per (row, joint), the label arithmetic
+ * of epb_project_labels (root = joint 0).
+ *   coords [V*T][J*3] f32; lse_ws [V*T][J][2] f32 or NULL: the softmax workspace of
+ *   epb_softargmax_fwd, whose second entry (the peak softmax probability of the joint) weights the
+ *   view in the robust refit (it never decides which views agree); NULL: weights 1.
+ *   box [V*T][6], P [V*T][12], cam [V*T][16] f64 in the layouts above.
+ * Outputs: X [T][J][3], inliers [T][J] (bit v: view v), resid [T][J], status [T][J] as
+ * epb_triangulate_robust; label, weight [V*T][J*3] f32.
+ * Weight rule: the three entries of (row v*T + t, joint j) have weight 1 and the projected label
+ * when status[t][j] = 1, status[t][0] = 1 (the root), and both the joint and the root lie at a
+ * positive, finite camera-frame depth in view v (with finite cameras and boxes the label is then
+ * finite); otherwise label 0 and weight 0, so a tuple whose root failed contributes nothing.  Views
+ * outside the inlier set still receive the label.  No NaN or Inf is written; deterministic; two
+ * launches, no host synchronisation.  EPB_EINVAL: V outside 2..8, a negative size, V*T*J > 2^31-1,
+ * threshold_px not finite or <= 0. */
+int epb_tuple_labels(const float* coords, const float* lse_ws, const double* box, const double* P,
+                     const double* cam, int T, int V, int J, double patch_w, double patch_h,
+                     double rect3d_w, double threshold_px, float* label, float* weight,
+                     double* X, int32_t* inliers, double* resid, int32_t* status, epb_stream_t stream);
 
 /* H36M evaluation protocol per sample (lib/dataset/h36m.py:168-378: CamBackProj
  * lib/utils/prep_h36m.py:85-89, compute_similarity_transform(..., compute_optimal_scale=True)
