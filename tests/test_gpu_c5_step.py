@@ -1,6 +1,5 @@
 """The C5 training step (R101, 384 x 384, J = 17, D = 96; bench.py --workload c5) against float64
-kernel by kernel at its own sizes, and a coverage gate: every C-ABI entry one C5-composition step
-calls must name the tests that hold it to float64 at C5 sizes (COVERAGE_C5).
+kernel by kernel at its own sizes.  tests/test_step_coverage.py gates the C5 step on these tests.
 
 C5 runs code C4 does not.  J D = 1632 is not a whole number of 64-channel blocks, so the head's
 backward leaves the split path (Engine16.takes_logit_sink() is False): the fp32 NHWC soft-argmax
@@ -13,20 +12,12 @@ n = 3264 in the joint loss, J = 17 in the geometry, R101's jobs and 53.4M parame
 Every reference is torch float64 on the device (or oracle/restate for the geometry), computed
 from the exact values the kernel read, in chunks of at most 8 images.  Bars (u = 2^-24):
 
-  * Shared kernels: the bars of the C4 tests, with C5's planner values (test_gpu_step_kernels,
-    test_gpu_bn_chain, test_gpu_split16 docstrings).  conv16 weight gradients: wgrad16's pixel
-    splits (`_wgrad16_plan`, wgrad16.cu) leave each CTA a run of R = tiles_per_split x 64
-    pixels, so the bar is _tc_bar(WGRAD16_BASE, R, 3) (test_gpu_tf32: wgmma accumulates toward
-    zero); WGRAD16_BASE = 2e-4 is the C4 contract.
-  * Soft-argmax backward, fp32 NHWC: p (s - s_bar) per element within the model of the split
-    backward's bar (exp ((6 + 3.5 |v - m|) u), the fp32 s and s_bar (6u on their terms, which
-    for s_bar are its three products: they cancel where |s_bar| is small), the
-    kernel's s_bar from its forward coords + 1/2, its 1 / sum exp from lse) without the
-    plane-rounding term: the output is fp32.
-  * epb_colsum: each thread adds kRowsPerThread = 64 rows in fp32 (<= 64 u sum|x| per column),
-    the CTA's row slots and all CTAs add in double (<= (rpi + CTAs) 2^-53 sum|x|), the result
-    rounds once to fp32 (u |S|).  Double atomics reorder between runs: two runs agree within one
-    fp32 ulp.
+  * Shared kernels: the bars of the C4 tests, with C5's planner values (tests/step_cases.py).
+    conv16 weight gradients: wgrad16's pixel splits (`_wgrad16_plan`, wgrad16.cu) leave each CTA
+    a run of R = tiles_per_split x 64 pixels, so the bar is _tc_bar(WGRAD16_BASE, R, 3) (wgmma
+    accumulates toward zero); WGRAD16_BASE = 2e-4 is the C4 contract.
+  * Soft-argmax backward, fp32 NHWC: step_cases._sabwd_ref_bar.
+  * epb_colsum: step_cases._check_colsum.
   * 3xTF32 final-layer weight gradient: _tc_bar(WGRAD_BAR, R, 3) with R the pixel run of one CTA
     from the TF32 wgrad planner (`_tf32_wgrad_plan`, conv_tc_wgrad.cu launch_wgrad).  Before the
     planner capped R, C5's final layer ran 5 splits of R = 117984 pixels: a bar of 2.0e-3, which
@@ -39,19 +30,17 @@ from the exact values the kernel read, in chunks of at most 8 images.  Bars (u =
   * 3xTF32 data gradient, K = 1632: _tc_bar(FPROP_BAR, 1632, 3) = 2.7e-5.
   * conv16 final forward (K = 256 + bias): 5e-5 of max|ref|, the split suite's bar.
 
-CPU tests below restate both planners, run the gate through the emulated ABI, and show against
-numpy emulations that the soft-argmax-backward bar rejects s_bar without the +1/2 shift, the
-colsum bar a dropped last partial CTA, and the plan-derived TF32 wgrad bar a lost correction
-pass at C5's run length."""
-import math
-
+CPU tests below check the restated planners (step_cases) and show against numpy emulations that
+the soft-argmax-backward bar rejects s_bar without the +1/2 shift, the colsum bar a dropped last
+partial CTA, and the plan-derived TF32 wgrad bar a lost correction pass at C5's run length."""
 import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_step_kernels import (NUM_SMS, U, _bench_meta, _cfg, _entry_names, _missing_coverage,
-                                         _record_calls)
-from tests.test_gpu_tf32 import FPROP_BAR, WGRAD_BAR, _emul_mma, _tc_bar, _tf32_np, _trunc_np
+from tests import step_cases as sc
+from tests.step_cases import (C5_LAYERS, FPROP_BAR, KPIX, RUN_BLOCKS3, U, WGRAD_BAR, _check_colsum,
+                              _check_softargmax_bwd_fp32, _emul_mma, _sabwd_ref_bar, _split_dev, _tc_bar,
+                              _tf32_np, _tf32_wgrad_plan, _trunc_np, _wgrad16_plan)
 
 gpu = pytest.mark.gpu
 
@@ -59,103 +48,8 @@ N5, HW5, J5, D5, HM5 = 64, 384, 17, 96, 96        # one GPU's C5 batch: 16 tuple
 M5 = N5 * HM5 * HM5                                # pixels of the last deconv / final layer: 589824
 WGRAD16_BASE = 2e-4
 
-S = "test_gpu_c5_step.py::"
-COVERAGE_C5 = {
-    "epb_im2col_split": [S + "test_c5_im2col_split_bit_exact_at_stem"],
-    "epb_conv16_fprop": [S + "test_c5_conv16_layers_vs_torch_float64", S + "test_c5_final_conv16_fprop_vs_float64",
-                         S + "test_c5_conv16_stats_vs_float64"],
-    "epb_conv16_wgrad": [S + "test_c5_conv16_layers_vs_torch_float64"],
-    "epb_bn_finalize_scale": [S + "test_c5_bn_finalize_scale_vs_float64"],
-    "epb_bn_finalize": [S + "test_c5_bn_finalize_vs_float64"],
-    "epb_bn_act_split": [S + "test_c5_bn_act_split_vs_float64"],
-    "epb_bn_relu_maxpool_split": [S + "test_c5_bn_relu_maxpool_split_vs_float64"],
-    "epb_maxpool_bwd": [S + "test_c5_maxpool_bwd_vs_float64"],
-    "epb_bn_bwd_split": [S + "test_c5_bn_bwd_split_vs_float64"],
-    "epb_softargmax_fwd": [S + "test_c5_softargmax_fwd_vs_float64"],
-    "epb_softargmax_bwd": [S + "test_c5_softargmax_bwd_fp32_vs_float64"],
-    "epb_colsum": [S + "test_c5_colsum_vs_float64"],
-    "epb_conv_wgrad": [S + "test_c5_final_tf32_wgrad_vs_float64"],
-    "epb_conv_fprop": [S + "test_c5_final_tf32_dgrad_vs_float64"],
-    "epb_jointloss_fwd_bwd": [S + "test_c5_jointloss_vs_float64"],
-    "epb_split16_batch": [S + "test_c5_split16_batch_bit_exact_on_model_jobs"],
-    "epb_pack_weight_batch": [S + "test_c5_pack_weight_batch_bit_exact_on_model_jobs"],
-    "epb_adam_step_dev": [S + "test_c5_fused_adam_vs_float64_on_model_buffer"],
-    "epb_patch_to_image": [S + "test_c5_selfsup_geometry_j17"],
-    "epb_triangulate": [S + "test_c5_selfsup_geometry_j17"],
-    "epb_project_labels": [S + "test_c5_selfsup_geometry_j17"],
-}
-# the head's fp32 backward: entries the C4 step does not call
-HEAD_C5 = {"epb_softargmax_bwd", "epb_colsum", "epb_conv_wgrad", "epb_conv_fprop"}
 
-
-# ------------------------------------------------------------------ planners restated
-KPIX, WM_TF32 = 32, 128          # conv_tc_wgrad.cu: pixels per tile, co rows per tile
-RUN_BLOCKS3 = 184                # conv_tc_wgrad.cu kMaxRunBlocks3
-
-
-def _tf32_wgrad_plan(M, Cin, Cout, T, NS, cap=True):
-    """conv_tc_wgrad.cu launch_wgrad: (pixel run per CTA, splits, tiles); cap=False is the
-    planner without the run cap"""
-    bnw = 128 if Cin >= 128 else (64 if Cin >= 64 else 32)
-    co_tiles, ci_tiles = -(-Cout // WM_TF32), -(-Cin // bnw)
-    total = T * ci_tiles
-    groups = -(-total // (128 // bnw))
-    nb = -(-total // groups)
-    tiles = co_tiles * -(-total // nb)
-    max_splits = -(-M // (8 * KPIX))
-    min_splits = -(-M // (RUN_BLOCKS3 * 3 // NS * KPIX)) if cap else 1
-    splits, best, sp = min_splits, -1, min_splits
-    while sp <= max_splits and (sp - min_splits) * tiles <= 3 * NUM_SMS:
-        cost = -(-(sp * tiles) // NUM_SMS) * (-(-(-(-M // sp)) // KPIX) + 6)
-        if best < 0 or cost < best:
-            best, splits = cost, sp
-        sp += 1
-    rows = -(-(-(-M // splits)) // KPIX) * KPIX
-    return rows, -(-M // rows), tiles
-
-
-def _choose_tile(N, Hp, Wp, rows):
-    """split16_common.cuh epb_choose_tile: (tw, th, tn)"""
-    best, out = -1, (rows, 1, 1)
-    a = rows
-    while a >= 1:
-        b = rows // a
-        while b >= 1:
-            c = rows // (a * b)
-            cov = -(-Wp // a) * -(-Hp // b) * -(-N // c)
-            if best < 0 or cov < best:
-                best, out = cov, (a, b, c)
-            b >>= 1
-        a >>= 1
-    return out
-
-
-def _wgrad16_plan(gm, ws_floats=48 << 20):
-    """wgrad16.cu epb_conv16_wgrad: (pixel run per CTA = tiles_per_split x 64, splits)"""
-    KT = 64
-    N, Hp, Wp = gm.N, gm.Hp, gm.Wp
-    if gm.T == 1 and gm.is_ == 1 and gm.os == 1 and gm.dh[0] == 0 and gm.dw[0] == 0 and \
-            Hp == gm.Hi and Wp == gm.Wi and Hp == gm.Ho and Wp == gm.Wo:
-        N, Hp, Wp = 1, 1, gm.N * gm.Hp * gm.Wp
-    tw, th, tn = _choose_tile(N, Hp, Wp, KT)
-    tiles = -(-Wp // tw) * -(-Hp // th) * -(-N // tn)
-    CH = gm.T * (gm.Cin // 64)
-    swap = gm.T == 1 and CH < 2 and gm.Cout // 64 > CH
-    if swap:
-        CH, Nn = gm.Cout // 64, gm.Cin
-    else:
-        Nn = gm.Cout
-    bn = 64 if Nn <= 64 else 128
-    basec = ((CH + 1) // 2) * -(-Nn // bn)
-    splits = min(2 * NUM_SMS // basec, tiles // 8)
-    per_split = gm.Cout * gm.Tw * gm.Cin
-    if splits * per_split > ws_floats:
-        splits = ws_floats // per_split
-    splits = max(splits, 1)
-    tps = -(-tiles // splits)
-    return tps * KT, -(-tiles // tps)
-
-
+# ------------------------------------------------------------------ the restated planners
 def test_tf32_wgrad_planner_caps_the_accumulation_run():
     """The restated planner: every CTA's pixel run R stays within 184 x 32 (three passes) or
     3 x that (one pass), so _tc_bar(WGRAD_BAR, R, passes) <= 1e-4, at C4 and C5 layer shapes and
@@ -181,100 +75,7 @@ def test_tf32_wgrad_planner_caps_the_accumulation_run():
                 assert (r, sp) == _tf32_wgrad_plan(M, cin, cout, T, ns, cap=False)[:2]
 
 
-# ------------------------------------------------------------------ coverage gate
-def test_coverage_c5_gate_has_teeth():
-    """Deleting any row, or pointing one at a test that does not exist, fails the gate."""
-    rec = sorted(COVERAGE_C5)
-    assert _missing_coverage(rec, COVERAGE_C5) == ([], [])
-    for k in rec:
-        t = dict(COVERAGE_C5)
-        del t[k]
-        assert _missing_coverage(rec, t)[0] == [k]
-    t = dict(COVERAGE_C5, epb_colsum=[S + "test_no_such_test"])
-    assert _missing_coverage(rec, t)[1]
-
-
-def test_coverage_c5_gate_cpu_emulated_step():
-    """One f16x3 step of C5's head composition (R18 trunk, J = 17, D = 96, 2 tuples x 4 views of
-    64 x 64 -> 16 x 16 heat-maps) through the emulated ABI: GraphedTrainStep.eager_step,
-    SmoothL1JointLocationLoss, FusedAdam, given labels (no CPU geometry).  The head takes the
-    fp32 path, so the step records the four entries C4 does not; every entry has a row."""
-    import lib.models as models
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    import lib.utils.utils as Ut
-    from epipolarpose_b200 import ops
-    from tests import emul_ops
-    rec, depth, saved = set(), [0], {}
-    for k, e in _entry_names(ops).items():
-        if not hasattr(emul_ops, k):
-            continue
-        f = saved[k] = getattr(emul_ops, k)
-
-        def wrap(*a, _f=f, _e=e, **kw):
-            if depth[0] == 0:
-                rec.update(_e)
-            depth[0] += 1
-            try:
-                return _f(*a, **kw)
-            finally:
-                depth[0] -= 1
-        setattr(emul_ops, k, wrap)
-    il._backend[0], Ut._backend[0] = emul_ops, emul_ops
-    try:
-        J, D, HW, B = J5, D5, 64, 8
-        torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(_cfg(18, J, D, HW), False, ops=emul_ops, precision="f16x3").train()
-        assert not m._engine().takes_logit_sink()
-        opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-        step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
-        g = torch.Generator().manual_seed(1)
-        loss = step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
-                               torch.ones(B, J * 3), None)
-        assert math.isfinite(float(loss))
-    finally:
-        for k, f in saved.items():
-            setattr(emul_ops, k, f)
-        il._backend[0] = Ut._backend[0] = ops
-    print("emulated C5-head step calls: %s" % sorted(rec))
-    assert HEAD_C5 <= rec, "the C5 head no longer takes the fp32 path: %s" % sorted(HEAD_C5 - rec)
-    assert "epb_softargmax_bwd_split" not in rec
-    missing, dangling = _missing_coverage(rec, COVERAGE_C5)
-    assert not missing, "entries without a float64 test at C5 size: %s" % missing
-    assert not dangling, dangling
-
-
 # ------------------------------------------------------------------ bars shared by the CPU and GPU tests
-def _sabwd_ref_bar(v, coords, lse, dco, H, W, D):
-    """float64 p (s - s_bar) for logits v [B, H, W, J, D] and its per-element bar (module
-    docstring) from the kernel's own coords / lse"""
-    B, J = v.shape[0], v.shape[3]
-    dev = v.device
-    xs = torch.arange(W, device=dev, dtype=torch.float64).view(1, 1, W, 1, 1)
-    ys = torch.arange(H, device=dev, dtype=torch.float64).view(1, H, 1, 1, 1)
-    zs = torch.arange(D, device=dev, dtype=torch.float64).view(1, 1, 1, 1, D)
-    m = v.amax((1, 2, 4), keepdim=True)
-    ex = torch.exp(v - m)
-    tot = ex.sum((1, 2, 4), keepdim=True)
-    p = ex / tot
-    del ex
-    dc = dco.double().view(B, 1, 1, J, 3)
-    gx, gy, gz = dc[..., 0:1] / W, dc[..., 1:2] / H, dc[..., 2:3] / D
-    s_ = gx * xs + gy * ys + gz * zs
-    sbar = (p * s_).sum((1, 2, 4), keepdim=True)
-    dl = p * (s_ - sbar)
-    cr = coords.double().view(B, 1, 1, J, 3)
-    tx, ty, tz = gx * (cr[..., 0:1] + 0.5) * W, gy * (cr[..., 1:2] + 0.5) * H, gz * (cr[..., 2:3] + 0.5) * D
-    sbar_k = tx + ty + tz
-    sbar_t = tx.abs() + ty.abs() + tz.abs()              # s_bar's terms: they may cancel
-    ik = lse.view(B, J, 2)[..., 1].double().view(B, 1, 1, J, 1)
-    e_inv = (ik * tot - 1).abs()
-    e = p * ((6 + 3.5 * (v - m).abs()) * U * (s_ - sbar).abs()
-             + 6 * U * ((gx * xs).abs() + (gy * ys).abs() + (gz * (zs + 3)).abs() + sbar_t)
-             + (sbar_k - sbar).abs() + e_inv * (s_ - sbar).abs())
-    return dl, e
-
-
 def _colsum_bar(x64, rpi, ctas):
     S_ = x64.sum(0)
     return S_, 64 * U * x64.abs().sum(0) + (rpi + ctas) * 2.0 ** -53 * x64.abs().sum(0) + U * S_.abs()
@@ -400,71 +201,15 @@ def dev():
     return torch.device("cuda:0")
 
 
-_MODEL = {}
-
-
 @pytest.fixture(scope="module", autouse=True)
 def _release_device_memory():
     """The C5 references hold tens of GB at their peak: after the module, drop its cached model
     and conv outputs and hand the allocator's reserve back to the device for the tests after it."""
     yield
-    from tests import test_gpu_bn_chain
-    _MODEL.clear()
-    for k in [k for k in test_gpu_bn_chain._PRODUCED if k[0].startswith("c5_")]:
-        del test_gpu_bn_chain._PRODUCED[k]
-    if torch.cuda.is_initialized():
-        import gc
-        gc.collect()
-        torch.cuda.empty_cache()
+    sc.release("c5_")
 
 
-def _r101(dev):
-    """the C5 model (R101, J = 17, D = 96, 384 x 384, f16x3) with FusedAdam over its parameters"""
-    if "m" not in _MODEL:
-        import lib.models as models
-        import lib.utils.utils as Ut
-        torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(_cfg(101, J5, D5, HW5), False, precision="f16x3").to(dev).train()
-        _MODEL["m"] = m
-        _MODEL["opt"] = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-    return _MODEL["m"], _MODEL["opt"]
-
-
-# ------------------------------------------------------------------ 1. coverage gate, GPU half
-@gpu
-def test_coverage_c5_gate_step(dev):
-    """One C5-composition step at a reduced batch (R101, J = 17, D = 96, 2 tuples x 4 views of
-    384 x 384): GraphedTrainStep(online=True, method="iterative").eager_step, SmoothL1,
-    FusedAdam.  It calls the four fp32 head entries, and every entry has a row in COVERAGE_C5
-    naming existing tests."""
-    import lib.models as models
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    import lib.utils.img_utils as iu
-    import lib.utils.utils as Ut
-    tuples = 2
-    B = 4 * tuples
-    torch.manual_seed(0)
-    m = models.pose3d_resnet.get_pose_net(_cfg(101, J5, D5, HW5), False, precision="f16x3").to(dev).train()
-    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J5).to(dev), opt, online=True, method="iterative")
-    meta = {k: v.to(dev) for k, v in _bench_meta(tuples).items()}
-    x = torch.randn(B, 3, HW5, HW5, device=dev)
-    with _record_calls() as names:
-        loss = step.eager_step(x, None, None, iu.pack_meta(meta, B, dev))
-        torch.cuda.synchronize()
-    assert math.isfinite(float(loss))
-    print("  C5 step calls %d entries:" % len(names))
-    for e in sorted(names):
-        print("    %-28s -> %s" % (e, ", ".join(COVERAGE_C5.get(e, ["(none)"]))))
-    assert HEAD_C5 <= names, sorted(HEAD_C5 - names)
-    assert "epb_adam_step_dev" in names and "epb_triangulate" in names
-    missing, dangling = _missing_coverage(names, COVERAGE_C5)
-    assert not missing, "entries without a float64 test at C5 size: %s" % missing
-    assert not dangling, dangling
-
-
-# ------------------------------------------------------------------ 2. the head at C5 sizes
+# ------------------------------------------------------------------ 1. the head at C5 sizes
 def _final_conv():
     from epipolarpose_b200 import net
     return net.Conv("final_layer", "conv", 256, J5 * D5, 1, 1, 0, 0)
@@ -477,7 +222,6 @@ def test_c5_final_conv16_fprop_vs_float64(dev):
     max|ref|.  Run into two buffers pre-filled with different NaN sentinels and followed by a guard
     band: every element written, identically, and nothing past the end."""
     from epipolarpose_b200 import ops
-    from tests.test_gpu_bn_chain import _split_dev
     conv = _final_conv()
     C = conv.cout
     g = torch.Generator(device=dev).manual_seed(91)
@@ -516,8 +260,7 @@ def test_c5_final_conv16_fprop_vs_float64(dev):
 def test_c5_softargmax_fwd_vs_float64(dev, kind):
     """N = 64, J = 17, D = 96, 96 x 96 NHWC (3.85 GB of logits): 408 threads per CTA, the bar of
     test_softargmax_fwd_vs_float64_at_bench_shape with _nhwc_geometry(64, 17, 96, 96, 96)."""
-    from tests.test_gpu_step_kernels import _check_softargmax_fwd
-    _check_softargmax_fwd(dev, kind, N5, J5, D5, HM5, HM5)
+    sc._check_softargmax_fwd(dev, kind, N5, J5, D5, HM5, HM5)
 
 
 @gpu
@@ -527,32 +270,6 @@ def test_c5_softargmax_bwd_fp32_vs_float64(dev):
     _check_softargmax_bwd_fp32(dev, N5, J5, D5, HM5, HM5)
 
 
-def _check_softargmax_bwd_fp32(dev, N, J, D, H, W):
-    """epb_softargmax_bwd (fp32 NHWC) at one shape against float64 within _sabwd_ref_bar"""
-    from epipolarpose_b200 import ops
-    C = J * D
-    g = torch.Generator(device=dev).manual_seed(93)
-    logits = torch.randn(N, H, W, C, device=dev, generator=g) * 3
-    dco = torch.randn(N, J * 3, device=dev, generator=g)
-    coords, lse = torch.empty(N, J * 3, device=dev), torch.empty(N * J * 2, device=dev)
-    ops.softargmax_fwd(logits, 1, N, J, D, H, W, coords, lse)
-    dl = torch.empty_like(logits)
-    ops.softargmax_bwd(logits, 1, N, J, D, H, W, coords, lse, dco, dl)
-    torch.cuda.synchronize()
-    ratio, worst = 0.0, 0.0
-    B = 8
-    for n0 in range(0, N, B):
-        v = logits[n0:n0 + B].double().view(B, H, W, J, D)
-        ref, e = _sabwd_ref_bar(v, coords[n0:n0 + B], lse.view(N, J * 2)[n0:n0 + B], dco[n0:n0 + B], H, W, D)
-        del v
-        err = (dl[n0:n0 + B].double().view(B, H, W, J, D) - ref).abs()
-        worst = max(worst, float(err.max()))
-        ratio = max(ratio, float((err / (e + 1e-300)).max()))
-        del ref, e, err
-    print("  softargmax bwd fp32 N %d J %d D %d %dx%d: max err %.3e, worst err / bar %.3f" % (N, J, D, H, W, worst, ratio))
-    assert ratio <= 1.0
-
-
 @gpu
 @pytest.mark.parametrize("M", [M5, M5 - 23], ids=["589824", "589801"])
 def test_c5_colsum_vs_float64(dev, M):
@@ -560,33 +277,6 @@ def test_c5_colsum_vs_float64(dev, M):
     last CTA of 41 rows) against float64 column sums within the module's bar; a second run
     within one fp32 ulp."""
     _check_colsum(dev, M, J5 * D5)
-
-
-def _check_colsum(dev, M, C):
-    """epb_colsum over M x C against float64 column sums within _colsum_bar's terms"""
-    from epipolarpose_b200 import ops
-    g = torch.Generator(device=dev).manual_seed(95)
-    x = torch.randn(M, C, device=dev, generator=g) * 1e-3
-    x[:, :8] += 1e-3                                            # columns with a consistent sign
-    out, out2 = torch.empty(C, device=dev), torch.empty(C, device=dev)
-    ops.colsum(x, M, C, out)
-    ops.colsum(x, M, C, out2)
-    torch.cuda.synchronize()
-    ref = torch.zeros(C, device=dev, dtype=torch.float64)
-    sab = torch.zeros(C, device=dev, dtype=torch.float64)
-    for r0 in range(0, M, 1 << 16):
-        xd = x[r0:r0 + (1 << 16)].double()
-        ref += xd.sum(0)
-        sab += xd.abs().sum(0)
-    rpi = max(256 // (C // 4), 1)                               # bn.cu make_rowmap
-    ctas = -(-M // (64 * rpi))
-    bar = 64 * U * sab + (rpi + ctas) * 2.0 ** -53 * sab + U * ref.abs()
-    err = (out.double() - ref).abs()
-    ulp = (out.double().abs() * 2.0 ** -23).clamp_min(2.0 ** -149)
-    print("  colsum M %d C %d: max err %.3e, worst err / bar %.3f, second run identical %s"
-          % (M, C, float(err.max()), float((err / bar).max()), bool(torch.equal(out, out2))))
-    assert bool((err <= bar).all())
-    assert bool(((out.double() - out2.double()).abs() <= ulp).all())
 
 
 @gpu
@@ -652,42 +342,22 @@ def test_c5_final_tf32_dgrad_vs_float64(dev):
 @pytest.mark.parametrize("kind,norm", [(2, 0), (1, 0), (1, 1), (2, 1)], ids=["smoothl1", "l1", "l1_norm", "smoothl1_norm"])
 def test_c5_jointloss_vs_float64(dev, kind, norm):
     """epb_jointloss_fwd_bwd at N = 64, J = 17 (n = 3264, not a multiple of 1024)."""
-    from tests.test_gpu_step_kernels import _check_jointloss
-    _check_jointloss(dev, kind, norm, N5, J5)
+    sc._check_jointloss(dev, kind, norm, N5, J5)
 
 
-# ------------------------------------------------------------------ 3. shared kernels at C5 sizes
-# every distinct conv of R101 at 384 x 384 (trunk at 96 / 48 / 24 / 12, deconvs 12 -> 96), the
-# stem's patch-matrix conv; (name, kind, cin, cout, k, stride, pad, input hw)
-C5_LAYERS = [
-    ("stem_col_192_64", "conv", 192, 64, 1, 1, 0, 192),
-    ("l1_1x1_64_64", "conv", 64, 64, 1, 1, 0, 96), ("l1_3x3_64", "conv", 64, 64, 3, 1, 1, 96),
-    ("l1_1x1_64_256", "conv", 64, 256, 1, 1, 0, 96), ("l1_1x1_256_64", "conv", 256, 64, 1, 1, 0, 96),
-    ("l2_1x1_256_128", "conv", 256, 128, 1, 1, 0, 96), ("l2_3x3_s2", "conv", 128, 128, 3, 2, 1, 96),
-    ("l2_1x1_s2_down", "conv", 256, 512, 1, 2, 0, 96), ("l2_3x3_128", "conv", 128, 128, 3, 1, 1, 48),
-    ("l2_1x1_512_128", "conv", 512, 128, 1, 1, 0, 48), ("l3_3x3_s2", "conv", 256, 256, 3, 2, 1, 48),
-    ("l3_1x1_s2_down", "conv", 512, 1024, 1, 2, 0, 48), ("l3_3x3_256", "conv", 256, 256, 3, 1, 1, 24),
-    ("l3_1x1_1024_256", "conv", 1024, 256, 1, 1, 0, 24), ("l3_1x1_256_1024", "conv", 256, 1024, 1, 1, 0, 24),
-    ("l4_3x3_s2", "conv", 512, 512, 3, 2, 1, 24), ("l4_1x1_s2_down", "conv", 1024, 2048, 1, 2, 0, 24),
-    ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 12), ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 12),
-    ("deconv0", "deconv", 2048, 256, 4, 2, 1, 12), ("deconv1", "deconv", 256, 256, 4, 2, 1, 24),
-    ("deconv2", "deconv", 256, 256, 4, 2, 1, 48),
-]
-
-
+# ------------------------------------------------------------------ 2. shared kernels at C5 sizes
 @gpu
 @pytest.mark.parametrize("layer", C5_LAYERS, ids=[c[0] for c in C5_LAYERS])
 def test_c5_conv16_layers_vs_torch_float64(dev, layer):
     """conv16 fprop (statistics), dgrad and wgrad at N = 64 against torch float64 (the bars of
     test_conv16_bench_layer_shapes_vs_torch_float64); the wgrad bar from wgrad16's planner."""
     from epipolarpose_b200 import net, ops
-    from tests.test_gpu_split16 import _check_conv16_layer
     name, kind, cin, cout, k, s, p, hw = layer
     conv = net.Conv("t", kind, cin, cout, k, s, p, 0)
     plans = [_wgrad16_plan(gm) for gm in conv.fprop_geoms(ops, N5, hw, hw, 3) if gm is not None]
     R = max(r for r, _ in plans)
     bar = _tc_bar(WGRAD16_BASE, R, 3)
-    e = _check_conv16_layer(dev, layer, N5, bar)
+    e = sc._check_conv16_layer(dev, layer, N5, bar)
     print("  C5 %-18s fprop %.2e dgrad %.2e wgrad %.2e (splits %s, run %d pixels, bar %.2e)"
           % (name, e[0], e[1], e[2], [sp for _, sp in plans], R, bar))
 
@@ -700,44 +370,38 @@ C5_STATS = [("c5_stem_col_192_64", "conv", 192, 64, 1, 1, 0, N5, 192, [(0, 0)]),
 @pytest.mark.parametrize("case", C5_STATS, ids=[c[0] for c in C5_STATS])
 def test_c5_conv16_stats_vs_float64(dev, case):
     """conv16 BatchNorm statistics at M = 2359296 (stem) and 589824 (layer1)."""
-    from tests.test_gpu_bn_chain import test_conv16_stats_vs_float64
-    test_conv16_stats_vs_float64(dev, case)
+    sc.check_conv16_stats(dev, case)
 
 
 @gpu
 @pytest.mark.parametrize("M", [2359296, 589824, 9216])
 def test_c5_bn_finalize_scale_vs_float64(dev, M):
-    from tests.test_gpu_bn_chain import test_bn_finalize_scale_vs_float64
-    test_bn_finalize_scale_vs_float64(dev, M)
+    sc.check_bn_finalize_scale(dev, M)
 
 
 @gpu
 @pytest.mark.parametrize("M", [589824, 147456, 36864, 9216])
 def test_c5_bn_finalize_vs_float64(dev, M):
     """the downsample layers' BatchNorm of R101 at 384"""
-    from tests.test_gpu_step_kernels import test_bn_finalize_vs_float64_at_bench_M
-    test_bn_finalize_vs_float64_at_bench_M(dev, M)
+    sc.check_bn_finalize(dev, M)
 
 
 @gpu
 @pytest.mark.parametrize("res", ["none", "split", "affine"])
 def test_c5_bn_act_split_vs_float64(dev, res):
     """layer1's conv16 output (589824 x 256) -> bn_finalize_scale -> bn_act_split"""
-    from tests.test_gpu_bn_chain import _check_bn_act_split
-    _check_bn_act_split(dev, res, C5_STATS[1])
+    sc._check_bn_act_split(dev, res, C5_STATS[1])
 
 
 @gpu
 def test_c5_bn_relu_maxpool_split_vs_float64(dev):
     """the stem's conv16 output (64 x 192 x 192 x 64) -> bn_relu_maxpool_split -> 96 x 96"""
-    from tests.test_gpu_bn_chain import _check_bn_relu_maxpool_split
-    _check_bn_relu_maxpool_split(dev, C5_STATS[0])
+    sc._check_bn_relu_maxpool_split(dev, C5_STATS[0])
 
 
 @gpu
 def test_c5_maxpool_bwd_vs_float64(dev):
-    from tests.test_gpu_step_kernels import _check_maxpool_bwd
-    _check_maxpool_bwd(dev, N5, 192)
+    sc._check_maxpool_bwd(dev, N5, 192)
 
 
 C5_BWD = [(2359296, 64), (589824, 256), (9216, 2048)]
@@ -747,35 +411,30 @@ C5_BWD = [(2359296, 64), (589824, 256), (9216, 2048)]
 @pytest.mark.parametrize("mode", ["relu", "bits_inplace"])
 @pytest.mark.parametrize("M,C", C5_BWD, ids=["%dx%d" % s for s in C5_BWD])
 def test_c5_bn_bwd_split_vs_float64(dev, M, C, mode):
-    from tests.test_gpu_bn_chain import test_bn_bwd_split_vs_float64_at_bench_M
-    test_bn_bwd_split_vs_float64_at_bench_M(dev, M, C, mode)
+    sc.check_bn_bwd_split(dev, M, C, mode)
 
 
 @gpu
 def test_c5_im2col_split_bit_exact_at_stem(dev):
     """the stem's patch matrix of 64 images of 384 x 384"""
-    from tests.test_gpu_step_kernels import _check_im2col_split
-    _check_im2col_split(dev, _r101(dev)[0]._engine().stem_kpad, N5, HW5)
+    sc._check_im2col_split(dev, sc.bench_model(dev, "c5")[0]._engine().stem_kpad, N5, HW5)
 
 
 @gpu
 def test_c5_split16_batch_bit_exact_on_model_jobs(dev):
     """split16_batch on the jobs the f16x3 engine builds for R101 / J17 / D96 (1632-channel head)"""
-    from tests.test_gpu_step_kernels import _check_split16_batch
-    _check_split16_batch(dev, *_r101(dev))
+    sc._check_split16_batch(dev, *sc.bench_model(dev, "c5"))
 
 
 @gpu
 def test_c5_pack_weight_batch_bit_exact_on_model_jobs(dev):
-    from tests.test_gpu_step_kernels import _check_pack_weight_batch
-    _check_pack_weight_batch(dev, _r101(dev)[0])
+    sc._check_pack_weight_batch(dev, sc.bench_model(dev, "c5")[0])
 
 
 @gpu
 def test_c5_fused_adam_vs_float64_on_model_buffer(dev):
     """FusedAdam over R101 / J17 / D96's flat parameter buffer: steps 1, 2 and 1000"""
-    from tests.test_gpu_step_kernels import _check_fused_adam
-    _check_fused_adam(dev, *_r101(dev))
+    sc._check_fused_adam(dev, *sc.bench_model(dev, "c5"))
 
 
 @gpu
@@ -785,7 +444,7 @@ def test_c5_selfsup_geometry_j17(dev):
     test_c3_selfsup_chain_64_images)."""
     import lib.utils.img_utils as iu
     from oracle import restate
-    from tests.test_gpu_sizes import _ring_meta
+    from tests.golden_inputs import _ring_meta
     tuples, J = 16, J5
     B = 4 * tuples
     meta_np = _ring_meta(tuples, 1075)

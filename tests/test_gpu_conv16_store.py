@@ -17,7 +17,7 @@ import torch
 
 from tests import emul_ops as em
 from tests.conftest import relerr
-from tests.test_gpu_split16 import _rand_split, _weights_split
+from tests.step_cases import _rand_split, _weights_split
 
 pytestmark = pytest.mark.gpu
 

@@ -19,7 +19,7 @@ from torch.utils.data import DataLoader
 
 from tests import dataset_cases as dc
 from tests.conftest import ROOT
-from tests.test_jpeg_transcode_host import INTERVALS, _build, _runner
+from tests.transcode_cases import INTERVALS, _build, _runner
 
 pytestmark = pytest.mark.gpu
 

@@ -164,7 +164,7 @@ PATCH = 256.0
 @pytest.fixture(scope="module")
 def c1(dev):
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     return _model(dev, gi.SIZE_CASES["c1"], "f16x3", train=False)
 
 

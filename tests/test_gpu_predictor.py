@@ -1,6 +1,6 @@
 """GPU (-m gpu): the split-K conv16 entry (epb_conv16_fprop_splitk) and PosePredictor.
 
-- Split-K against torch float64 at every layer shape of the bench (test_gpu_split16.C4_LAYERS) for
+- Split-K against torch float64 at every layer shape of the bench (step_cases.C4_LAYERS_SPLIT16) for
   N = 1 and 32, at the planner's split count and at forced counts 2, 3 and K/64, with a bias so
   that a bias applied twice, or statistics that count the rows past the output view of a ragged
   tile, show.  Float64 uses the exact values the fp16 planes hold, so the bars are the fp32
@@ -26,11 +26,10 @@ import pytest
 import torch
 
 from tests import emul_splitk as es
-from tests.test_gpu_split16 import C4_LAYERS
+from tests.step_cases import C4_LAYERS_SPLIT16, _split_dev
 
 pytestmark = pytest.mark.gpu
 
-H16 = torch.float16
 LOGIT_BAR = 1e-4
 PATCH = 256.0
 
@@ -42,15 +41,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _split_dev(v, dev):
-    from epipolarpose_b200 import ops
-    h = torch.empty(2 * v.numel(), device=dev, dtype=H16)
-    sc = torch.ones(2, device=dev)
-    ops.split16_batch(ops.SplitBatch([(v.reshape(-1), h, sc)]))
-    val = ((h[:v.numel()].double() + h[v.numel():].double()) * float(sc[1])).view(v.shape)
-    return h.view((2,) + tuple(v.shape)), sc, val
-
-
 def _layer(dev, layer, N, seed=7):
     """conv, geoms, split operands, bias and the float64 reference [N, Ho, Wo, Cout] with bias."""
     import torch.nn.functional as F
@@ -59,10 +49,10 @@ def _layer(dev, layer, N, seed=7):
     conv = net.Conv("t", kind, cin, cout, k, s, p, 0)
     T = k * k
     g = torch.Generator(device=dev).manual_seed(seed)
-    x, x_sc, xv = _split_dev(torch.relu(torch.randn(N, hw, hw, cin, device=dev, generator=g)), dev)
+    x, x_sc, xv = _split_dev(torch.relu(torch.randn(N, hw, hw, cin, device=dev, generator=g)))
     w = torch.randn((cout, cin, k, k) if kind == "conv" else (cin, cout, k, k), device=dev,
                     generator=g) * (2.0 / (T * cin)) ** 0.5
-    wf, wf_sc, wfv = _split_dev(conv.pack(ops, w)[0], dev)
+    wf, wf_sc, wfv = _split_dev(conv.pack(ops, w)[0])
     bias = torch.randn(cout, device=dev, generator=g)
     pk = wfv.view(cout, T, cin)
     wq = pk.permute(0, 2, 1).reshape(cout, cin, k, k) if kind == "conv" else \
@@ -86,7 +76,7 @@ def _run(geoms, opnds, bias, out, stats, splits):
         ops.conv16_fprop_splitk(gm, x, x_sc, w, w_sc, out, bias, stats, s, ws)
 
 
-CASES = [(l, N) for l in C4_LAYERS for N in (1, 32)]
+CASES = [(l, N) for l in C4_LAYERS_SPLIT16 for N in (1, 32)]
 
 
 @pytest.mark.parametrize("case", CASES, ids=["%s-N%d" % (c[0][0], c[1]) for c in CASES])
@@ -108,7 +98,7 @@ def test_splitk_vs_torch_float64(dev, case):
         assert e1 <= 5e-5 and e2 <= 5e-5, "S=%s statistics %.3e / %.3e" % (splits, e1, e2)
 
 
-BITS = [c for c in C4_LAYERS if c[0] in ("l4_3x3_512", "deconv0", "l3_1x1_1024_256", "final")]
+BITS = [c for c in C4_LAYERS_SPLIT16 if c[0] in ("l4_3x3_512", "deconv0", "l3_1x1_1024_256", "final")]
 
 
 @pytest.mark.parametrize("layer", BITS, ids=[c[0] for c in BITS])
@@ -138,7 +128,7 @@ def test_splitk_writes_exactly_the_phase_view(dev):
     """deconv0 at N = 1 (2 tiles per phase, split 32 ways): every phase call writes its view and
     leaves the rest of the tensor and a guard band past its end at their sentinels."""
     sentinels, guard = (0x7FC0DEAD, 0x7FC0BEEF), 4096
-    layer = [c for c in C4_LAYERS if c[0] == "deconv0"][0]
+    layer = [c for c in C4_LAYERS_SPLIT16 if c[0] == "deconv0"][0]
     conv, geoms, opnds, bias, ref = _layer(dev, layer, 1)
     shape = tuple(ref.shape)
     n = int(np.prod(shape))
@@ -164,7 +154,7 @@ def test_splitk_writes_exactly_the_phase_view(dev):
 @pytest.fixture(scope="module")
 def c1(dev):
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     c = gi.SIZE_CASES["c1"]
     return c, _model(dev, c, "f16x3", train=False)
 
@@ -203,7 +193,7 @@ def _close(pred, model, x):
 
 def test_predictor_c1_vs_reference(golden, c1):
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _check_output
+    from tests.golden_inputs import _check_output
     from lib.core.inference import PosePredictor
     c, model = c1
     pred = PosePredictor(model, flip_test=False)
@@ -272,7 +262,7 @@ def test_predictor_boxes(c1):
 def test_predictor_graphs_snapshot_and_modes(dev):
     from lib.core.inference import PosePredictor
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     model = _model(dev, gi.SIZE_CASES["c1"], "f16x3", train=False)     # its own: the test edits it
     pred = PosePredictor(model, flip_test=False)
     a, b = _images(2, 1), _images(2, 2)

@@ -203,7 +203,7 @@ def test_two_runs_write_the_same_bytes(dev, tmp_path):
 @pytest.fixture(scope="module")
 def c1(dev):
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     return _model(dev, gi.SIZE_CASES["c1"], "f16x3", train=False)         # R50, J 16, 256x256
 
 

@@ -322,7 +322,7 @@ def test_refined_pose_predictor(dev, tmp_path):
     from refiner.model import Refiner
     from lib.core.inference import PosePredictor, RefinedPosePredictor
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     c = gi.SIZE_CASES["c1"]
     model = _model(dev, c, "f16x3", train=False)
     HW = c["HW"]

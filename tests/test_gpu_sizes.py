@@ -18,8 +18,9 @@ import numpy as np
 import pytest
 import torch
 
-from oracle import restate, restate_net
+from oracle import restate
 from tests import golden_inputs as gi
+from tests.golden_inputs import _check_output, _model, _ring_meta
 from tests.conftest import relerr
 
 pytestmark = pytest.mark.gpu
@@ -31,35 +32,6 @@ def dev():
     from epipolarpose_b200 import ops
     ops.device_check()
     return torch.device("cuda:0")
-
-
-def _model(dev, c, precision, train):
-    import lib.models as models
-    from tools.bench_cfg import make_cfg
-    cfg = make_cfg(num_layers=c["layers"], num_joints=c["J"], volume=True, depth_res=c["D"],
-                   image_size=(c["HW"], c["HW"]))
-    model = models.pose3d_resnet.get_pose_net(cfg, False, precision=precision)
-    shapes = restate_net.param_shapes(num_layers=c["layers"], num_joints=c["J"], volume=True,
-                                      depth_res=c["D"])
-    model.load_state_dict(restate_net.init_state(shapes, c["seed"]))
-    model = model.to(dev)
-    return model.train() if train else model.eval()
-
-
-def _check_output(out, g, tol=1e-3):
-    """Heat-maps against the unmodified reference (north_star: <= 1e-3 rel)."""
-    o = out.detach().cpu().numpy()
-    s = gi.sample_output(o)
-    mx = float(g["ref/out_max"])
-    e = float(np.max(np.abs(s["out_sample"] - g["ref/out_sample"])) / mx)
-    e64 = float(np.max(np.abs(s["out_sample"] - g["f64/out_sample"])) / mx)
-    r64 = float(np.max(np.abs(g["ref/out_sample"] - g["f64/out_sample"])) / mx)
-    # per-(image, channel) sums over the map: error relative to the summed magnitudes
-    es = float(np.max(np.abs(s["out_chan_sum"] - g["ref/out_chan_sum"]) / (g["ref/out_chan_abs"] + 1e-30)))
-    print("heat-maps: vs reference %.2e (channel sums %.2e); vs float64 %.2e (the reference's own "
-          "float32 run: %.2e)" % (e, es, e64, r64))
-    assert e <= tol and es <= tol
-    assert abs(float(s["out_max"]) - mx) <= tol * mx
 
 
 def _check_gradients(model, g, head_keys):
@@ -127,23 +99,6 @@ def test_c2_train_slice_vs_reference(golden, dev, precision):
     sd = model.state_dict()
     assert relerr(sd["bn1.running_mean"].cpu().numpy(), g["ref/bn1.running_mean"]) <= 1e-4
     assert relerr(sd["bn1.running_var"].cpu().numpy(), g["ref/bn1.running_var"]) <= 1e-4
-
-
-def _ring_meta(tuples, seed):
-    """Cameras / boxes of the bench workload (SURVEY 8(d) C3): batch laid out
-    [view0 | view3 | view1 | view2] of every tuple so the half-split pairs (0,1) and (3,2)."""
-    from lib.dataset.synthetic import ring_camera
-    rng = np.random.default_rng(seed)
-    n_img = tuples * 4
-    order = [(t, 0) for t in range(tuples)] + [(t, 3) for t in range(tuples)] + \
-            [(t, 1) for t in range(tuples)] + [(t, 2) for t in range(tuples)]
-    cams = {(t, v): ring_camera(rng, v) for t in range(tuples) for v in range(4)}
-    return {"center_x": 500 + rng.uniform(-50, 50, n_img), "center_y": 500 + rng.uniform(-50, 50, n_img),
-            "width": 800 + rng.uniform(-100, 100, n_img), "height": 800 + rng.uniform(-100, 100, n_img),
-            "scale": np.ones(n_img), "rot": np.zeros(n_img),
-            "R": np.stack([cams[o][0] for o in order]), "T": np.stack([cams[o][1] for o in order]),
-            "f": np.stack([cams[o][2] for o in order]), "c": np.stack([cams[o][3] for o in order]),
-            "projection_matrix": np.stack([cams[o][4] for o in order])}
 
 
 @pytest.mark.parametrize("precision", ["f16x3"])

@@ -11,10 +11,9 @@ import torch
 
 from tests import emul_ops as em
 from tests.conftest import relerr
+from tests.step_cases import C4_LAYERS_SPLIT16, H16, _check_conv16_layer, _rand_split, _weights_split
 
 pytestmark = pytest.mark.gpu
-
-H16 = torch.float16
 
 
 @pytest.fixture(scope="module")
@@ -22,28 +21,6 @@ def dev():
     from epipolarpose_b200 import ops
     ops.device_check()
     return torch.device("cuda:0")
-
-
-def _rand_split(shape, seed, scale=16.0, relu=True, mag=1.0):
-    g = torch.Generator().manual_seed(seed)
-    v = torch.randn(shape, generator=g) * mag
-    if relu:
-        v = torch.relu(v)
-    if scale is None:
-        scale = em._pow2_scale(float(v.abs().max()))
-    t = torch.empty((2,) + tuple(shape), dtype=H16)
-    em._store_split(t, v, scale)
-    sc = torch.tensor([scale, 1.0 / scale])
-    return t, sc
-
-
-def _weights_split(cout, K, seed):
-    g = torch.Generator().manual_seed(seed)
-    w = torch.randn(cout * K, generator=g) * (2.0 / K) ** 0.5
-    h = torch.empty(2 * cout * K, dtype=H16)
-    sc = torch.ones(2)
-    em.split16_batch(em.SplitBatch([(w, h, sc)]))
-    return h, sc
 
 
 def _conv_cases():
@@ -399,87 +376,8 @@ def test_bn_bwd_fused_entry_vs_emulation_and_deterministic(dev, M, C, mode):
 
 
 # ------------------------------------------------------------------ the bench's own layer shapes
-# (profiles/r2_step_table_f16x3.md): N = 128 images, every distinct conv kind / channel pair of
-# ResNet-50 at 256x256.  Reference: torch float64 convolutions (cuDNN / cuBLAS fp64 on the same
-# device -- none of this repo's code) of the EXACT values the fp16 planes hold.
-C4_LAYERS = [
-    ("l1_1x1_64_256", "conv", 64, 256, 1, 1, 0, 64), ("l1_1x1_256_64", "conv", 256, 64, 1, 1, 0, 64),
-    ("l1_3x3_64", "conv", 64, 64, 3, 1, 1, 64), ("l2_3x3_s2", "conv", 128, 128, 3, 2, 1, 64),
-    ("l2_1x1_s2_down", "conv", 256, 512, 1, 2, 0, 64), ("l3_3x3_256", "conv", 256, 256, 3, 1, 1, 16),
-    ("l3_1x1_1024_256", "conv", 1024, 256, 1, 1, 0, 16), ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 8),
-    ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 8), ("deconv0", "deconv", 2048, 256, 4, 2, 1, 8),
-    ("deconv2", "deconv", 256, 256, 4, 2, 1, 32), ("final", "conv", 256, 1024, 1, 1, 0, 64),
-]
-
-
-@pytest.mark.parametrize("layer", C4_LAYERS, ids=[c[0] for c in C4_LAYERS])
+# step_cases.C4_LAYERS_SPLIT16; reference: torch float64 convolutions (cuDNN / cuBLAS fp64 on the
+# same device -- none of this repo's code) of the EXACT values the fp16 planes hold.
+@pytest.mark.parametrize("layer", C4_LAYERS_SPLIT16, ids=[c[0] for c in C4_LAYERS_SPLIT16])
 def test_conv16_bench_layer_shapes_vs_torch_float64(dev, layer):
     _check_conv16_layer(dev, layer, 128, 2e-4)
-
-
-def _check_conv16_layer(dev, layer, N, wgrad_bar):
-    """conv16 fprop (with statistics), dgrad and wgrad of one layer over N images against torch
-    float64 on the values the planes hold; returns the three errors"""
-    import torch.nn.functional as F
-    from epipolarpose_b200 import net, ops
-    name, kind, cin, cout, k, s, p, hw = layer
-    conv = net.Conv("t", kind, cin, cout, k, s, p, 0)
-    Ho, Wo = conv.out_hw(hw, hw)
-    T = k * k
-    g = torch.Generator(device=dev).manual_seed(7)
-
-    def split_dev(v):
-        h = torch.empty(2 * v.numel(), device=dev, dtype=H16)
-        sc = torch.ones(2, device=dev)
-        ops.split16_batch(ops.SplitBatch([(v.reshape(-1), h, sc)]))
-        val = ((h[:v.numel()].double() + h[v.numel():].double()) * float(sc[1])).view(v.shape)
-        return h.view((2,) + tuple(v.shape)), sc, val
-
-    x, x_sc, xv = split_dev(torch.relu(torch.randn(N, hw, hw, cin, device=dev, generator=g)))
-    dz, dz_sc, dzv = split_dev(torch.randn(N, Ho, Wo, cout, device=dev, generator=g) * 3e-5)
-    w = torch.randn((cout, cin, k, k) if kind == "conv" else (cin, cout, k, k), device=dev,
-                    generator=g) * (2.0 / (T * cin)) ** 0.5
-    wf32, wd32 = conv.pack(ops, w)
-    wf, wf_sc, wfv = split_dev(wf32)
-    wd, wd_sc, _ = split_dev(wd32)
-    # the weights the planes hold, back in the state_dict layout (for the float64 reference)
-    pk = wfv.view(cout, T, cin)
-    wq64 = pk.permute(0, 2, 1).reshape(cout, cin, k, k) if kind == "conv" else \
-        pk.permute(2, 0, 1).reshape(cin, cout, k, k)
-    xa = xv.permute(0, 3, 1, 2).contiguous().requires_grad_(True)
-    wt = wq64.contiguous().requires_grad_(True)
-    ref = F.conv2d(xa, wt, None, s, p) if kind == "conv" else F.conv_transpose2d(xa, wt, None, s, p)
-    ref.backward(dzv.permute(0, 3, 1, 2).contiguous())
-    # fprop
-    out = torch.zeros(N, Ho, Wo, cout, device=dev)
-    stats = torch.zeros(2 * cout, device=dev, dtype=torch.float64)
-    for gm in conv.fprop_geoms(ops, N, hw, hw, 3):
-        if gm is not None:
-            gm.in_relu, gm.accumulate = 0, 0
-            ops.conv16_fprop(gm, x, x_sc, wf, wf_sc, out, None, stats)
-    r = ref.detach().permute(0, 2, 3, 1)
-    e_f = e = float((out.double() - r).abs().max() / r.abs().max())
-    assert e <= 5e-5, "fprop %.3e" % e
-    # per-channel sums: fp32 partial sums over up to 3584 rows per CTA, then float64 atomics
-    assert float((stats[:cout] - r.sum((0, 1, 2))).abs().max() / r.abs().sum((0, 1, 2)).max()) <= 5e-5
-    # dgrad: only the dz * w_dgrad-operand product differs from the reference by the weight planes
-    din = torch.zeros(N, hw, hw, cin, device=dev)
-    for gm in conv.dgrad_geoms(ops, N, hw, hw, 3):
-        if gm is not None:
-            gm.in_relu, gm.accumulate = 0, 0
-            ops.conv16_fprop(gm, dz, dz_sc, wd, wd_sc, din, None, None)
-    r = xa.grad.permute(0, 2, 3, 1)
-    e_d = e = float((din.double() - r).abs().max() / r.abs().max())
-    assert e <= 5e-5, "dgrad %.3e" % e
-    # wgrad (packed [cout][T][cin])
-    dw = torch.zeros(cout * T * cin, device=dev)
-    ws = torch.empty(48 << 20, device=dev)
-    for gm in conv.fprop_geoms(ops, N, hw, hw, 3):
-        if gm is not None:
-            gm.in_relu, gm.accumulate = 0, 0
-            ops.conv16_wgrad(gm, x, x_sc, dz, dz_sc, dw, ws)
-    gw = wt.grad
-    r = (gw.permute(0, 2, 3, 1) if kind == "conv" else gw.permute(1, 2, 3, 0)).reshape(cout, T, cin)
-    e = float((dw.view(cout, T, cin).double() - r).abs().max() / r.abs().max())
-    assert e <= wgrad_bar, "wgrad %.3e (bar %.2e)" % (e, wgrad_bar)   # C4: fp32 runs over up to 524288 / 74 pixels
-    return e_f, e_d, e

@@ -12,13 +12,8 @@ fprop / dgrad <= 2e-5, wgrad <= 3e-5 (max|d| / max|ref|).  A 3xTF32 product with
 correction pass lost, or a single pass that truncates instead of rounding, is ~1e-4 .. 1e-3
 off (test_tf32_emulation_bars_have_teeth shows it on the CPU).
 
-The H100's wgmma adds into its fp32 accumulator rounding toward zero, so that noise floor
-grows linearly with the number of k-steps x passes instead of as its square root.  Measured on
-one H100 80GB HBM3 at a 700 W power limit: 3.6e-5 .. 4.0e-5 for 3xTF32 and 1.2e-5 for TF32 at
-K = 4608 (3x3, 512 channels), ~7e-9 per 3xTF32 k-element; a round-toward-zero emulation of the
-same product gives the same numbers.  The tensor-core output bar is therefore
-max(2e-5, 0.75 * 2^-24 * passes * K / 8) (`_tc_bar`): 7.7e-5 for 3xTF32 at K = 4608, where a
-lost correction pass is still ~2e-4 off.
+The H100's wgmma adds into its fp32 accumulator rounding toward zero, so the tensor-core output
+bar grows with K: `step_cases._tc_bar` (its docstring has the measurement).
 
 The shapes reach what the small shapes of test_gpu_parity.py cannot: more tiles than SMs (the
 persistent tile loop, the producers' flat k-block stream across tiles, ring phase wrap over
@@ -26,31 +21,17 @@ tiles), N tails of both tile widths, odd channel-block counts, Cin > 256 on 3x3 
 phase-grid tap count of the transposed convolutions, and the wgrad ci / co tile tails and
 slot-group splits.  Each case names the kernel instantiation it is meant to reach and checks,
 from the profiler's kernel names, that it ran."""
-import re
-
 import numpy as np
 import pytest
 import torch
 
-gpu = pytest.mark.gpu
+from tests.step_cases import (FPROP_BAR, STATS_SELF_BAR, WGRAD_BAR, _act64, _emul_mma, _fwd64, _geoms, _guarded,
+                              _layer, _ran, _tc_bar, _tf32_np, _trunc_np)
 
-FPROP_BAR = 2e-5       # fprop / dgrad output (and BatchNorm sums) against float64
-WGRAD_BAR = 3e-5       # weight gradient: pixel reductions split over CTAs (red.add)
-STATS_SELF_BAR = 1e-6  # BatchNorm sums against float64 sums of the kernel's own output
+gpu = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------ operand rounding
-def _tf32_np(x):
-    """round to nearest TF32, ties away from zero (tc::to_tf32), in an fp32 container"""
-    u = np.asarray(x, dtype=np.float32).view(np.uint32)
-    return ((u + np.uint32(0x1000)) & np.uint32(0xffffe000)).view(np.float32)
-
-
-def _trunc_np(x):
-    """TF32 by truncation: what the tensor core reads from an fp32 container"""
-    return (np.asarray(x, dtype=np.float32).view(np.uint32) & np.uint32(0xffffe000)).view(np.float32)
-
-
 def _tf32(t):
     """_tf32_np for a float32 torch tensor (int32 wrap-around == the unsigned add)"""
     return ((t.contiguous().view(torch.int32) + 0x1000) & -8192).view(torch.float32)
@@ -61,34 +42,7 @@ def _relerr(a, ref):
     return float((a - ref).abs().max() / ref.abs().max().clamp_min(1e-300))
 
 
-def _tc_bar(base, K, passes):
-    """Output bar of a tensor-core product over K: `base`, or the round-toward-zero accumulation
-    floor of passes * K / 8 wgmma k-steps (module docstring) where that is larger."""
-    return max(base, 0.75 * 2.0 ** -24 * passes * K / 8)
-
-
 # ------------------------------------------------------------------ CPU: the bars have teeth
-def _rz32(x):
-    """float64 -> fp32 rounded toward zero"""
-    f = x.astype(np.float32)
-    over = np.abs(f.astype(np.float64)) > np.abs(x)
-    f[over] = np.nextafter(f[over], np.float32(0))
-    return f
-
-
-def _emul_mma(passes, K, toward_zero=False):
-    """The tensor-core product of the kernels: per k-step of 8, each pass (a, b) adds the exact
-    8-term dot products to the fp32 accumulator, in the order given; the add rounds to nearest,
-    or toward zero as the H100's wgmma does."""
-    M, N = passes[0][0].shape[0], passes[0][1].shape[1]
-    acc = np.zeros((M, N), np.float32)
-    for k0 in range(0, K, 8):
-        for a, b in passes:
-            part = a[:, k0:k0 + 8].astype(np.float64) @ b[k0:k0 + 8].astype(np.float64)
-            acc = _rz32(acc + part) if toward_zero else acc + part.astype(np.float32)
-    return acc
-
-
 def test_tf32_emulation_bars_have_teeth():
     """At a 3x3 x 64-channel layer's K = 576: the emulated 3xTF32 product (RN hi, truncated lo,
     the mma3_tf32 pass order) and the single-pass TF32 product meet the fprop bar; dropping the
@@ -145,34 +99,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-_KNAME = re.compile(r"conv_(fprop|wgrad)_(?:tc_kernel(?:<(\d+), ?(\d+)>|ILi(\d+)ELi(\d+)E)|(simt))")
-
-
-def _ran(fn):
-    """Runs fn under torch.profiler; returns the conv kernels that ran, as 'fprop_tc<128,3>',
-    'wgrad_simt', ...  fn writes scratch buffers only: a short profiling session now and then
-    delivers no device activity at all, and is then repeated (up to eight sessions).  Each
-    session starts on an idle device and stays open a few milliseconds after fn's kernels have
-    finished, so that their activity records are inside its window when it stops."""
-    import time
-    from torch.profiler import ProfilerActivity, profile
-    tags = set()
-    for _ in range(8):
-        torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            fn()
-            torch.cuda.synchronize()
-            time.sleep(0.005)
-        for ev in prof.events():
-            m = _KNAME.search(ev.name)
-            if m:
-                kind, a, b, c, d, simt = m.groups()
-                tags.add("%s_simt" % kind if simt else "%s_tc<%s,%s>" % (kind, a or c, b or d))
-        if tags:
-            break
-    return tags
-
-
 def _expect(kind, which, precision):
     """which: 'tc64' / 'tc128' / 'tc32' or 'simt' -> the kernel tag _ran reports"""
     if which == "simt" or precision == 0:
@@ -191,64 +117,6 @@ def _out_bar(geoms, which, precision):
         return FPROP_BAR
     K = max(gm.T * gm.Cin for gm in geoms if gm is not None)
     return _tc_bar(FPROP_BAR, K, 3 if precision == 3 else 1)
-
-
-def _layer(dev, kind, cin, cout, k, s, p, opad, N, H, W, seed):
-    """Random layer at the padded channel counts the engine uses: NHWC input x, BatchNorm affine
-    (sc, sh) of the producing layer, weights in the state_dict layout with the padding rows /
-    columns zero, and the upstream gradient of the output."""
-    from epipolarpose_b200 import net
-    conv = net.Conv("t", kind, cin, cout, k, s, p, opad)
-    Ho, Wo = conv.out_hw(H, W)
-    g = torch.Generator(device=dev).manual_seed(seed)
-    ci, co = conv.cin_p, conv.cout_p
-    x = torch.randn(N, H, W, ci, device=dev, generator=g)
-    sc = torch.rand(ci, device=dev, generator=g) + 0.5
-    sh = torch.randn(ci, device=dev, generator=g) * 0.1
-    w = torch.randn((co, ci, k, k) if kind == "conv" else (ci, co, k, k), device=dev, generator=g)
-    w *= (2.0 / (k * k * cin)) ** 0.5
-    if kind == "conv":
-        w[cout:], w[:, cin:] = 0, 0
-    else:
-        w[cin:], w[:, cout:] = 0, 0
-    gout = torch.randn(N, Ho, Wo, co, device=dev, generator=g)
-    gout[..., cout:] = 0
-    return conv, Ho, Wo, x, sc, sh, w.contiguous(), gout
-
-
-def _act64(x, sc, sh, relu):
-    """f(x) = max(fma(x, sc, sh), lb) exactly as the producers compute it (one fp32 rounding), as
-    float64 NCHW; affine None -> x itself"""
-    if sc is None:
-        f = x
-    else:
-        f = (x.double() * sc.double() + sh.double()).float()
-        if relu:
-            f = torch.relu(f)
-    return f.permute(0, 3, 1, 2).double()
-
-
-def _fwd64(conv, a, w):
-    import torch.nn.functional as F
-    if conv.kind == "conv":
-        return F.conv2d(a, w, None, conv.stride, conv.pad)
-    return F.conv_transpose2d(a, w, None, conv.stride, conv.pad, conv.opad)
-
-
-def _guarded(shape, dev, fill):
-    """A tensor followed by a 64-float guard band that must stay untouched."""
-    n = int(np.prod(shape))
-    buf = torch.full((n + 64,), fill, device=dev)
-    return buf[:n].view(shape), buf[n:]
-
-
-def _geoms(geoms, relu=0, acc=0):
-    out = []
-    for gm in geoms:
-        if gm is not None:
-            gm.in_relu, gm.accumulate = relu, acc
-            out.append(gm)
-    return out
 
 
 def _report(what, tags, **errs):

@@ -1,16 +1,15 @@
 """The tf32x3 training step (net.Engine at precision 3: the 3xTF32 wgmma convolutions and the fp32
 bn.cu BatchNorm chain; MODEL.PRECISION's default, bench.py --precision tf32x3, and the engine
 get_pose_net falls back to for plans net16 refuses) against float64 kernel by kernel at the bench's
-sizes (R50, J = 16, D = 64, 256 x 256, N = 128: 32 tuples x 4 views), and a coverage gate: every
-C-ABI entry one tf32x3 step calls must name the tests that hold it to float64 at those sizes
-(COVERAGE_TF32X3).
+sizes (R50, J = 16, D = 64, 256 x 256, N = 128: 32 tuples x 4 views).  tests/test_step_coverage.py
+gates the tf32x3 step on these tests.
 
 Every reference is torch float64 on the device, computed from the exact fp32 values the kernel
 read, in image or row chunks where memory needs it.  Bars (u = 2^-24):
 
   * Convolutions (fprop, dgrad, wgrad at every distinct R50 conv of the step, with the step's
-    operand modes): the bars of test_gpu_tf32.  fprop / dgrad: _tc_bar(FPROP_BAR, K, 3), K the
-    longest taps x Cin of the call's geometries; wgrad: _tc_bar(WGRAD_BAR, R, 3), R the pixel
+    operand modes: step_cases.C4_LAYERS_TF32X3): the bars of test_gpu_tf32.  fprop / dgrad:
+    _tc_bar(FPROP_BAR, K, 3), K the longest taps x Cin of the call's geometries; wgrad: _tc_bar(WGRAD_BAR, R, 3), R the pixel
     run of one CTA from the TF32 wgrad planner (`_tf32_wgrad_plan` over each geometry's
     N Hp Wp pixels), since wgmma accumulates toward zero.  Statistics: STATS_SELF_BAR against
     the float64 sums of the kernel's own output, the fprop bar against the reference's sums.
@@ -34,109 +33,30 @@ read, in image or row chunks where memory needs it.  Bars (u = 2^-24):
     order) must give y and argidx bit for bit, and y is within one rounding, u y64, of the
     float64 pool (the maximum is 1-Lipschitz).
   * add_masked, im2col, nchw_to_nhwc: data movement and one fp32 add, bit-exact with torch.
-  * Soft-argmax backward (fp32 NHWC) and colsum at C4's shape: the bars of test_gpu_c5_step.
+  * Soft-argmax backward (fp32 NHWC) and colsum at C4's shape: step_cases._sabwd_ref_bar and
+    _check_colsum.
 
-CPU tests below run the gate through the emulated ABI and show against numpy emulations of the
-kernels' arithmetic that each new bar holds for the kernel's order and rejects a plausible
+CPU tests below show against numpy emulations of the kernels' arithmetic that each new bar holds for the kernel's order and rejects a plausible
 mistake: M - 1 in k1 / k2, a reduce that ignores y_out, a reduce that drops the last partial CTA,
 bn_act without the residual's affine, a pool that keeps the last maximum or skips the ReLU, and a
 3xTF32 wgrad that loses a correction pass at the longest C4 run."""
-import math
-import re
-
 import numpy as np
 import pytest
 import torch
 
-from tests.test_gpu_c5_step import (KPIX, RUN_BLOCKS3, _check_colsum, _check_softargmax_bwd_fp32,
-                                    _tf32_wgrad_plan)
-from tests.test_gpu_step_kernels import _bench_meta, _cfg, _entry_names, _missing_coverage, _record_calls
-from tests.test_gpu_tf32 import (FPROP_BAR, STATS_SELF_BAR, WGRAD_BAR, _act64, _emul_mma, _fwd64, _geoms,
-                                 _guarded, _layer, _ran, _tc_bar, _tf32_np, _trunc_np)
+from tests import step_cases as sc
+from tests.step_cases import (C4_LAYERS_TF32X3, EPS, FPROP_BAR, KPIX, RUN_BLOCKS3, STATS_SELF_BAR, U, WGRAD_BAR,
+                              _act64, _all_three_pass, _emul_mma, _fwd64, _geoms, _guarded, _layer, _ran, _tc_bar,
+                              _tf32_np, _tf32_wgrad_plan, _trunc_np)
 
 gpu = pytest.mark.gpu
 
-U = 2.0 ** -24
-EPS = 1e-5
 NB, HWB, JB, DB, HMB = 128, 256, 16, 64, 64      # one GPU's bench batch: 32 tuples x 4 views
 ROWS_PER_THREAD = 64                             # bn.cu kRowsPerThread
 
-S = "test_gpu_tf32x3_step.py::"
-SK = "test_gpu_step_kernels.py::"
-COVERAGE_TF32X3 = {
-    "epb_nchw_to_nhwc": [S + "test_tf32x3_nchw_to_nhwc_bit_exact"],
-    "epb_im2col": [S + "test_tf32x3_im2col_bit_exact_at_stem"],
-    "epb_conv_fprop": [S + "test_tf32x3_conv_layers_vs_float64"],
-    "epb_conv_wgrad": [S + "test_tf32x3_conv_layers_vs_float64", S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
-    "epb_bn_finalize": [S + "test_tf32x3_bn_finalize_vs_float64", SK + "test_bn_finalize_vs_float64_at_bench_M"],
-    "epb_bn_relu_maxpool": [S + "test_tf32x3_bn_relu_maxpool_vs_float64"],
-    "epb_bn_act": [S + "test_tf32x3_bn_act_vs_float64"],
-    "epb_bn_bwd_reduce": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
-    "epb_bn_bwd_apply": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
-    "epb_add_masked": [S + "test_tf32x3_add_masked_bit_exact"],
-    "epb_maxpool_bwd": [SK + "test_maxpool_bwd_vs_float64_at_stem_bench_size"],
-    "epb_softargmax_fwd": [SK + "test_softargmax_fwd_vs_float64_at_bench_shape"],
-    "epb_softargmax_bwd": [S + "test_tf32x3_softargmax_bwd_fp32_vs_float64"],
-    "epb_colsum": [S + "test_tf32x3_colsum_vs_float64"],
-    "epb_jointloss_fwd_bwd": [SK + "test_jointloss_vs_float64_at_bench_shape"],
-    "epb_pack_weight_batch": [S + "test_tf32x3_pack_weight_batch_bit_exact_on_model_jobs",
-                              S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
-    "epb_adam_step_dev": [S + "test_tf32x3_fused_adam_vs_float64_on_model_buffer"],
-    "epb_patch_to_image": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
-    "epb_triangulate": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
-    "epb_project_labels": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
-}
-# the fp32 engine's own entries: the f16x3 step calls none of them
-FP32_ENGINE = {"epb_nchw_to_nhwc", "epb_im2col", "epb_conv_fprop", "epb_conv_wgrad", "epb_bn_finalize",
-               "epb_bn_relu_maxpool", "epb_bn_act", "epb_bn_bwd_reduce", "epb_bn_bwd_apply", "epb_add_masked",
-               "epb_softargmax_bwd", "epb_colsum"}
-_THREE_PASS = re.compile(r"^(fprop|wgrad)_tc<\d+,3>$")
-
-
-def _all_three_pass(tags):
-    """every conv kernel tag _ran reported is a 3xTF32 tensor-core instantiation"""
-    return bool(tags) and all(_THREE_PASS.match(t) for t in tags)
-
-
-# every distinct conv of R50 at 256 x 256 (trunk at 64 / 32 / 16 / 8, deconvs 8 -> 64, the final
-# 1 x 1 with bias), the stem as a 1 x 1 conv over its 160-column patch matrix; (name, kind, cin,
-# cout, k, stride, pad, input hw, operand, dgrad).  operand "in": a materialised tensor (patch
-# matrix, pool or block output); "act": the producer's BatchNorm + ReLU applied on load.
-# dgrad "write", "acc" (a downsample adds into the block's input gradient) or None (the stem).
-C4_LAYERS = [
-    ("stem_col_160_64", "conv", 160, 64, 1, 1, 0, 128, "in", None),
-    ("l1_1x1_64_64", "conv", 64, 64, 1, 1, 0, 64, "in", "write"),
-    ("l1_3x3_64", "conv", 64, 64, 3, 1, 1, 64, "act", "write"),
-    ("l1_1x1_64_256", "conv", 64, 256, 1, 1, 0, 64, "act", "write"),
-    ("l1_down_64_256", "conv", 64, 256, 1, 1, 0, 64, "in", "acc"),
-    ("l1_1x1_256_64", "conv", 256, 64, 1, 1, 0, 64, "in", "write"),
-    ("l2_1x1_256_128", "conv", 256, 128, 1, 1, 0, 64, "in", "write"),
-    ("l2_3x3_s2_128", "conv", 128, 128, 3, 2, 1, 64, "act", "write"),
-    ("l2_1x1_128_512", "conv", 128, 512, 1, 1, 0, 32, "act", "write"),
-    ("l2_down_s2_256_512", "conv", 256, 512, 1, 2, 0, 64, "in", "acc"),
-    ("l2_1x1_512_128", "conv", 512, 128, 1, 1, 0, 32, "in", "write"),
-    ("l2_3x3_128", "conv", 128, 128, 3, 1, 1, 32, "act", "write"),
-    ("l3_1x1_512_256", "conv", 512, 256, 1, 1, 0, 32, "in", "write"),
-    ("l3_3x3_s2_256", "conv", 256, 256, 3, 2, 1, 32, "act", "write"),
-    ("l3_1x1_256_1024", "conv", 256, 1024, 1, 1, 0, 16, "act", "write"),
-    ("l3_down_s2_512_1024", "conv", 512, 1024, 1, 2, 0, 32, "in", "acc"),
-    ("l3_1x1_1024_256", "conv", 1024, 256, 1, 1, 0, 16, "in", "write"),
-    ("l3_3x3_256", "conv", 256, 256, 3, 1, 1, 16, "act", "write"),
-    ("l4_1x1_1024_512", "conv", 1024, 512, 1, 1, 0, 16, "in", "write"),
-    ("l4_3x3_s2_512", "conv", 512, 512, 3, 2, 1, 16, "act", "write"),
-    ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 8, "act", "write"),
-    ("l4_down_s2_1024_2048", "conv", 1024, 2048, 1, 2, 0, 16, "in", "acc"),
-    ("l4_1x1_2048_512", "conv", 2048, 512, 1, 1, 0, 8, "in", "write"),
-    ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 8, "act", "write"),
-    ("deconv0_2048_256", "deconv", 2048, 256, 4, 2, 1, 8, "in", "write"),
-    ("deconv1_256", "deconv", 256, 256, 4, 2, 1, 16, "act", "write"),
-    ("deconv2_256", "deconv", 256, 256, 4, 2, 1, 32, "act", "write"),
-    ("final_256_1024", "conv", 256, JB * DB, 1, 1, 0, 64, "act", "write"),
-]
-
 
 def _wgrad_runs(layer, N=NB):
-    """(pixels N Hp Wp, Cin, Cout, taps) of each wgrad geometry of a C4_LAYERS row: one for a
+    """(pixels N Hp Wp, Cin, Cout, taps) of each wgrad geometry of a C4_LAYERS_TF32X3 row: one for a
     convolution, one per output phase (2 x 2, 4 taps each) for the 4 x 4 / 2 deconvolutions"""
     _, kind, cin, cout, k, s, p, hw, _, _ = layer
     if kind == "conv":
@@ -150,82 +70,10 @@ def _wgrad_run(layer):
     return max(_tf32_wgrad_plan(M, ci, co, T, 3)[0] for M, ci, co, T in _wgrad_runs(layer))
 
 
-# ------------------------------------------------------------------ coverage gate, CPU
-def test_coverage_tf32x3_gate_has_teeth():
-    """Deleting any row, or pointing one at a test that does not exist, fails the gate; the kernel
-    tag check rejects a single-pass or CUDA-core conv among three-pass ones."""
-    rec = sorted(COVERAGE_TF32X3)
-    assert _missing_coverage(rec, COVERAGE_TF32X3) == ([], [])
-    for k in rec:
-        t = dict(COVERAGE_TF32X3)
-        del t[k]
-        assert _missing_coverage(rec, t)[0] == [k]
-    for k in rec:
-        t = dict(COVERAGE_TF32X3)
-        t[k] = [S + "test_no_such_test"]
-        assert _missing_coverage(rec, t)[1]
-    good = {"fprop_tc<64,3>", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
-    assert _all_three_pass(good)
-    for bad in ("fprop_tc<128,1>", "wgrad_tc<64,1>", "wgrad_simt", "fprop_simt"):
-        assert not _all_three_pass(good | {bad})
-    assert not _all_three_pass(set())
-
-
-def test_coverage_tf32x3_gate_cpu_emulated_step():
-    """One tf32x3 training step (R18, J = 16, D = 64, 2 tuples x 4 views of 64 x 64) through the
-    emulated ABI: GraphedTrainStep.eager_step, SmoothL1JointLocationLoss, FusedAdam, given labels
-    (no CPU geometry).  The model runs net.Engine at precision 3 and the step records the fp32
-    engine's entries; every entry has a row."""
-    import lib.models as models
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    import lib.utils.utils as Ut
-    from epipolarpose_b200 import net, ops
-    from tests import emul_ops
-    rec, depth, saved = set(), [0], {}
-    for k, e in _entry_names(ops).items():
-        if not hasattr(emul_ops, k):
-            continue
-        f = saved[k] = getattr(emul_ops, k)
-
-        def wrap(*a, _f=f, _e=e, **kw):
-            if depth[0] == 0:
-                rec.update(_e)
-            depth[0] += 1
-            try:
-                return _f(*a, **kw)
-            finally:
-                depth[0] -= 1
-        setattr(emul_ops, k, wrap)
-    il._backend[0], Ut._backend[0] = emul_ops, emul_ops
-    try:
-        J, D, HW, B = JB, DB, 64, 8
-        torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(_cfg(18, J, D, HW), False, ops=emul_ops, precision="tf32x3").train()
-        eng = m._engine()
-        assert type(eng) is net.Engine and eng.precision == 3 and eng.wgrad_precision == 3
-        opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-        step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
-        g = torch.Generator().manual_seed(1)
-        loss = step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
-                               torch.ones(B, J * 3), None)
-        assert math.isfinite(float(loss))
-    finally:
-        for k, f in saved.items():
-            setattr(emul_ops, k, f)
-        il._backend[0] = Ut._backend[0] = ops
-    print("emulated tf32x3 step calls: %s" % sorted(rec))
-    assert FP32_ENGINE <= rec, sorted(FP32_ENGINE - rec)
-    assert not any(e.endswith("_split") or "conv16" in e for e in rec), sorted(rec)
-    missing, dangling = _missing_coverage(rec, COVERAGE_TF32X3)
-    assert not missing, "entries without a float64 test at bench size: %s" % missing
-    assert not dangling, dangling
-
-
 def test_c4_layer_table_wgrad_runs():
-    """The restated planner over C4_LAYERS at N = 128: every run within the three-pass cap, and
+    """The restated planner over C4_LAYERS_TF32X3 at N = 128: every run within the three-pass cap, and
     the bar of the longest run under 1e-4."""
-    runs = [(c[0], _wgrad_run(c)) for c in C4_LAYERS]
+    runs = [(c[0], _wgrad_run(c)) for c in C4_LAYERS_TF32X3]
     for name, r in runs:
         assert 0 < r <= RUN_BLOCKS3 * KPIX and r % KPIX == 0, (name, r)
     R = max(r for _, r in runs)
@@ -492,10 +340,10 @@ def test_pool_restatement_rejects_the_last_maximum_and_a_missing_relu():
 
 
 def test_tf32_wgrad_bar_rejects_a_lost_correction_pass_at_the_longest_c4_run():
-    """The wgrad product at the longest pixel run of C4_LAYERS (R from the planner), with the
+    """The wgrad product at the longest pixel run of C4_LAYERS_TF32X3 (R from the planner), with the
     toward-zero accumulation of test_gpu_tf32: 3xTF32 meets _tc_bar(WGRAD_BAR, R, 3); dropping
     the dout lo pass or the activation lo pass misses it."""
-    R = max(_wgrad_run(c) for c in C4_LAYERS)
+    R = max(_wgrad_run(c) for c in C4_LAYERS_TF32X3)
     rng = np.random.default_rng(17)
     co, ci = 128, 64
     a = (rng.standard_normal((co, R)) * 1e-3).astype(np.float32)         # dz^T
@@ -521,9 +369,6 @@ def dev():
     return torch.device("cuda:0")
 
 
-_MODEL = {}
-
-
 @pytest.fixture(scope="module", autouse=True)
 def _release_device_memory():
     """After the module, drop its cached model and hand the allocator's reserve back to the
@@ -531,69 +376,23 @@ def _release_device_memory():
     if torch.cuda.is_available() and torch.cuda.is_initialized():
         torch.cuda.reset_peak_memory_stats()
     yield
-    _MODEL.clear()
+    sc.release("c4_tf32x3")
     if torch.cuda.is_initialized():
-        import gc
-        gc.collect()
         print("\n  tf32x3 step module: peak device allocation %.1f GB" % (torch.cuda.max_memory_allocated() / 2 ** 30))
-        torch.cuda.empty_cache()
 
 
 def _r50(dev):
     """the bench model (R50, J = 16, D = 64, 256 x 256) on net.Engine at precision 3, with
     FusedAdam over its parameters"""
-    if "m" not in _MODEL:
-        import lib.models as models
-        import lib.utils.utils as Ut
-        from epipolarpose_b200 import net
-        torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(_cfg(50, JB, DB, HWB), False, precision="tf32x3").to(dev).train()
-        assert type(m._engine()) is net.Engine and m._engine().precision == 3
-        _MODEL["m"] = m
-        _MODEL["opt"] = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-    return _MODEL["m"], _MODEL["opt"]
+    from epipolarpose_b200 import net
+    m, opt = sc.bench_model(dev, "c4_tf32x3")
+    assert type(m._engine()) is net.Engine and m._engine().precision == 3
+    return m, opt
 
 
-# ------------------------------------------------------------------ 1. coverage gate, GPU half
+# ------------------------------------------------------------------ 1. convolutions at N = 128
 @gpu
-def test_coverage_tf32x3_gate_step(dev):
-    """One tf32x3 bench-composition step at a reduced batch (R50, J = 16, D = 64, 2 tuples x 4
-    views of 256 x 256): GraphedTrainStep(online=True, method="iterative").eager_step, SmoothL1,
-    FusedAdam, under the profiler.  Every entry it calls has a row in COVERAGE_TF32X3 naming
-    existing tests, and every conv kernel that ran is a three-pass instantiation."""
-    import lib.models as models
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    import lib.utils.img_utils as iu
-    import lib.utils.utils as Ut
-    tuples = 2
-    B = 4 * tuples
-    torch.manual_seed(0)
-    m = models.pose3d_resnet.get_pose_net(_cfg(50, JB, DB, HWB), False, precision="tf32x3").to(dev).train()
-    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(JB).to(dev), opt, online=True, method="iterative")
-    meta = iu.pack_meta({k: v.to(dev) for k, v in _bench_meta(tuples).items()}, B, dev)
-    x = torch.randn(B, 3, HWB, HWB, device=dev)
-    losses = []
-    with _record_calls() as names:
-        tags = _ran(lambda: losses.append(float(step.eager_step(x, None, None, meta))))
-        torch.cuda.synchronize()
-    assert losses and all(math.isfinite(v) for v in losses)
-    print("  tf32x3 step calls %d entries; conv kernels %s" % (len(names), sorted(tags)))
-    for e in sorted(names):
-        print("    %-28s -> %s" % (e, ", ".join(COVERAGE_TF32X3.get(e, ["(none)"]))))
-    assert FP32_ENGINE <= names, sorted(FP32_ENGINE - names)
-    assert "epb_adam_step_dev" in names and "epb_triangulate" in names
-    assert _all_three_pass(tags), "a conv of the tf32x3 step ran below three passes: %s" % sorted(tags)
-    assert any(t.startswith("fprop") for t in tags) and any(t.startswith("wgrad") for t in tags), tags
-    missing, dangling = _missing_coverage(names, COVERAGE_TF32X3)
-    assert not missing, "entries without a float64 test at bench size: %s" % missing
-    assert not dangling, dangling
-
-
-# ------------------------------------------------------------------ 2. convolutions at N = 128
-@gpu
-@pytest.mark.parametrize("layer", C4_LAYERS, ids=[c[0] for c in C4_LAYERS])
+@pytest.mark.parametrize("layer", C4_LAYERS_TF32X3, ids=[c[0] for c in C4_LAYERS_TF32X3])
 def test_tf32x3_conv_layers_vs_float64(dev, layer):
     """fprop (statistics into a zeroed buffer, or the bias for the final layer), dgrad (written,
     or added into the block's input gradient for a downsample) and wgrad (into a zeroed dW) at
@@ -773,7 +572,7 @@ def test_tf32x3_stem_wgrad_through_flat_buffer(dev):
     assert e_flat <= bar and e_w <= bar
 
 
-# ------------------------------------------------------------------ 3. the fp32 BatchNorm chain
+# ------------------------------------------------------------------ 2. the fp32 BatchNorm chain
 # (M, C, mask) of every BatchNorm backward of the step: "y_out" for the last BatchNorm of a block
 # and the downsample BatchNorms, "relu" for the stem, the inner BatchNorms and the deconvs'
 BN_BWD = [(2097152, 64, "relu"), (524288, 64, "relu"), (524288, 128, "relu"), (524288, 256, "y_out"),
@@ -973,36 +772,33 @@ def test_tf32x3_nchw_to_nhwc_bit_exact(dev):
 @pytest.mark.parametrize("M", [131072, 32768, 8192])
 def test_tf32x3_bn_finalize_vs_float64(dev, M):
     """bn_finalize at the step's other M (the bench test covers 524288 and 2097152)"""
-    from tests.test_gpu_step_kernels import test_bn_finalize_vs_float64_at_bench_M
-    test_bn_finalize_vs_float64_at_bench_M(dev, M)
+    sc.check_bn_finalize(dev, M)
 
 
-# ------------------------------------------------------------------ 4. the fp32 head at C4's shape
+# ------------------------------------------------------------------ 3. the fp32 head at C4's shape
 @gpu
 def test_tf32x3_softargmax_bwd_fp32_vs_float64(dev):
     """epb_softargmax_bwd (fp32 NHWC) at N = 128, J = 16, D = 64, 64 x 64"""
-    _check_softargmax_bwd_fp32(dev, NB, JB, DB, HMB, HMB)
+    sc._check_softargmax_bwd_fp32(dev, NB, JB, DB, HMB, HMB)
 
 
 @gpu
 @pytest.mark.parametrize("M", [NB * HMB * HMB, NB * HMB * HMB - 23], ids=["524288", "524265"])
 def test_tf32x3_colsum_vs_float64(dev, M):
     """epb_colsum over M x 1024 (the final layer's bias gradient; 524265 leaves a partial last CTA)"""
-    _check_colsum(dev, M, JB * DB)
+    sc._check_colsum(dev, M, JB * DB)
 
 
-# ------------------------------------------------------------------ 5. weights and optimiser on the fp32 engine
+# ------------------------------------------------------------------ 4. weights and optimiser on the fp32 engine
 @gpu
 def test_tf32x3_pack_weight_batch_bit_exact_on_model_jobs(dev):
     """pack_weight_batch on net.Engine's own jobs for R50 / J16 / D64 (every layer's fprop and
     dgrad operands, the stem's [64][160] patch-matrix operand, the per-stage unpacks of the
     packed weight gradients), bit-exact with the CPU emulation"""
-    from tests.test_gpu_step_kernels import _check_pack_weight_batch
-    _check_pack_weight_batch(dev, _r50(dev)[0])
+    sc._check_pack_weight_batch(dev, _r50(dev)[0])
 
 
 @gpu
 def test_tf32x3_fused_adam_vs_float64_on_model_buffer(dev):
     """FusedAdam over the tf32x3 model's flat parameter buffer: steps 1, 2 and 1000"""
-    from tests.test_gpu_step_kernels import _check_fused_adam
-    _check_fused_adam(dev, *_r50(dev))
+    sc._check_fused_adam(dev, *_r50(dev))

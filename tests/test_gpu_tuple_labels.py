@@ -7,7 +7,6 @@
   * a tuple whose root failed has all-zero weights; run to run, and split into sub-batches of
     tuples, every output is bit-identical;
   * V = 2 without failures or confidences is the two-ray DLT of epb_triangulate method 0;
-  * the coverage gate of tests/test_gpu_step_kernels.py over one robust graphed training step;
   * the robust online loss captured in a CUDA graph and replayed on three batches: loss, labels and
     logit gradient bit-identical to eager; the graphed robust training step against eager steps;
   * the script flow on the fixture tree with DATASET.TRI_VIEWS: 4 and the robust method."""
@@ -115,54 +114,6 @@ def test_v2_is_the_two_ray_dlt(dev):
     assert np.max(np.abs(ref.cpu().numpy() - label)) <= 1e-6
 
 
-def _r18(dev, J, D, HW, seed=0):
-    import lib.models as models
-    import lib.utils.utils as U
-    from oracle import refshim
-    torch.manual_seed(seed)
-    cfg = refshim.make_cfg(num_layers=18, num_joints=J, volume=True, depth_res=D, image_size=(HW, HW))
-    m = models.pose3d_resnet.get_pose_net(cfg, False, precision="f16x3").to(dev).train()
-    return m, U.FusedAdam(list(m.parameters()), lr=1e-4)
-
-
-def _synthetic_batch(J, HW, tuples, views=4):
-    """one view-major batch of SyntheticH36M through tuple_batch_sampler and loader_batch"""
-    from torch.utils.data import default_collate
-    from lib.core.config import AttrDict, _DEFAULTS
-    from lib.core.function import loader_batch
-    from lib.dataset.synthetic import SyntheticH36M
-    c = AttrDict(_DEFAULTS)
-    c.MODEL.NUM_JOINTS, c.MODEL.IMAGE_SIZE, c.DATASET.SYNTHETIC_LEN = J, [HW, HW], 4 * tuples
-    ds = SyntheticH36M(c)
-    idx = next(iter(ds.tuple_batch_sampler(tuples, views)))
-    return loader_batch(default_collate([ds[i] for i in idx]))
-
-
-def test_coverage_gate_robust_step(dev):
-    """One robust graphed step (R18, J = 16, D = 64, 2 tuples x 4 views of 256 x 256: warm-up,
-    capture, replay): every C-ABI entry it calls has a row in COVERAGE (test_gpu_step_kernels.py)
-    plus epb_tuple_labels, naming existing tests."""
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    from tests.test_gpu_step_kernels import COVERAGE, _missing_coverage, _record_calls
-    J, D, HW = 16, 64, 256
-    m, opt = _r18(dev, J, D, HW)
-    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method="robust",
-                               views=4)
-    x, _, _, meta = _synthetic_batch(J, HW, 2)
-    with _record_calls() as names:
-        for _ in range(2):
-            loss = step(x, meta=meta)
-        torch.cuda.synchronize()
-    assert step.graph is not None and math.isfinite(float(loss))
-    table = dict(COVERAGE, epb_tuple_labels=["test_gpu_tuple_labels.py::test_kernel_vs_restatement"])
-    print("  robust step calls %d entries: %s" % (len(names), sorted(names)))
-    assert "epb_tuple_labels" in names and "epb_triangulate" not in names
-    missing, dangling = _missing_coverage(names, table)
-    assert not missing, "entries without a float64 test: %s" % missing
-    assert not dangling, dangling
-
-
 def test_captured_robust_loss_matches_eager(dev):
     """online_epipolar_loss(method='robust', V = 4) and its backward captured in a CUDA graph on one
     resident batch of logits, replayed with three others: loss, labels, weights and logit gradient
@@ -220,11 +171,11 @@ def test_graphed_robust_step_matches_eager(dev):
     import lib.core.function as fn
     import lib.utils.img_utils as iu
     J, D, HW = 16, 16, 64
-    x, _, _, meta = _synthetic_batch(J, HW, 4)
+    x, _, _, meta = tc.synthetic_batch(J, HW, 4)
     x = x.to(dev)
     out = {}
     for mode in ("eager", "graph", "graph2"):
-        m, opt = _r18(dev, J, D, HW)
+        m, opt = tc.r18(dev, J, D, HW)
         step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method="robust",
                                    views=4)
         losses = []

@@ -1,0 +1,341 @@
+"""The coverage gate of the training step: every C-ABI entry one step of a composition calls must
+have a row in the composition's table naming the tests that hold it to float64 (or bit-exact
+against an exact restatement) at that composition's sizes.
+
+Each row of COMPOSITIONS runs one step of its composition at a reduced size and records the
+entries it calls: on the CPU through the emulated ABI (tests/emul_ops.py; the labels given, since
+the epipolar geometry has no CPU emulation) where the composition has one, and on the device with
+online labels.  A new composition is a new row; its float64 tests go in its own module, with the
+shared check bodies of tests/step_cases.py."""
+import contextlib
+import importlib
+import inspect
+import math
+import re
+
+import pytest
+import torch
+
+from tests import step_cases as sc
+from tests import tuple_label_cases as tc
+
+gpu = pytest.mark.gpu
+
+# ------------------------------------------------------------------ coverage tables
+# C-ABI entry of the step -> tests that check it against float64 (or bit-exact against an exact
+# restatement) at the composition's sizes.  C3 (test_c3_selfsup_chain_64_images) runs the geometry
+# on 16 tuples x 4 views: half the bench's batch of 32 tuples.
+COVERAGE = {
+    "epb_im2col_split": ["test_gpu_step_kernels.py::test_im2col_split_bit_exact_at_stem_bench_size"],
+    "epb_conv16_fprop": ["test_gpu_split16.py::test_conv16_bench_layer_shapes_vs_torch_float64",
+                         "test_gpu_bn_chain.py::test_conv16_stats_vs_float64"],
+    "epb_conv16_wgrad": ["test_gpu_split16.py::test_conv16_bench_layer_shapes_vs_torch_float64"],
+    "epb_bn_finalize_scale": ["test_gpu_bn_chain.py::test_bn_finalize_scale_vs_float64"],
+    "epb_bn_finalize": ["test_gpu_step_kernels.py::test_bn_finalize_vs_float64_at_bench_M",
+                        "test_gpu_split16.py::test_bn_finalize_scale_vs_two_calls"],
+    "epb_act_scale": ["test_gpu_bn_chain.py::test_scale_contract_adversarial"],
+    "epb_bn_act_split": ["test_gpu_bn_chain.py::test_bn_act_split_vs_float64_at_bench_M"],
+    "epb_bn_relu_maxpool_split": ["test_gpu_bn_chain.py::test_bn_relu_maxpool_split_vs_float64_at_stem_size"],
+    "epb_maxpool_bwd": ["test_gpu_step_kernels.py::test_maxpool_bwd_vs_float64_at_stem_bench_size"],
+    "epb_bn_bwd_split": ["test_gpu_bn_chain.py::test_bn_bwd_split_vs_float64_at_bench_M"],
+    "epb_softargmax_fwd": ["test_gpu_step_kernels.py::test_softargmax_fwd_vs_float64_at_bench_shape"],
+    "epb_softargmax_bwd_split": ["test_gpu_bn_chain.py::test_softargmax_bwd_split_vs_float64_at_bench_shape"],
+    "epb_jointloss_fwd_bwd": ["test_gpu_step_kernels.py::test_jointloss_vs_float64_at_bench_shape"],
+    "epb_split16_batch": ["test_gpu_step_kernels.py::test_split16_batch_bit_exact_on_model_jobs"],
+    "epb_split16": ["test_gpu_step_kernels.py::test_split16_batch_bit_exact_on_model_jobs"],
+    "epb_pack_weight_batch": ["test_gpu_step_kernels.py::test_pack_weight_batch_bit_exact_on_model_jobs"],
+    "epb_adam_step_dev": ["test_gpu_step_kernels.py::test_fused_adam_vs_float64_on_model_buffer",
+                          "test_gpu_step_kernels.py::test_adam_dev_cases_vs_float64",
+                          "test_gpu_step_kernels.py::test_adam_dev_multi_step_drift"],
+    "epb_adam_step": ["test_gpu_step_kernels.py::test_adam_per_tensor_paths_vs_float64"],
+    "epb_patch_to_image": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_triangulate": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_project_labels": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+}
+
+S = "test_gpu_c5_step.py::"
+COVERAGE_C5 = {
+    "epb_im2col_split": [S + "test_c5_im2col_split_bit_exact_at_stem"],
+    "epb_conv16_fprop": [S + "test_c5_conv16_layers_vs_torch_float64", S + "test_c5_final_conv16_fprop_vs_float64",
+                         S + "test_c5_conv16_stats_vs_float64"],
+    "epb_conv16_wgrad": [S + "test_c5_conv16_layers_vs_torch_float64"],
+    "epb_bn_finalize_scale": [S + "test_c5_bn_finalize_scale_vs_float64"],
+    "epb_bn_finalize": [S + "test_c5_bn_finalize_vs_float64"],
+    "epb_bn_act_split": [S + "test_c5_bn_act_split_vs_float64"],
+    "epb_bn_relu_maxpool_split": [S + "test_c5_bn_relu_maxpool_split_vs_float64"],
+    "epb_maxpool_bwd": [S + "test_c5_maxpool_bwd_vs_float64"],
+    "epb_bn_bwd_split": [S + "test_c5_bn_bwd_split_vs_float64"],
+    "epb_softargmax_fwd": [S + "test_c5_softargmax_fwd_vs_float64"],
+    "epb_softargmax_bwd": [S + "test_c5_softargmax_bwd_fp32_vs_float64"],
+    "epb_colsum": [S + "test_c5_colsum_vs_float64"],
+    "epb_conv_wgrad": [S + "test_c5_final_tf32_wgrad_vs_float64"],
+    "epb_conv_fprop": [S + "test_c5_final_tf32_dgrad_vs_float64"],
+    "epb_jointloss_fwd_bwd": [S + "test_c5_jointloss_vs_float64"],
+    "epb_split16_batch": [S + "test_c5_split16_batch_bit_exact_on_model_jobs"],
+    "epb_pack_weight_batch": [S + "test_c5_pack_weight_batch_bit_exact_on_model_jobs"],
+    "epb_adam_step_dev": [S + "test_c5_fused_adam_vs_float64_on_model_buffer"],
+    "epb_patch_to_image": [S + "test_c5_selfsup_geometry_j17"],
+    "epb_triangulate": [S + "test_c5_selfsup_geometry_j17"],
+    "epb_project_labels": [S + "test_c5_selfsup_geometry_j17"],
+}
+# the head's fp32 backward: entries the C4 step does not call
+HEAD_C5 = {"epb_softargmax_bwd", "epb_colsum", "epb_conv_wgrad", "epb_conv_fprop"}
+
+S = "test_gpu_tf32x3_step.py::"
+SK = "test_gpu_step_kernels.py::"
+COVERAGE_TF32X3 = {
+    "epb_nchw_to_nhwc": [S + "test_tf32x3_nchw_to_nhwc_bit_exact"],
+    "epb_im2col": [S + "test_tf32x3_im2col_bit_exact_at_stem"],
+    "epb_conv_fprop": [S + "test_tf32x3_conv_layers_vs_float64"],
+    "epb_conv_wgrad": [S + "test_tf32x3_conv_layers_vs_float64", S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
+    "epb_bn_finalize": [S + "test_tf32x3_bn_finalize_vs_float64", SK + "test_bn_finalize_vs_float64_at_bench_M"],
+    "epb_bn_relu_maxpool": [S + "test_tf32x3_bn_relu_maxpool_vs_float64"],
+    "epb_bn_act": [S + "test_tf32x3_bn_act_vs_float64"],
+    "epb_bn_bwd_reduce": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
+    "epb_bn_bwd_apply": [S + "test_tf32x3_bn_bwd_vs_float64", S + "test_tf32x3_bn_bwd_edge_shapes"],
+    "epb_add_masked": [S + "test_tf32x3_add_masked_bit_exact"],
+    "epb_maxpool_bwd": [SK + "test_maxpool_bwd_vs_float64_at_stem_bench_size"],
+    "epb_softargmax_fwd": [SK + "test_softargmax_fwd_vs_float64_at_bench_shape"],
+    "epb_softargmax_bwd": [S + "test_tf32x3_softargmax_bwd_fp32_vs_float64"],
+    "epb_colsum": [S + "test_tf32x3_colsum_vs_float64"],
+    "epb_jointloss_fwd_bwd": [SK + "test_jointloss_vs_float64_at_bench_shape"],
+    "epb_pack_weight_batch": [S + "test_tf32x3_pack_weight_batch_bit_exact_on_model_jobs",
+                              S + "test_tf32x3_stem_wgrad_through_flat_buffer"],
+    "epb_adam_step_dev": [S + "test_tf32x3_fused_adam_vs_float64_on_model_buffer"],
+    "epb_patch_to_image": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_triangulate": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+    "epb_project_labels": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+}
+# the fp32 engine's own entries: the f16x3 step calls none of them
+FP32_ENGINE = {"epb_nchw_to_nhwc", "epb_im2col", "epb_conv_fprop", "epb_conv_wgrad", "epb_bn_finalize",
+               "epb_bn_relu_maxpool", "epb_bn_act", "epb_bn_bwd_reduce", "epb_bn_bwd_apply", "epb_add_masked",
+               "epb_softargmax_bwd", "epb_colsum"}
+
+COVERAGE_ROBUST = dict(COVERAGE, epb_tuple_labels=["test_gpu_tuple_labels.py::test_kernel_vs_restatement"])
+
+
+def _missing_coverage(recorded, table):
+    """entries without a row, and rows that name a test function that does not exist"""
+    missing = sorted(set(recorded) - set(table))
+    dangling = []
+    for entry in sorted(set(recorded) & set(table)):
+        for tid in table[entry]:
+            mod, _, fn = tid.partition("::")
+            m = importlib.import_module("tests." + mod[:-3])
+            if not callable(getattr(m, fn, None)):
+                dangling.append((entry, tid))
+    return missing, dangling
+
+
+def _entry_names(mod_ops):
+    """ops wrapper name -> the C-ABI entries it calls"""
+    out = {}
+    for k, f in vars(mod_ops).items():
+        if inspect.isfunction(f) and f.__module__ == mod_ops.__name__:
+            e = re.findall(r'_call\("(epb_[a-z0-9_]+)"', inspect.getsource(f))
+            if e:
+                out[k] = e
+    return out
+
+
+@contextlib.contextmanager
+def _emulated_abi():
+    """The model code runs on tests/emul_ops.py: the set of C-ABI entries its wrappers stand for.
+    Nested emulations (an emulated entry that calls another) count as their outer entry only."""
+    import lib.core.integral_loss as il
+    import lib.utils.utils as Ut
+    from epipolarpose_b200 import ops
+    from tests import emul_ops
+    rec, depth, saved = set(), [0], {}
+    for k, e in _entry_names(ops).items():
+        if not hasattr(emul_ops, k):
+            continue
+        f = saved[k] = getattr(emul_ops, k)
+
+        def wrap(*a, _f=f, _e=e, **kw):
+            if depth[0] == 0:
+                rec.update(_e)
+            depth[0] += 1
+            try:
+                return _f(*a, **kw)
+            finally:
+                depth[0] -= 1
+        setattr(emul_ops, k, wrap)
+    il._backend[0], Ut._backend[0] = emul_ops, emul_ops
+    try:
+        yield rec
+    finally:
+        for k, f in saved.items():
+            setattr(emul_ops, k, f)
+        il._backend[0] = Ut._backend[0] = ops
+
+
+def _three_pass_convs(tags):
+    """every conv kernel that ran is a three-pass instantiation, and both an fprop and a wgrad ran"""
+    return sc._all_three_pass(tags) and any(t.startswith("fprop") for t in tags) and \
+        any(t.startswith("wgrad") for t in tags)
+
+
+def _fp32_engine(eng):
+    from epipolarpose_b200 import net
+    return type(eng) is net.Engine and eng.precision == 3 and eng.wgrad_precision == 3
+
+
+# ------------------------------------------------------------------ steps
+def _eager_step(dev, row):
+    """GraphedTrainStep(online=True).eager_step on the bench's cameras, FusedAdam, SmoothL1"""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    import lib.utils.img_utils as iu
+    import lib.utils.utils as Ut
+    layers, J, D, HW, tuples = row["device"]
+    B = 4 * tuples
+    torch.manual_seed(0)
+    m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW), False, precision=row["precision"]).to(dev).train()
+    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method=row["method"])
+    meta = iu.pack_meta({k: v.to(dev) for k, v in sc._bench_meta(tuples).items()}, B, dev)
+    x = torch.randn(B, 3, HW, HW, device=dev)
+    return m, lambda: step.eager_step(x, None, None, meta)
+
+
+def _graphed_step(dev, row):
+    """GraphedTrainStep(online=True) on a SyntheticH36M tuple batch: warm-up, capture, replay"""
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    layers, J, D, HW, tuples = row["device"]
+    assert layers == 18
+    m, opt = tc.r18(dev, J, D, HW)
+    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method=row["method"],
+                               views=row["views"])
+    x, _, _, meta = tc.synthetic_batch(J, HW, tuples, row["views"])
+
+    def run():
+        for _ in range(2):
+            loss = step(x, meta=meta)
+        assert step.graph is not None, "no graph captured"
+        return loss
+    return m, run
+
+
+# ------------------------------------------------------------------ compositions
+# emulated / device: (layers, J, D, image size, and for the device half tuples of 4 views); calls:
+# entries every half must call; online: entries the device half (online labels) must call too
+COMPOSITIONS = {
+    "c4_f16x3": dict(
+        table=COVERAGE, precision="f16x3", method="iterative", views=4, driver=_eager_step,
+        emulated=(18, 16, 64, 64), device=(18, 16, 64, 256, 2),
+        calls={"epb_adam_step_dev", "epb_split16_batch"}, online={"epb_triangulate"}, not_called=set(),
+        engine=None, tags=None),
+    "c5": dict(
+        table=COVERAGE_C5, precision="f16x3", method="iterative", views=4, driver=_eager_step,
+        emulated=(18, 17, 96, 64), device=(101, 17, 96, 384, 2),
+        calls=HEAD_C5 | {"epb_adam_step_dev"}, online={"epb_triangulate"}, not_called={"epb_softargmax_bwd_split"},
+        engine=lambda eng: not eng.takes_logit_sink(), tags=None),
+    "c4_tf32x3": dict(
+        table=COVERAGE_TF32X3, precision="tf32x3", method="iterative", views=4, driver=_eager_step,
+        emulated=(18, 16, 64, 64), device=(50, 16, 64, 256, 2),
+        calls=FP32_ENGINE | {"epb_adam_step_dev"}, online={"epb_triangulate"},
+        not_called=lambda e: e.endswith("_split") or "conv16" in e,
+        engine=_fp32_engine, tags=_three_pass_convs),
+    "robust_tuples": dict(
+        table=COVERAGE_ROBUST, precision="f16x3", method="robust", views=4, driver=_graphed_step,
+        emulated=None, device=(18, 16, 64, 256, 2),
+        calls=set(), online={"epb_tuple_labels"}, not_called={"epb_triangulate"},
+        engine=None, tags=None),
+}
+EMULATED = [k for k, row in COMPOSITIONS.items() if row["emulated"] is not None]
+
+
+def _check_calls(row, calls, required, what):
+    print("  %s calls %d entries:" % (what, len(calls)))
+    for e in sorted(calls):
+        print("    %-28s -> %s" % (e, ", ".join(row["table"].get(e, ["(none)"]))))
+    assert required <= calls, "not called: %s" % sorted(required - calls)
+    nc = row["not_called"]
+    called = sorted(e for e in calls if (nc(e) if callable(nc) else e in nc))
+    assert not called, "called: %s" % called
+    missing, dangling = _missing_coverage(calls, row["table"])
+    assert not missing, "entries without a float64 test at the composition's sizes: %s" % missing
+    assert not dangling, dangling
+
+
+@pytest.mark.parametrize("comp", list(COMPOSITIONS))
+def test_gate_has_teeth(comp):
+    """Deleting any row, or pointing one at a test that does not exist, fails the gate; the kernel
+    tag check rejects a single-pass or CUDA-core conv among three-pass ones, and an empty set."""
+    table, tags = COMPOSITIONS[comp]["table"], COMPOSITIONS[comp]["tags"]
+    rec = sorted(table)
+    assert _missing_coverage(rec, table) == ([], [])
+    for k in rec:
+        t = dict(table)
+        del t[k]
+        assert _missing_coverage(rec, t)[0] == [k]
+        t[k] = ["test_gpu_step_kernels.py::test_no_such_test"]
+        assert _missing_coverage(rec, t)[1]
+    if tags is not None:
+        good = {"fprop_tc<64,3>", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
+        assert tags(good)
+        for bad in ("fprop_tc<128,1>", "wgrad_tc<64,1>", "wgrad_simt", "fprop_simt"):
+            assert not tags(good | {bad})
+        assert not tags(set())
+
+
+@pytest.mark.parametrize("comp", EMULATED)
+def test_gate_emulated_step(comp):
+    """One training step of the composition (R18 trunk, its J and D, 2 tuples x 4 views of 64 x 64)
+    through the emulated ABI: GraphedTrainStep.eager_step with given labels,
+    SmoothL1JointLocationLoss, FusedAdam.  Every entry it calls has a row naming existing tests."""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    import lib.utils.utils as Ut
+    from tests import emul_ops
+    row = COMPOSITIONS[comp]
+    layers, J, D, HW = row["emulated"]
+    B = 8
+    with _emulated_abi() as rec:
+        torch.manual_seed(0)
+        m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW), False, ops=emul_ops,
+                                              precision=row["precision"]).train()
+        if row["engine"] is not None:
+            assert row["engine"](m._engine())
+        opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+        step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
+        g = torch.Generator().manual_seed(1)
+        loss = step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
+                               torch.ones(B, J * 3), None)
+        assert math.isfinite(float(loss))
+    _check_calls(row, rec, row["calls"], "emulated %s step" % comp)
+
+
+@pytest.fixture(scope="module")
+def dev():
+    from epipolarpose_b200 import ops
+    ops.device_check()
+    return torch.device("cuda:0")
+
+
+@gpu
+@pytest.mark.parametrize("comp", list(COMPOSITIONS))
+def test_gate_device_step(dev, comp):
+    """One step of the composition at a reduced batch (2 tuples x 4 views) with online labels, on
+    the device.  Every entry it calls has a row naming existing tests; where the row has a tag
+    predicate, the step runs under the profiler and the conv kernels that ran must meet it."""
+    row = COMPOSITIONS[comp]
+    m, run = row["driver"](dev, row)
+    if row["engine"] is not None:
+        assert row["engine"](m._engine())
+    losses, tags = [], None
+    with sc._record_calls() as names:
+        if row["tags"] is None:
+            losses.append(float(run()))
+        else:
+            tags = sc._ran(lambda: losses.append(float(run())))
+        torch.cuda.synchronize()
+    assert losses and all(math.isfinite(v) for v in losses)
+    if tags is not None:
+        print("  conv kernels %s" % sorted(tags))
+        assert row["tags"](tags), "conv kernels: %s" % sorted(tags)
+    _check_calls(row, names, row["calls"] | row["online"], "%s step" % comp)

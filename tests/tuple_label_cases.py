@@ -2,7 +2,9 @@
 restatement of epb_tuple_labels (written from its contract in include/epb.h on top of the oracle's
 trans_coords_from_patch_to_org_3d for patch -> image, tests/multiview_cases.py::robust_point for
 the robust fit and the oracle's labels_from_global_coords for the projection, plus the weight rule),
-and seeded view-major batches of ring-camera tuples with known joints."""
+seeded view-major batches of ring-camera tuples with known joints, and the small robust-step model
+and SyntheticH36M batch that test_gpu_tuple_labels and the coverage gate of tests/test_step_coverage.py
+train on."""
 import numpy as np
 
 from oracle import restate
@@ -107,3 +109,28 @@ def packed(meta):
                           np.asarray(meta["f"], np.float64).reshape(B, 2), np.asarray(meta["c"], np.float64).reshape(B, 2)],
                          axis=1)
     return box, P, cam
+
+
+def r18(dev, J, D, HW, seed=0):
+    """R18 (f16x3) of J joints, D depth bins, HW x HW images in train mode, with FusedAdam"""
+    import torch
+    import lib.models as models
+    import lib.utils.utils as U
+    from oracle import refshim
+    torch.manual_seed(seed)
+    cfg = refshim.make_cfg(num_layers=18, num_joints=J, volume=True, depth_res=D, image_size=(HW, HW))
+    m = models.pose3d_resnet.get_pose_net(cfg, False, precision="f16x3").to(dev).train()
+    return m, U.FusedAdam(list(m.parameters()), lr=1e-4)
+
+
+def synthetic_batch(J, HW, tuples, views=4):
+    """one view-major batch of SyntheticH36M through tuple_batch_sampler and loader_batch"""
+    from torch.utils.data import default_collate
+    from lib.core.config import AttrDict, _DEFAULTS
+    from lib.core.function import loader_batch
+    from lib.dataset.synthetic import SyntheticH36M
+    c = AttrDict(_DEFAULTS)
+    c.MODEL.NUM_JOINTS, c.MODEL.IMAGE_SIZE, c.DATASET.SYNTHETIC_LEN = J, [HW, HW], 4 * tuples
+    ds = SyntheticH36M(c)
+    idx = next(iter(ds.tuple_batch_sampler(tuples, views)))
+    return loader_batch(default_collate([ds[i] for i in idx]))

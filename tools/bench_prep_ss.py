@@ -90,7 +90,7 @@ def main():
     from lib.dataset.JointIntegralDataset import load_pickle
     from lib.utils.prep_h36m import save_triangulations, _make_predictor, joint_layout
     from tests import golden_inputs as gi
-    from tests.test_gpu_sizes import _model
+    from tests.golden_inputs import _model
     from tests import dataset_cases as dc
     from epipolarpose_b200 import ops
     ops.device_check()

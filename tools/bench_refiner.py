@@ -130,7 +130,7 @@ with tempfile.TemporaryDirectory() as tmp:
 # RefinedPosePredictor against PosePredictor (R50, J16, D64, 256x256 images, random init)
 from lib.core.inference import PosePredictor, RefinedPosePredictor  # noqa: E402
 from tests import golden_inputs as gi  # noqa: E402
-from tests.test_gpu_sizes import _model  # noqa: E402
+from tests.golden_inputs import _model  # noqa: E402
 net = _model(dev, gi.SIZE_CASES["c1"], "f16x3", train=False)
 rp = RefinedPosePredictor(net, model, None, flip_test=False)
 pp = PosePredictor(net, flip_test=False)
