@@ -407,7 +407,9 @@ class Engine16(_net.Engine):
             self._conv_wgrad16(fin, fsrc, fsrc_sc, dl16, dl_sc, N, h, w)
             dcur = self._conv_dgrad16(fin, dl16, dl_sc, N, h, w, wd16(fin))
         else:
-            # few output channels (test-sized heads): the 3xTF32 kernels take the fp32 gradient
+            # few output channels (test-sized heads): the fp32-operand kernels take the fp32
+            # gradient (3xTF32, or the CUDA-core kernels where a channel count is not a multiple
+            # of 32: conv.cu)
             self._conv_wgrad(fin, src, dlogits, N, h, w, grads[fin.name + ".weight"], affine=aff)
             dcur = self._conv_dgrad(fin, dlogits, N, h, w, S["packed"][fin.name][1])
         # ---- deconv head, reversed

@@ -1,5 +1,5 @@
 """Shared by the training-step tests (test_gpu_step_kernels, test_gpu_c5_step, test_gpu_tf32x3_step,
-test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32, test_gpu_predictor, test_gpu_conv16_store and
+test_gpu_c2_flat_step, test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32, test_gpu_predictor, test_gpu_conv16_store and
 test_step_coverage): the float64 check bodies each composition runs at its own sizes, the bars and
 the emulations they rest on, the restated planners, the layer tables, the device data makers and
 one cache of models and conv outputs keyed by composition.
@@ -33,7 +33,9 @@ STATS_SELF_BAR = 1e-6  # BatchNorm sums against float64 sums of the kernel's own
 _CACHE = {}
 # composition -> (layers, J, D, image size, precision) of its bench model
 MODELS = {"c4_f16x3": (50, 16, 64, 256, "f16x3"), "c5": (101, 17, 96, 384, "f16x3"),
-          "c4_tf32x3": (50, 16, 64, 256, "tf32x3")}
+          "c4_tf32x3": (50, 16, 64, 256, "tf32x3"), "c2_flat": (50, 17, 64, 256, "f16x3")}
+# compositions whose model has the VOLUME=False head: 2-D heat-maps and depth_fc (2048 -> J D)
+FLAT_HEAD = {"c2_flat"}
 
 
 def release(prefix):
@@ -56,14 +58,15 @@ def bench_model(dev, comp):
         import lib.utils.utils as Ut
         layers, J, D, HW, precision = MODELS[comp]
         torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(_cfg(layers, J, D, HW), False, precision=precision).to(dev).train()
+        m = models.pose3d_resnet.get_pose_net(_cfg(layers, J, D, HW, volume=comp not in FLAT_HEAD), False,
+                                              precision=precision).to(dev).train()
         _CACHE[key] = (m, Ut.FusedAdam(list(m.parameters()), lr=1e-3))
     return _CACHE[key]
 
 
-def _cfg(layers, J, D, HW):
+def _cfg(layers, J, D, HW, volume=True):
     from oracle import refshim
-    return refshim.make_cfg(num_layers=layers, num_joints=J, volume=True, depth_res=D, image_size=(HW, HW))
+    return refshim.make_cfg(num_layers=layers, num_joints=J, volume=volume, depth_res=D, image_size=(HW, HW))
 
 
 def _bench_meta(tuples, seed=1000):
@@ -397,6 +400,26 @@ C5_LAYERS = [
     ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 12), ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 12),
     ("deconv0", "deconv", 2048, 256, 4, 2, 1, 12), ("deconv1", "deconv", 256, 256, 4, 2, 1, 24),
     ("deconv2", "deconv", 256, 256, 4, 2, 1, 48),
+]
+
+# every distinct split-path conv of R50 at 256 x 256 (trunk at 64 / 32 / 16 / 8, deconvs 8 -> 64),
+# the stem's patch-matrix conv (K 147 -> 192, whole 64-channel blocks); (name, kind, cin, cout, k,
+# stride, pad, input hw).  The final layer (256 -> J with bias) has its own test.
+C2_LAYERS = [
+    ("stem_col_192_64", "conv", 192, 64, 1, 1, 0, 128),
+    ("l1_1x1_64_64", "conv", 64, 64, 1, 1, 0, 64), ("l1_3x3_64", "conv", 64, 64, 3, 1, 1, 64),
+    ("l1_1x1_64_256", "conv", 64, 256, 1, 1, 0, 64), ("l1_1x1_256_64", "conv", 256, 64, 1, 1, 0, 64),
+    ("l2_1x1_256_128", "conv", 256, 128, 1, 1, 0, 64), ("l2_3x3_s2", "conv", 128, 128, 3, 2, 1, 64),
+    ("l2_1x1_128_512", "conv", 128, 512, 1, 1, 0, 32), ("l2_1x1_s2_down", "conv", 256, 512, 1, 2, 0, 64),
+    ("l2_1x1_512_128", "conv", 512, 128, 1, 1, 0, 32), ("l2_3x3_128", "conv", 128, 128, 3, 1, 1, 32),
+    ("l3_1x1_512_256", "conv", 512, 256, 1, 1, 0, 32), ("l3_3x3_s2", "conv", 256, 256, 3, 2, 1, 32),
+    ("l3_1x1_256_1024", "conv", 256, 1024, 1, 1, 0, 16), ("l3_1x1_s2_down", "conv", 512, 1024, 1, 2, 0, 32),
+    ("l3_1x1_1024_256", "conv", 1024, 256, 1, 1, 0, 16), ("l3_3x3_256", "conv", 256, 256, 3, 1, 1, 16),
+    ("l4_1x1_1024_512", "conv", 1024, 512, 1, 1, 0, 16), ("l4_3x3_s2", "conv", 512, 512, 3, 2, 1, 16),
+    ("l4_1x1_512_2048", "conv", 512, 2048, 1, 1, 0, 8), ("l4_1x1_s2_down", "conv", 1024, 2048, 1, 2, 0, 16),
+    ("l4_1x1_2048_512", "conv", 2048, 512, 1, 1, 0, 8), ("l4_3x3_512", "conv", 512, 512, 3, 1, 1, 8),
+    ("deconv0", "deconv", 2048, 256, 4, 2, 1, 8), ("deconv1", "deconv", 256, 256, 4, 2, 1, 16),
+    ("deconv2", "deconv", 256, 256, 4, 2, 1, 32),
 ]
 
 
@@ -1500,3 +1523,300 @@ def _check_conv16_layer(dev, layer, N, wgrad_bar):
     e = float((dw.view(cout, T, cin).double() - r).abs().max() / r.abs().max())
     assert e <= wgrad_bar, "wgrad %.3e (bar %.2e)" % (e, wgrad_bar)   # C4: fp32 runs over up to 524288 / 74 pixels
     return e_f, e_d, e
+
+
+# ------------------------------------------------------------------ 3xTF32 conv at a layer shape
+def _pad4(c):
+    return (c + 3) // 4 * 4
+
+
+def tf32_wgrad_runs(layer, N):
+    """(pixels N Hp Wp, Cin, Cout, taps) of each wgrad geometry of a C4_LAYERS_TF32X3-style row: one
+    for a convolution, one per output phase (2 x 2, 4 taps each) for the 4 x 4 / 2 deconvolutions"""
+    _, kind, cin, cout, k, s, p, hw, _, _ = layer
+    if kind == "conv":
+        ho = (hw + 2 * p - k) // s + 1
+        return [(N * ho * ho, cin, cout, k * k)]
+    return [(N * hw * hw, cin, cout, 4)] * 4
+
+
+def tf32_wgrad_run(layer, N):
+    """the longest pixel run of one CTA over the layer's wgrad geometries"""
+    return max(_tf32_wgrad_plan(M, ci, co, T, 3)[0] for M, ci, co, T in tf32_wgrad_runs(layer, N))
+
+
+def tc_supported(gm, wgrad):
+    """conv_tc.cu epb_conv_tc_supported / conv_tc_wgrad.cu epb_conv_wgrad_tc_supported: whether
+    epb_conv_fprop / epb_conv_wgrad at precision 1 or 3 run the tensor-core kernels on geometry gm
+    (else the fp32 CUDA-core kernels)"""
+    fits = gm.N * gm.Hi * gm.Wi * gm.Cin < 1 << 31
+    if wgrad:
+        return gm.Cin % 32 == 0 and gm.Cout % 4 == 0 and gm.Cout >= 32 and fits and gm.N * gm.Ho * gm.Wo < 1 << 31
+    return gm.Cin % 32 == 0 and gm.Cout % 32 == 0 and gm.Cout >= 32 and fits
+
+
+def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
+    """3xTF32 fprop (statistics into a zeroed buffer, or the bias for a layer named final* or
+    depth_fc*), dgrad (written, or added into the block's input gradient for a downsample) and
+    wgrad (into a zeroed dW) of a C4_LAYERS_TF32X3-style row over N images with its operand mode,
+    each against torch float64 within its bar: fprop / dgrad _tc_bar(FPROP_BAR, K, 3), K the
+    longest taps x Cin of the call's geometries; wgrad _tc_bar(WGRAD_BAR, R, 3), R the pixel run
+    of one CTA from the restated planner.  Every output followed by a guard band; the conv
+    kernels that ran (_ran's tags) must meet `kernels`: by default every one a three-pass
+    instantiation.  kernels=None opens no profiler session: the caller shows which kernels run."""
+    import torch.nn.functional as F
+    from epipolarpose_b200 import ops
+    name, kind, cin, cout, k, s, p, hw, operand, dmode = layer
+    final = name.startswith(("final", "depth_fc"))
+    conv, Ho, Wo, x, sc, sh, w, gout = _layer(dev, kind, cin, cout, k, s, p, 0, N, hw, hw, 17)
+    ci, co, T = conv.cin_p, conv.cout_p, k * k
+    act = operand == "act"
+    aff = (sc, sh) if act else (None, None)
+    wf, wd = conv.pack(ops, w)
+    tags, errs = set(), {}
+    # ---- fprop
+    bias = torch.randn(co, device=dev, generator=torch.Generator(device=dev).manual_seed(5)) * 0.5 if final else None
+    geoms = conv.fprop_geoms(ops, N, hw, hw, 3)
+    gms = _geoms(geoms, int(act), 0)
+    out, guard = _guarded((N, Ho, Wo, co), dev, 0.0 if any(gm is None for gm in geoms) else float("nan"))
+    guard.fill_(1234.5)
+    stats = sguard = None
+    if not final:
+        sbuf = torch.zeros(2 * co + 64, device=dev, dtype=torch.float64)
+        stats, sguard = sbuf[:2 * co], sbuf[2 * co:]
+
+    def fwd(o, st):
+        for gm in gms:
+            ops.conv_fprop(gm, x, wf, o, aff[0], aff[1], bias, st)
+    if kernels is not None:
+        tags |= _ran(lambda: fwd(out.clone(), None if stats is None else stats.clone()))
+    fwd(out, stats)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "fprop guard band overwritten"
+    a64 = _act64(x, *aff, act)
+    with torch.no_grad():
+        ref = _fwd64(conv, a64, w.double())
+        if bias is not None:
+            ref += bias.double()[None, :, None, None]
+        ref = ref.permute(0, 2, 3, 1)
+        bar_f = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in gms), 3)
+        errs["fprop"] = float((out.double() - ref).abs().max() / ref.abs().max())   # NaN fails
+        if stats is not None:
+            assert bool((sguard == 0).all()), "statistics guard band overwritten"
+            o = out.double().reshape(-1, co)
+            s1, s2 = stats[:co], stats[co:]
+            errs["st_self"] = max(float(((s1 - o.sum(0)).abs() / o.abs().sum(0).clamp_min(1e-300)).max()),
+                                  float(((s2 - (o * o).sum(0)).abs() / (o * o).sum(0).clamp_min(1e-300)).max()))
+            del o
+            r = ref.reshape(-1, co)
+            r2 = (r * r).sum(0)
+            errs["st_ref"] = max(float(((s1 - r.sum(0)).abs() / r.abs().sum(0).clamp_min(1e-300)).max()),
+                                 float((s2 - r2).abs().max() / r2.abs().max()))
+            del r, r2
+    del out, ref
+    # ---- dgrad
+    bar_d = None
+    if dmode is not None:
+        dgeoms = conv.dgrad_geoms(ops, N, hw, hw, 3)
+        acc = int(dmode == "acc")
+        dgms = _geoms(dgeoms, 0, acc)
+        with torch.no_grad():
+            g64, w64 = gout.permute(0, 3, 1, 2).double(), w.double()
+            if kind == "conv":
+                ref = torch.nn.grad.conv2d_input((N, ci, hw, hw), w64, g64, s, p)
+            else:
+                ref = F.conv2d(g64, w64, None, s, p)
+            del g64
+            ref = ref.permute(0, 2, 3, 1)
+        din, guard = _guarded((N, hw, hw, ci), dev, 0.0 if (acc or any(gm is None for gm in dgeoms)) else float("nan"))
+        guard.fill_(1234.5)
+        init = None
+        if acc:
+            init = torch.randn(din.shape, device=dev, generator=torch.Generator(device=dev).manual_seed(9))
+            init *= float(ref.abs().max()) / 3
+            din.copy_(init)
+
+        def bwd(o):
+            for gm in dgms:
+                ops.conv_fprop(gm, gout, wd, o, None, None, None, None)
+        if kernels is not None:
+            tags |= _ran(lambda: bwd(din.clone()))
+        bwd(din)
+        torch.cuda.synchronize()
+        assert bool((guard == 1234.5).all()), "dgrad guard band overwritten"
+        base = init.double() if init is not None else 0.0
+        errs["dgrad"] = float((din.double() - (base + ref)).abs().max() / ref.abs().max())
+        bar_d = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in dgms), 3)
+        del din, ref, init
+    # ---- wgrad
+    runs = sorted((gm.N * gm.Hp * gm.Wp, gm.Cin, gm.Cout, gm.T) for gm in gms)
+    assert runs == sorted((M, _pad4(a), _pad4(b), t) for M, a, b, t in tf32_wgrad_runs(layer, N)), runs
+    R = tf32_wgrad_run(layer, N)
+    bar_w = _tc_bar(WGRAD_BAR, R, 3)
+    w64 = w.double().requires_grad_(True)
+    _fwd64(conv, a64, w64).backward(gout.permute(0, 3, 1, 2).double())
+    del a64
+    gw = w64.grad
+    ref = (gw.permute(0, 2, 3, 1) if kind == "conv" else gw.permute(1, 2, 3, 0)).reshape(co, T, ci)
+    del w64, gw
+    dw, guard = _guarded((co * T * ci,), dev, 0.0)
+    guard.fill_(1234.5)
+
+    def wgr(o):
+        for gm in gms:
+            ops.conv_wgrad(gm, x, gout, o, aff[0], aff[1])
+    if kernels is not None:
+        tags |= _ran(lambda: wgr(torch.zeros_like(dw)))
+    wgr(dw)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "dW guard band overwritten"
+    errs["wgrad"] = float((dw.view(co, T, ci).double() - ref).abs().max() / ref.abs().max())
+    print("  %-22s %-36s fprop %.2e (bar %.2e)%s%s wgrad %.2e (run %d, bar %.2e)" % (
+        name, ",".join(sorted(tags)), errs["fprop"], bar_f,
+        " stats %.1e / %.1e" % (errs["st_self"], errs["st_ref"]) if "st_self" in errs else "",
+        " dgrad %.2e (bar %.2e)" % (errs["dgrad"], bar_d) if bar_d else "", errs["wgrad"], R, bar_w))
+    assert kernels is None or kernels(tags), tags
+    assert errs["fprop"] <= bar_f, errs
+    if "st_self" in errs:
+        assert errs["st_self"] <= STATS_SELF_BAR and errs["st_ref"] <= bar_f, errs
+    if bar_d is not None:
+        assert errs["dgrad"] <= bar_d, errs
+    assert errs["wgrad"] <= bar_w, errs
+
+
+# ------------------------------------------------------------------ the VOLUME=False head: pooling, heat-map loss
+HM_THREADS, HM_MAX_BLOCKS = 256, 8 * NUM_SMS     # softargmax.cu kHmThreads, kHmMaxBlocks
+
+
+def _check_avgpool_split(dev, N, HW, C):
+    """epb_avgpool_split of trunk planes [N, HW, C] (relu(randn) x 3: block outputs) with their
+    scale, against float64 of the joined planes.  The kernel adds the HW (hi + lo) pairs of a
+    channel in fp32 in pixel order (one rounding per pair, one per running sum), multiplies by the
+    power-of-two scale (exact) and divides by HW (one rounding): |d y| <= (HW + 1) u sum_p |v_p| /
+    HW + u |y|, v the joined values."""
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(101)
+    x, x_sc, xv = _split_dev(torch.relu(torch.randn(N, HW, C, device=dev, generator=g)) * 3)
+    y, guard = _guarded((N, C), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.avgpool_split(x, x_sc, y, N, HW, C)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    ref = xv.mean(1)
+    bar = (HW + 1) * U * xv.abs().mean(1) + U * ref.abs()
+    err = (y.double() - ref).abs()                              # NaN fails
+    print("  avgpool_split [%d, %d, %d] scale 2^%d: max err %.3e, worst err / bar %.3f"
+          % (N, HW, C, -int(math.log2(float(x_sc[1]))), float(err.max()), float((err / bar).max())))
+    assert bool((err <= bar).all())
+
+
+def _check_avgpool_bwd(dev, N, HW, C, accumulate):
+    """epb_avgpool_bwd bit-exact against fp32 dx + dy / HW (accumulate) or dy / HW restated in
+    numpy: the kernel's one IEEE division and one add, in that order (no product to contract, and
+    the build does not use fast-math); every element written, a guard band untouched.  Then the
+    fp32 engine's epb_avgpool forward over the same [N, HW, C] against float64: a sequential fp32
+    sum of HW terms and one division, within HW u mean|x|."""
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(103 + HW + C + accumulate)
+    dy = torch.randn(N, C, device=dev, generator=g) * 1e-3
+    dx0 = torch.randn(N, HW, C, device=dev, generator=g) * 1e-4
+    dx, guard = _guarded((N, HW, C), dev, float("nan"))
+    guard.fill_(1234.5)
+    if accumulate:
+        dx.copy_(dx0)
+    ops.avgpool_bwd(dy, dx, N, HW, C, accumulate)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    q = dy.cpu().numpy() / np.float32(HW)
+    ref = dx0.cpu().numpy() + q[:, None, :] if accumulate else np.broadcast_to(q[:, None, :], (N, HW, C))
+    assert ref.dtype == np.float32
+    got = dx.cpu().numpy()
+    same = got.view(np.int32) == np.ascontiguousarray(ref).view(np.int32)
+    # the fp32 forward
+    x = torch.randn(N, HW, C, device=dev, generator=g)
+    y, guard = _guarded((N, C), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.avgpool(x, y, N, HW, C)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "forward guard band overwritten"
+    xd = x.double()
+    err = (y.double() - xd.mean(1)).abs()
+    bar = HW * U * xd.abs().mean(1)
+    print("  avgpool_bwd [%d, %d, %d] accumulate %d: %d of %d elements differ; avgpool fwd worst err / bar %.3f"
+          % (N, HW, C, accumulate, int((~same).sum()), same.size, float((err / bar).max())))
+    assert bool(same.all())
+    assert bool((err <= bar).all())
+
+
+def hm_grid(R, HW):
+    """epb_heatmap_joint_loss's launch: (CTAs, trips of the slowest thread): quads of 4 elements
+    when HW % 4 == 0 (main loop of four quads per trip, then single quads), else single elements"""
+    work = -(-(R * HW) // 4)
+    blocks = min(-(-work // HM_THREADS), HM_MAX_BLOCKS)
+    per = R * HW // 4 if HW % 4 == 0 else R * HW
+    return blocks, -(-per // (blocks * HM_THREADS))
+
+
+def hm_loss_ref_bar(hm, tg, wr, x, t, w, R, HW, div):
+    """float64 heat-map MSE + L1 joint loss with hm_scale = jt_scale = 1, and the bars of the
+    kernel's partition: (L_hm, L_jt, L_tot, dhm, dx, bars {hm, jt, tot, dhm, dx}).  hm / tg [R, HW],
+    wr [R] (the weight multiplies the difference, so it enters the loss squared).
+
+    Heat-map part: d = wr (h - g) rounds twice, d^2 once (5u relative per element).  With quads
+    (HW % 4 == 0) the four squares of a quad add in a two-level tree, each thread adds its quads in
+    fp32 over q trips (hm_grid): 7 + q roundings on every term; per element (HW % 4 != 0) the
+    squares add in double.  The per-thread partials then add in double (depth < 64) and L_hm
+    rounds to fp32: |d L_hm| <= ((7 + q) u + 64 2^-53) L_hm + u L_hm.  Joint part: |x - t| and
+    the product with w round once each, the sum is in double (depth < 256): |d L_jt| <= (2u +
+    256 2^-53) sum|l w| / div + u L_jt; the total adds them in fp32: + u |L_tot|.
+    dhm = gs wr d with gs = 2 / (R HW) (1 / (R HW) rounds once; R HW < 2^24 is exact): the
+    reciprocal, gs wr, d (two) and the product: 5 roundings, (5 + 1e-5) u |dhm|.  dx = sign(x - t)
+    w / div: the sign of the fp32 difference is exact, so one rounding at most, u |dx|."""
+    h, g, wr = hm.double(), tg.double(), wr.double().view(R, 1)
+    d = wr * (h - g)
+    total = R * HW
+    L_hm = float((d * d).sum()) / total
+    _, q = hm_grid(R, HW)
+    depth = 7 + q if HW % 4 == 0 else 5
+    dj = x.double() - t.double()
+    lw = dj.abs() * w.double()
+    L_jt = float(lw.sum()) / div
+    L_tot = L_hm + L_jt
+    bars = {"hm": (depth * U + 64 * 2.0 ** -53) * L_hm + U * L_hm,
+            "jt": (2 * U + 256 * 2.0 ** -53) * L_jt + U * L_jt}
+    bars["tot"] = bars["hm"] + bars["jt"] + U * L_tot
+    dhm = 2.0 / total * wr * d
+    dx = torch.sign(dj) * w.double() / div
+    bars["dhm"] = (5 + 1e-5) * U * dhm.abs()
+    bars["dx"] = U * dx.abs()
+    return L_hm, L_jt, L_tot, dhm, dx, bars
+
+
+def hm_case(dev, N, J, H, W, D, seed):
+    """The C2(ii) objective's inputs on the device: heat-maps, Gaussian sigma = 2 targets and
+    visibility weights from golden_inputs.heatmap_case, the weights of the visible joints scaled
+    by dyadic factors in [1/4, 7/4] (so that a weight applied once instead of squared shows); the
+    joint part an L1 term on a depth_fc-shaped output [N, J D] against U(-0.5, 0.5) targets,
+    weights in {0, 1}."""
+    from tests import golden_inputs as gi
+    hm, tg, wh, _, _, _ = gi.heatmap_case(N, J, H, W, seed)
+    rng = np.random.default_rng(seed + 1)
+    wh = (wh * np.round(rng.uniform(0.25, 1.75, wh.shape) * 64) / 64).astype(np.float32)
+    n = N * J * D
+    x = (rng.standard_normal(n) * 0.5).astype(np.float32)
+    t = (rng.random(n) - 0.5).astype(np.float32)
+    w = (rng.random(n) > 0.1).astype(np.float32)
+    T = lambda a: torch.from_numpy(np.ascontiguousarray(a)).to(dev)
+    return T(hm), T(tg), T(wh.reshape(-1)), T(x), T(t), T(w)
+
+
+def run_hm_loss(case, N, J, H, W):
+    """one epb_heatmap_joint_loss launch (L1, hm_scale = jt_scale = 1, div = N): (loss [3], dhm, dx)"""
+    from epipolarpose_b200 import ops
+    hm, tg, wh, x, t, w = case
+    R, HW = N * J, H * W
+    loss = torch.empty(3, device=hm.device)
+    dhm = torch.full_like(hm, float("nan"))
+    dx = torch.full_like(x, float("nan"))
+    ops.heatmap_joint_loss(hm, tg, wh, R, HW, 1.0, x, t, w, x.numel(), 1, float(N), 1.0, loss, dhm, dx)
+    return loss, dhm, dx

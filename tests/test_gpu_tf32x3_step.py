@@ -45,9 +45,8 @@ import pytest
 import torch
 
 from tests import step_cases as sc
-from tests.step_cases import (C4_LAYERS_TF32X3, EPS, FPROP_BAR, KPIX, RUN_BLOCKS3, STATS_SELF_BAR, U, WGRAD_BAR,
-                              _act64, _all_three_pass, _emul_mma, _fwd64, _geoms, _guarded, _layer, _ran, _tc_bar,
-                              _tf32_np, _tf32_wgrad_plan, _trunc_np)
+from tests.step_cases import (C4_LAYERS_TF32X3, EPS, KPIX, RUN_BLOCKS3, U, WGRAD_BAR, _emul_mma, _guarded,
+                              _tc_bar, _tf32_np, _tf32_wgrad_plan, _trunc_np)
 
 gpu = pytest.mark.gpu
 
@@ -56,18 +55,11 @@ ROWS_PER_THREAD = 64                             # bn.cu kRowsPerThread
 
 
 def _wgrad_runs(layer, N=NB):
-    """(pixels N Hp Wp, Cin, Cout, taps) of each wgrad geometry of a C4_LAYERS_TF32X3 row: one for a
-    convolution, one per output phase (2 x 2, 4 taps each) for the 4 x 4 / 2 deconvolutions"""
-    _, kind, cin, cout, k, s, p, hw, _, _ = layer
-    if kind == "conv":
-        ho = (hw + 2 * p - k) // s + 1
-        return [(N * ho * ho, cin, cout, k * k)]
-    return [(N * hw * hw, cin, cout, 4)] * 4
+    return sc.tf32_wgrad_runs(layer, N)
 
 
 def _wgrad_run(layer):
-    """the longest pixel run of one CTA over the layer's wgrad geometries"""
-    return max(_tf32_wgrad_plan(M, ci, co, T, 3)[0] for M, ci, co, T in _wgrad_runs(layer))
+    return sc.tf32_wgrad_run(layer, NB)
 
 
 def test_c4_layer_table_wgrad_runs():
@@ -398,126 +390,7 @@ def test_tf32x3_conv_layers_vs_float64(dev, layer):
     or added into the block's input gradient for a downsample) and wgrad (into a zeroed dW) at
     N = 128 with the step's operand mode, each against torch float64 within its bar; every
     output followed by a guard band, every kernel a three-pass instantiation."""
-    import torch.nn.functional as F
-    from epipolarpose_b200 import ops
-    name, kind, cin, cout, k, s, p, hw, operand, dmode = layer
-    N = NB
-    final = name.startswith("final")
-    conv, Ho, Wo, x, sc, sh, w, gout = _layer(dev, kind, cin, cout, k, s, p, 0, N, hw, hw, 17)
-    ci, co, T = conv.cin_p, conv.cout_p, k * k
-    act = operand == "act"
-    aff = (sc, sh) if act else (None, None)
-    wf, wd = conv.pack(ops, w)
-    tags, errs = set(), {}
-    # ---- fprop
-    bias = torch.randn(co, device=dev, generator=torch.Generator(device=dev).manual_seed(5)) * 0.5 if final else None
-    geoms = conv.fprop_geoms(ops, N, hw, hw, 3)
-    gms = _geoms(geoms, int(act), 0)
-    out, guard = _guarded((N, Ho, Wo, co), dev, 0.0 if any(gm is None for gm in geoms) else float("nan"))
-    guard.fill_(1234.5)
-    stats = sguard = None
-    if not final:
-        sbuf = torch.zeros(2 * co + 64, device=dev, dtype=torch.float64)
-        stats, sguard = sbuf[:2 * co], sbuf[2 * co:]
-
-    def fwd(o, st):
-        for gm in gms:
-            ops.conv_fprop(gm, x, wf, o, aff[0], aff[1], bias, st)
-    tags |= _ran(lambda: fwd(out.clone(), None if stats is None else stats.clone()))
-    fwd(out, stats)
-    torch.cuda.synchronize()
-    assert bool((guard == 1234.5).all()), "fprop guard band overwritten"
-    a64 = _act64(x, *aff, act)
-    with torch.no_grad():
-        ref = _fwd64(conv, a64, w.double())
-        if bias is not None:
-            ref += bias.double()[None, :, None, None]
-        ref = ref.permute(0, 2, 3, 1)
-        bar_f = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in gms), 3)
-        errs["fprop"] = float((out.double() - ref).abs().max() / ref.abs().max())   # NaN fails
-        if stats is not None:
-            assert bool((sguard == 0).all()), "statistics guard band overwritten"
-            o = out.double().reshape(-1, co)
-            s1, s2 = stats[:co], stats[co:]
-            errs["st_self"] = max(float(((s1 - o.sum(0)).abs() / o.abs().sum(0).clamp_min(1e-300)).max()),
-                                  float(((s2 - (o * o).sum(0)).abs() / (o * o).sum(0).clamp_min(1e-300)).max()))
-            del o
-            r = ref.reshape(-1, co)
-            r2 = (r * r).sum(0)
-            errs["st_ref"] = max(float(((s1 - r.sum(0)).abs() / r.abs().sum(0).clamp_min(1e-300)).max()),
-                                 float((s2 - r2).abs().max() / r2.abs().max()))
-            del r, r2
-    del out, ref
-    # ---- dgrad
-    bar_d = None
-    if dmode is not None:
-        dgeoms = conv.dgrad_geoms(ops, N, hw, hw, 3)
-        acc = int(dmode == "acc")
-        dgms = _geoms(dgeoms, 0, acc)
-        with torch.no_grad():
-            g64, w64 = gout.permute(0, 3, 1, 2).double(), w.double()
-            if kind == "conv":
-                ref = torch.nn.grad.conv2d_input((N, ci, hw, hw), w64, g64, s, p)
-            else:
-                ref = F.conv2d(g64, w64, None, s, p)
-            del g64
-            ref = ref.permute(0, 2, 3, 1)
-        din, guard = _guarded((N, hw, hw, ci), dev, 0.0 if (acc or any(gm is None for gm in dgeoms)) else float("nan"))
-        guard.fill_(1234.5)
-        init = None
-        if acc:
-            init = torch.randn(din.shape, device=dev, generator=torch.Generator(device=dev).manual_seed(9))
-            init *= float(ref.abs().max()) / 3
-            din.copy_(init)
-
-        def bwd(o):
-            for gm in dgms:
-                ops.conv_fprop(gm, gout, wd, o, None, None, None, None)
-        tags |= _ran(lambda: bwd(din.clone()))
-        bwd(din)
-        torch.cuda.synchronize()
-        assert bool((guard == 1234.5).all()), "dgrad guard band overwritten"
-        base = init.double() if init is not None else 0.0
-        errs["dgrad"] = float((din.double() - (base + ref)).abs().max() / ref.abs().max())
-        bar_d = _tc_bar(FPROP_BAR, max(gm.T * gm.Cin for gm in dgms), 3)
-        del din, ref, init
-    # ---- wgrad
-    runs = sorted((gm.N * gm.Hp * gm.Wp, gm.Cin, gm.Cout, gm.T) for gm in gms)
-    assert runs == sorted((M, _pad4(a), _pad4(b), t) for M, a, b, t in _wgrad_runs(layer)), runs
-    R = _wgrad_run(layer)
-    bar_w = _tc_bar(WGRAD_BAR, R, 3)
-    w64 = w.double().requires_grad_(True)
-    _fwd64(conv, a64, w64).backward(gout.permute(0, 3, 1, 2).double())
-    del a64
-    gw = w64.grad
-    ref = (gw.permute(0, 2, 3, 1) if kind == "conv" else gw.permute(1, 2, 3, 0)).reshape(co, T, ci)
-    del w64, gw
-    dw, guard = _guarded((co * T * ci,), dev, 0.0)
-    guard.fill_(1234.5)
-
-    def wgr(o):
-        for gm in gms:
-            ops.conv_wgrad(gm, x, gout, o, aff[0], aff[1])
-    tags |= _ran(lambda: wgr(torch.zeros_like(dw)))
-    wgr(dw)
-    torch.cuda.synchronize()
-    assert bool((guard == 1234.5).all()), "dW guard band overwritten"
-    errs["wgrad"] = float((dw.view(co, T, ci).double() - ref).abs().max() / ref.abs().max())
-    print("  %-22s %-36s fprop %.2e (bar %.2e)%s%s wgrad %.2e (run %d, bar %.2e)" % (
-        name, ",".join(sorted(tags)), errs["fprop"], bar_f,
-        " stats %.1e / %.1e" % (errs["st_self"], errs["st_ref"]) if "st_self" in errs else "",
-        " dgrad %.2e (bar %.2e)" % (errs["dgrad"], bar_d) if bar_d else "", errs["wgrad"], R, bar_w))
-    assert _all_three_pass(tags), tags
-    assert errs["fprop"] <= bar_f, errs
-    if "st_self" in errs:
-        assert errs["st_self"] <= STATS_SELF_BAR and errs["st_ref"] <= bar_f, errs
-    if bar_d is not None:
-        assert errs["dgrad"] <= bar_d, errs
-    assert errs["wgrad"] <= bar_w, errs
-
-
-def _pad4(c):
-    return (c + 3) // 4 * 4
+    sc.check_tf32x3_layer(dev, layer, NB)
 
 
 @gpu

@@ -112,6 +112,37 @@ FP32_ENGINE = {"epb_nchw_to_nhwc", "epb_im2col", "epb_conv_fprop", "epb_conv_wgr
                "epb_softargmax_bwd", "epb_colsum"}
 
 COVERAGE_ROBUST = dict(COVERAGE, epb_tuple_labels=["test_gpu_tuple_labels.py::test_kernel_vs_restatement"])
+COVERAGE_RELPOSE = dict(COVERAGE, epb_relative_pose=["test_gpu_relpose.py::test_relative_pose_kernel_matches_oracle"])
+
+S = "test_gpu_c2_flat_step.py::"
+COVERAGE_C2FLAT = {
+    "epb_im2col_split": [S + "test_c2_im2col_split_bit_exact_at_stem"],
+    "epb_conv16_fprop": [S + "test_c2_conv16_layers_vs_torch_float64", S + "test_c2_final_conv16_fprop_vs_float64",
+                         S + "test_c2_conv16_stats_vs_float64"],
+    "epb_conv16_wgrad": [S + "test_c2_conv16_layers_vs_torch_float64"],
+    "epb_bn_finalize_scale": [S + "test_c2_bn_finalize_scale_vs_float64"],
+    "epb_bn_finalize": [S + "test_c2_bn_finalize_vs_float64"],
+    "epb_bn_act_split": [S + "test_c2_bn_act_split_vs_float64"],
+    "epb_bn_relu_maxpool_split": [S + "test_c2_bn_relu_maxpool_split_vs_float64"],
+    "epb_maxpool_bwd": [S + "test_c2_maxpool_bwd_vs_float64"],
+    "epb_bn_bwd_split": [S + "test_c2_bn_bwd_split_vs_float64"],
+    "epb_avgpool_split": [S + "test_c2_avgpool_split_vs_float64"],
+    "epb_avgpool_bwd": [S + "test_c2_avgpool_bwd_bit_exact"],
+    "epb_conv_fprop": [S + "test_c2_head_tf32x3_vs_float64"],
+    "epb_conv_wgrad": [S + "test_c2_head_tf32x3_vs_float64"],
+    "epb_colsum": [S + "test_c2_colsum_vs_float64"],
+    "epb_nhwc_to_nchw": [S + "test_c2_heatmap_layout_bit_exact"],
+    "epb_nchw_to_nhwc": [S + "test_c2_heatmap_layout_bit_exact"],
+    "epb_heatmap_joint_loss": [S + "test_c2_heatmap_joint_loss_vs_float64",
+                               S + "test_c2_heatmap_loss_repeatable_across_grid_sizes"],
+    "epb_split16_batch": [S + "test_c2_split16_batch_bit_exact_on_model_jobs"],
+    "epb_pack_weight_batch": [S + "test_c2_pack_weight_batch_bit_exact_on_model_jobs"],
+    "epb_adam_step_dev": [S + "test_c2_fused_adam_vs_float64_on_model_buffer"],
+}
+# the VOLUME=False head: entries the C4 step does not call
+HEAD_C2FLAT = {"epb_avgpool_split", "epb_avgpool_bwd", "epb_heatmap_joint_loss", "epb_conv_fprop", "epb_conv_wgrad",
+               "epb_colsum"}
+GEOMETRY = {"epb_patch_to_image", "epb_triangulate", "epb_project_labels", "epb_relative_pose", "epb_tuple_labels"}
 
 
 def _missing_coverage(recorded, table):
@@ -183,7 +214,8 @@ def _fp32_engine(eng):
 
 # ------------------------------------------------------------------ steps
 def _eager_step(dev, row):
-    """GraphedTrainStep(online=True).eager_step on the bench's cameras, FusedAdam, SmoothL1"""
+    """GraphedTrainStep(online=True).eager_step on the bench's cameras, FusedAdam, SmoothL1; with
+    the row's estimate_extrinsics, the cameras' extrinsics estimated from the predicted joints"""
     import lib.models as models
     import lib.core.integral_loss as il
     import lib.core.function as fn
@@ -191,13 +223,75 @@ def _eager_step(dev, row):
     import lib.utils.utils as Ut
     layers, J, D, HW, tuples = row["device"]
     B = 4 * tuples
+    est = row.get("estimate_extrinsics", False)
     torch.manual_seed(0)
     m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW), False, precision=row["precision"]).to(dev).train()
     opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method=row["method"])
-    meta = iu.pack_meta({k: v.to(dev) for k, v in sc._bench_meta(tuples).items()}, B, dev)
+    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J).to(dev), opt, online=True, method=row["method"],
+                               estimate_extrinsics=est)
+    meta = iu.pack_meta({k: v.to(dev) for k, v in sc._bench_meta(tuples).items()}, B, dev, estimate_extrinsics=est)
     x = torch.randn(B, 3, HW, HW, device=dev)
     return m, lambda: step.eager_step(x, None, None, meta)
+
+
+def _flat_step(dev, row, shape, ops=None):
+    """The VOLUME=False step, eager: forward to (heat-maps, depth_fc output), HeatmapJointLoss
+    (L1; Gaussian targets and visibility weights of golden_inputs.heatmap_case, U(-0.5, 0.5)
+    depth targets), backward, FusedAdam.step().  shape: (layers, J, D, image size, images)."""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.utils.utils as Ut
+    from tests import golden_inputs as gi
+    layers, J, D, HW, B = shape
+    torch.manual_seed(0)
+    m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW, volume=False), False, ops=ops,
+                                          precision=row["precision"]).to(dev).train()
+    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    crit = il.HeatmapJointLoss(J, kind="l1")
+    _, tg, wh, _, _, _ = gi.heatmap_case(B, J, HW // 4, HW // 4, 5)
+    g = torch.Generator().manual_seed(1)
+    x = torch.randn(B, 3, HW, HW, generator=g).to(dev)
+    t = (torch.rand(B, J * D, generator=g) - 0.5).to(dev)
+    w = torch.ones(B, J * D, device=dev)
+    tg, wh = torch.from_numpy(tg).to(dev), torch.from_numpy(wh).to(dev)
+
+    def run():
+        loss = crit(m(x), tg, t, w, hm_weight=wh)
+        loss.backward()
+        opt.step()
+        return loss.detach()
+    return m, run
+
+
+def _flat_device_step(dev, row):
+    layers, J, D, HW, tuples = row["device"]
+    return _flat_step(dev, row, (layers, J, D, HW, 4 * tuples))
+
+
+def _emulated_graphed_step(row):
+    """GraphedTrainStep.eager_step with given labels (R18 trunk or the row's, its J and D, 2 tuples
+    x 4 views of 64 x 64), SmoothL1JointLocationLoss, FusedAdam, on the emulated ABI"""
+    import lib.models as models
+    import lib.core.integral_loss as il
+    import lib.core.function as fn
+    import lib.utils.utils as Ut
+    from tests import emul_ops
+    layers, J, D, HW = row["emulated"]
+    B = 8
+    torch.manual_seed(0)
+    m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW), False, ops=emul_ops,
+                                          precision=row["precision"]).train()
+    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
+    g = torch.Generator().manual_seed(1)
+    return m, lambda: step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
+                                      torch.ones(B, J * 3), None)
+
+
+def _emulated_flat_step(row):
+    from tests import emul_ops
+    layers, J, D, HW = row["emulated"]
+    return _flat_step(torch.device("cpu"), row, (layers, J, D, HW, 4), ops=emul_ops)
 
 
 def _graphed_step(dev, row):
@@ -225,16 +319,19 @@ def _graphed_step(dev, row):
 COMPOSITIONS = {
     "c4_f16x3": dict(
         table=COVERAGE, precision="f16x3", method="iterative", views=4, driver=_eager_step,
+        emulated_driver=_emulated_graphed_step,
         emulated=(18, 16, 64, 64), device=(18, 16, 64, 256, 2),
         calls={"epb_adam_step_dev", "epb_split16_batch"}, online={"epb_triangulate"}, not_called=set(),
         engine=None, tags=None),
     "c5": dict(
         table=COVERAGE_C5, precision="f16x3", method="iterative", views=4, driver=_eager_step,
+        emulated_driver=_emulated_graphed_step,
         emulated=(18, 17, 96, 64), device=(101, 17, 96, 384, 2),
         calls=HEAD_C5 | {"epb_adam_step_dev"}, online={"epb_triangulate"}, not_called={"epb_softargmax_bwd_split"},
         engine=lambda eng: not eng.takes_logit_sink(), tags=None),
     "c4_tf32x3": dict(
         table=COVERAGE_TF32X3, precision="tf32x3", method="iterative", views=4, driver=_eager_step,
+        emulated_driver=_emulated_graphed_step,
         emulated=(18, 16, 64, 64), device=(50, 16, 64, 256, 2),
         calls=FP32_ENGINE | {"epb_adam_step_dev"}, online={"epb_triangulate"},
         not_called=lambda e: e.endswith("_split") or "conv16" in e,
@@ -243,6 +340,19 @@ COMPOSITIONS = {
         table=COVERAGE_ROBUST, precision="f16x3", method="robust", views=4, driver=_graphed_step,
         emulated=None, device=(18, 16, 64, 256, 2),
         calls=set(), online={"epb_tuple_labels"}, not_called={"epb_triangulate"},
+        engine=None, tags=None),
+    # MODEL.VOLUME: false (SURVEY 8(d) C2(ii)); emulated on R50, since depth_fc takes 2048 inputs
+    "c2_flat": dict(
+        table=COVERAGE_C2FLAT, precision="f16x3", method=None, views=4, driver=_flat_device_step,
+        emulated_driver=_emulated_flat_step, emulated=(50, 17, 4, 64), device=(50, 17, 64, 256, 2),
+        calls=HEAD_C2FLAT | {"epb_adam_step_dev"}, online=set(),
+        not_called=lambda e: e.startswith("epb_softargmax_") or e == "epb_jointloss_fwd_bwd" or e in GEOMETRY,
+        engine=lambda eng: type(eng).__name__ == "Engine16" and not eng.takes_logit_sink(), tags=None),
+    # TRAIN.ESTIMATE_EXTRINSICS: each view pair's relative pose from the predicted joints
+    "c4_relpose": dict(
+        table=COVERAGE_RELPOSE, precision="f16x3", method="iterative", views=4, driver=_eager_step,
+        estimate_extrinsics=True, emulated=None, device=(18, 16, 64, 256, 2),
+        calls=set(), online={"epb_relative_pose"}, not_called={"epb_tuple_labels"},
         engine=None, tags=None),
 }
 EMULATED = [k for k, row in COMPOSITIONS.items() if row["emulated"] is not None]
@@ -284,28 +394,16 @@ def test_gate_has_teeth(comp):
 
 @pytest.mark.parametrize("comp", EMULATED)
 def test_gate_emulated_step(comp):
-    """One training step of the composition (R18 trunk, its J and D, 2 tuples x 4 views of 64 x 64)
-    through the emulated ABI: GraphedTrainStep.eager_step with given labels,
-    SmoothL1JointLocationLoss, FusedAdam.  Every entry it calls has a row naming existing tests."""
-    import lib.models as models
-    import lib.core.integral_loss as il
-    import lib.core.function as fn
-    import lib.utils.utils as Ut
-    from tests import emul_ops
+    """One training step of the composition through the emulated ABI, by the row's emulated
+    driver: GraphedTrainStep.eager_step with given labels, SmoothL1JointLocationLoss and FusedAdam
+    (R18 trunk, its J and D, 2 tuples x 4 views of 64 x 64), or the VOLUME=False step (R50, 4
+    images).  Every entry it calls has a row naming existing tests."""
     row = COMPOSITIONS[comp]
-    layers, J, D, HW = row["emulated"]
-    B = 8
     with _emulated_abi() as rec:
-        torch.manual_seed(0)
-        m = models.pose3d_resnet.get_pose_net(sc._cfg(layers, J, D, HW), False, ops=emul_ops,
-                                              precision=row["precision"]).train()
+        m, run = row["emulated_driver"](row)
         if row["engine"] is not None:
             assert row["engine"](m._engine())
-        opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
-        step = fn.GraphedTrainStep(m, il.SmoothL1JointLocationLoss(J), opt, online=False)
-        g = torch.Generator().manual_seed(1)
-        loss = step.eager_step(torch.randn(B, 3, HW, HW, generator=g), torch.rand(B, J * 3, generator=g) - 0.5,
-                               torch.ones(B, J * 3), None)
+        loss = run()
         assert math.isfinite(float(loss))
     _check_calls(row, rec, row["calls"], "emulated %s step" % comp)
 
