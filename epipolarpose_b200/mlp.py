@@ -79,6 +79,11 @@ class MLPEngine:
         p = params
         if C != c_real:                       # padded columns: gamma 1 / beta 0 / stats untouched
             raise ValueError("BatchNorm1d width %d must be a multiple of 4" % c_real)
+        if training and N == 1:
+            # torch.nn.BatchNorm1d refuses a one-row training batch (the reference's loop stops on
+            # a last batch of 1); bn_finalize would map it to a zero variance and every output to beta
+            raise ValueError("Expected more than 1 value per channel when training, got input size %s"
+                             % (tuple(z.shape),))
         st = eng._bn_train(name, C, stats, N, p, None) if training else eng._bn_eval(name, C, p)
         a = torch.empty_like(z)
         ops.bn_act(z, st.scale, st.shift, None, None, None, 1, a, N, C)

@@ -1,6 +1,6 @@
 """Shared by the training-step tests (test_gpu_step_kernels, test_gpu_c5_step, test_gpu_tf32x3_step,
-test_gpu_c2_flat_step, test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32, test_gpu_predictor, test_gpu_conv16_store and
-test_step_coverage): the float64 check bodies each composition runs at its own sizes, the bars and
+test_gpu_c2_flat_step, test_gpu_refiner_step, test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32,
+test_gpu_predictor, test_gpu_conv16_store and test_step_coverage): the float64 check bodies each composition runs at its own sizes, the bars and
 the emulations they rest on, the restated planners, the layer tables, the device data makers and
 one cache of models and conv outputs keyed by composition.
 
@@ -169,6 +169,11 @@ def _tf32_np(x):
     """round to nearest TF32, ties away from zero (tc::to_tf32), in an fp32 container"""
     u = np.asarray(x, dtype=np.float32).view(np.uint32)
     return ((u + np.uint32(0x1000)) & np.uint32(0xffffe000)).view(np.float32)
+
+
+def _tf32(t):
+    """_tf32_np for a float32 torch tensor (int32 wrap-around == the unsigned add)"""
+    return ((t.contiguous().view(torch.int32) + 0x1000) & -8192).view(torch.float32)
 
 
 def _trunc_np(x):
@@ -1206,12 +1211,11 @@ def check_bn_finalize_scale(dev, M):
         assert _scale_ok(s, bound, _act_rule) and abs(float(out["sc"][2]) - bound) <= 1e-6 * bound
 
 
-def check_bn_finalize(dev, M):
+def check_bn_finalize(dev, M, C=256):
     """epb_bn_finalize (the layers whose post-activation scale comes from elsewhere): every output
     within 1 fp32 ulp of float64 on the same statistics, gamma < 0 and = 0 channels, constant
-    channels, running statistics."""
+    channels, running statistics (unbiased, momentum) over C channels."""
     from epipolarpose_b200 import ops
-    C = 256
     rng = np.random.default_rng(M + 1)
     mean = rng.standard_normal(C) * 3
     var = rng.uniform(0.01, 4, C)
@@ -1233,7 +1237,7 @@ def check_bn_finalize(dev, M):
         u = _ulps(t.cpu().numpy(), ref[k])
         worst = max(worst, float(u.max()))
         assert u.max() <= 1, "%s: %.2f ulp at channel %d" % (k, u.max(), u.argmax())
-    print("  bn_finalize M %d: worst %.2f ulp" % (M, worst))
+    print("  bn_finalize M %d C %d: worst %.2f ulp" % (M, C, worst))
 
 
 def _apply_bar(zd, scd, shd, res_terms, ymax):
@@ -1464,6 +1468,151 @@ def check_bn_bwd_split(dev, M, C, mode):
     assert _no_clamp(dz) and s * dzmax < HALF_MAX
 
 
+# ------------------------------------------------------------------ the fp32 BatchNorm chain (bn.cu)
+ROWS_PER_THREAD = 64                             # bn.cu kRowsPerThread
+
+
+def _bn_stats64(x):
+    """float64 batch mean and invstd of x [M, C] (the fp32 eps, as bn_finalize adds it)"""
+    xd = x.double()
+    mu = xd.mean(0)
+    var = (xd - mu).pow(2).mean(0)
+    return mu, 1 / torch.sqrt(var + float(np.float32(EPS)))
+
+
+def _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv):
+    """float64 BatchNorm backward of g = dy * keep on x [M, C] with batch statistics (mu, inv),
+    and the bars of bn_bwd_reduce + bn_bwd_apply: (dbeta, dgamma, dx, bar_b, bar_g, bar_dx).
+
+    Each thread adds kRowsPerThread = 64 rows in fp32, the CTA's row slots and all CTAs add in
+    double, so with d = 64 + 2, |d dbeta| <= d u sum|g| and |d dgamma| <= (d + 1) u sum|g xhat| +
+    sum|g| e_xhat, where e_xhat = 4u (|xhat| + |mean| invstd) is the error of the fp32 xhat formed
+    from the fp32 mean and invstd.  dgamma and dbeta then round once to fp32 (_bn_bwd_ratios).
+    Not from max|dgamma|: dgamma cancels.  k0 = gamma invstd, k1 = sum g / M, k2 = sum g xhat / M
+    round to fp32, and dx = k0 (g - k1 - xhat k2) takes four more roundings: |d dx| <= |gamma
+    invstd| (4u (|g| + |k1| + |xhat k2|) + bar_b / M + |xhat| bar_g / M + |k2| e_xhat) + 2u |dx|."""
+    M = x.shape[0]
+    g = dy.double() * keep
+    xh = (x.double() - mu) * inv
+    sg, sgx = g.sum(0), (g * xh).sum(0)
+    d = ROWS_PER_THREAD + 2
+    ag = g.abs()
+    e_xh = 4 * U * (xh.abs() + mu.abs() * inv)
+    bar_b = d * U * ag.sum(0)
+    bar_g = (d + 1) * U * (ag * xh.abs()).sum(0) + (ag * e_xh).sum(0)
+    k1, k2 = sg / M, sgx / M
+    a = gamma.double() * inv
+    dx = a * (g - k1 - xh * k2)
+    bar = a.abs() * (4 * U * (ag + k1.abs() + (xh * k2).abs()) + bar_b / M + xh.abs() * (bar_g / M)
+                     + k2.abs() * e_xh) + 2 * U * dx.abs()
+    return sg, sgx, dx, bar_b, bar_g, bar
+
+
+def _bn_bwd_ratios(dbeta, dgamma, dx, ref):
+    """worst err / bar of dbeta, dgamma (each after its one fp32 rounding) and dx"""
+    sg, sgx, dx64, bar_b, bar_g, bar = ref
+    eb = ((dbeta.double() - sg).abs() - U * sg.abs()).clamp_min(0) / (bar_b + 1e-300)   # a fully masked
+    eg = ((dgamma.double() - sgx).abs() - U * sgx.abs()).clamp_min(0) / (bar_g + 1e-300)  # channel: 0 / 0
+    ex = (dx.double() - dx64).abs() / (bar + 1e-300)
+    return float(eb.max()), float(eg.max()), float(ex.max())
+
+
+def check_bn_bwd(dev, M, C, mode):
+    """bn_bwd_reduce + bn_bwd_apply over M x C against float64 within _bn_bwd_ref_bar: dbeta,
+    dgamma per channel and dx per element, with a constant channel (invstd = 316), one huge
+    gradient element and a fully masked channel beside ordinary ones.  mode "y_out": g is dy
+    masked by y_out > 0; "relu": by the BatchNorm's own ReLU, fma(z, scale, shift) > 0, whose sign
+    the float64 z scale + shift gives exactly, so the reference masks alike."""
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(M + C)
+    x = torch.randn(M, C, device=dev, generator=g) * (torch.rand(C, device=dev, generator=g) * 2 + 0.2) \
+        + torch.randn(C, device=dev, generator=g) * 2
+    x[:, 0] = 0.37                                           # var 0: invstd = 1 / sqrt(eps)
+    dy = (torch.randn(M, C, device=dev, generator=g) + torch.randn(C, device=dev, generator=g) * 0.5) * 1e-4
+    dy[M // 2, 1] = 3.0                                      # one huge element
+    gamma = torch.rand(C, device=dev, generator=g) + 0.5
+    beta = torch.randn(C, device=dev, generator=g) * 0.1
+    mu, inv = _bn_stats64(x)
+    mean, invstd = mu.float(), inv.float()
+    scale, shift = (gamma.double() * inv).float(), (beta.double() - mu * gamma.double() * inv).float()
+    y_out = None
+    if mode == "relu":
+        scale[2], shift[2] = 0.0, -1.0                       # a fully masked channel
+        keep = (x.double() * scale.double() + shift.double()) > 0
+    else:
+        y_out = torch.relu(torch.randn(M, C, device=dev, generator=g))
+        y_out[:, 2] = 0
+        keep = y_out > 0
+    relu = int(mode == "relu")
+    sums = torch.zeros(2 * C, device=dev, dtype=torch.float64)
+    dx, dg, db = torch.empty(M, C, device=dev), torch.empty(C, device=dev), torch.empty(C, device=dev)
+    ops.bn_bwd_reduce(dy, x, y_out, scale, shift, mean, invstd, relu, M, C, sums)
+    ops.bn_bwd_apply(dy, x, y_out, scale, shift, mean, invstd, gamma, relu, sums, M, C, dx, dg, db)
+    torch.cuda.synchronize()
+    del y_out
+    ref = _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv)
+    rb, rg, rx = _bn_bwd_ratios(db, dg, dx, ref)
+    print("  bn bwd %7d x %-4d %-5s worst err / bar: dbeta %.3f dgamma %.3f dx %.3f (max dx err %.2e)"
+          % (M, C, mode, rb, rg, rx, float((dx.double() - ref[2]).abs().max())))
+    assert rb <= 1.0 and rg <= 1.0 and rx <= 1.0
+
+
+def _bn_act_ref_bar(x, s, b, r, rs, rb):
+    """float64 x s + b (+ r rs + rb, or + r) and the bar 4u on its terms: bn_act computes y =
+    relu(fma(x, s, b) + q), q = fma(r, rs, rb), r or 0, three roundings on the terms"""
+    xd = x.double()
+    t = xd * s.double() + b.double()
+    terms = (xd * s.double()).abs() + b.double().abs()
+    if r is not None:
+        rd = r.double()
+        if rs is not None:
+            t = t + rd * rs.double() + rb.double()
+            terms = terms + (rd * rs.double()).abs() + rb.double().abs()
+        else:
+            t = t + rd
+            terms = terms + rd.abs()
+    return t, 4 * U * terms
+
+
+def _bn_act_check(y, t, bar):
+    """(worst |y - relu(t)| / bar, elements below -bar that are not exactly 0, negative y)"""
+    err = (y.double() - t.clamp_min(0)).abs()
+    dead = t < -bar
+    return (float((err / (bar + 1e-300)).max()), int((dead & (y != 0)).sum()), int((y < 0).sum()))
+
+
+def check_bn_act(dev, M, C, res):
+    """bn_act with ReLU over M x C: the residual with the downsample BatchNorm's affine ("affine"),
+    the identity residual ("identity") or ReLU alone ("relu"); within _bn_act_ref_bar's 4u of the
+    terms, exactly 0 where the float64 value is below minus that bar, a guard band untouched."""
+    from epipolarpose_b200 import ops
+    g = torch.Generator(device=dev).manual_seed(M + C + len(res))
+    x = torch.randn(M, C, device=dev, generator=g) * 3 + 0.5
+    s, b = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
+    r = rs = rb = None
+    if res != "relu":
+        r = torch.randn(M, C, device=dev, generator=g) * 2
+        if res == "identity":
+            r = torch.relu(r)                                     # a block output
+        else:
+            rs, rb = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
+    y, guard = _guarded((M, C), dev, float("nan"))
+    guard.fill_(1234.5)
+    ops.bn_act(x, s, b, r, rs, rb, 1, y, M, C)
+    torch.cuda.synchronize()
+    assert bool((guard == 1234.5).all()), "guard band overwritten"
+    worst, bad0, neg = 0.0, 0, 0
+    step = max((1 << 24) // C, 1)
+    for r0 in range(0, M, step):
+        sl = slice(r0, r0 + step)
+        t, bar = _bn_act_ref_bar(x[sl], s, b, None if r is None else r[sl], rs, rb)
+        w_, z_, n_ = _bn_act_check(y[sl], t, bar)
+        worst, bad0, neg = max(worst, w_), bad0 + z_, neg + n_
+        del t, bar
+    print("  bn_act %6d x %-4d %-8s worst err / bar %.3f" % (M, C, res, worst))
+    assert worst <= 1.0 and bad0 == 0 and neg == 0, (worst, bad0, neg)
+
+
 # ------------------------------------------------------------------ conv16 at a layer shape
 def _check_conv16_layer(dev, layer, N, wgrad_bar):
     """conv16 fprop (with statistics), dgrad and wgrad of one layer over N images against torch
@@ -1555,7 +1704,7 @@ def tc_supported(gm, wgrad):
     return gm.Cin % 32 == 0 and gm.Cout % 32 == 0 and gm.Cout >= 32 and fits
 
 
-def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
+def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass, bias_stats=False):
     """3xTF32 fprop (statistics into a zeroed buffer, or the bias for a layer named final* or
     depth_fc*), dgrad (written, or added into the block's input gradient for a downsample) and
     wgrad (into a zeroed dW) of a C4_LAYERS_TF32X3-style row over N images with its operand mode,
@@ -1563,11 +1712,17 @@ def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
     longest taps x Cin of the call's geometries; wgrad _tc_bar(WGRAD_BAR, R, 3), R the pixel run
     of one CTA from the restated planner.  Every output followed by a guard band; the conv
     kernels that ran (_ran's tags) must meet `kernels`: by default every one a three-pass
-    instantiation.  kernels=None opens no profiler session: the caller shows which kernels run."""
+    instantiation.  kernels=None opens no profiler session: the caller shows which kernels run.
+
+    bias_stats: the bias (zero in the padding columns) and the statistics in the same fprop call,
+    as MLPEngine.linear makes it.  The kernels add the bias before they accumulate the sums, so
+    the sums must meet STATS_SELF_BAR against the kernel's own output and the fprop bar against
+    float64 x W^T + b; the same sums with the bias left out of the reference must miss that bar
+    by more than 100x (the check has teeth at these seeds); padding output columns are exactly 0."""
     import torch.nn.functional as F
     from epipolarpose_b200 import ops
     name, kind, cin, cout, k, s, p, hw, operand, dmode = layer
-    final = name.startswith(("final", "depth_fc"))
+    final = name.startswith(("final", "depth_fc")) and not bias_stats
     conv, Ho, Wo, x, sc, sh, w, gout = _layer(dev, kind, cin, cout, k, s, p, 0, N, hw, hw, 17)
     ci, co, T = conv.cin_p, conv.cout_p, k * k
     act = operand == "act"
@@ -1575,7 +1730,10 @@ def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
     wf, wd = conv.pack(ops, w)
     tags, errs = set(), {}
     # ---- fprop
-    bias = torch.randn(co, device=dev, generator=torch.Generator(device=dev).manual_seed(5)) * 0.5 if final else None
+    bias = torch.randn(co, device=dev, generator=torch.Generator(device=dev).manual_seed(5)) * 0.5 \
+        if final or bias_stats else None
+    if bias_stats:
+        bias[cout:] = 0
     geoms = conv.fprop_geoms(ops, N, hw, hw, 3)
     gms = _geoms(geoms, int(act), 0)
     out, guard = _guarded((N, Ho, Wo, co), dev, 0.0 if any(gm is None for gm in geoms) else float("nan"))
@@ -1612,7 +1770,16 @@ def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
             r2 = (r * r).sum(0)
             errs["st_ref"] = max(float(((s1 - r.sum(0)).abs() / r.abs().sum(0).clamp_min(1e-300)).max()),
                                  float((s2 - r2).abs().max() / r2.abs().max()))
+            if bias is not None:
+                r = r - bias.double()
+                r2n = (r * r).sum(0)
+                errs["st_nobias"] = max(float(((s1 - r.sum(0)).abs() / r.abs().sum(0).clamp_min(1e-300)).max()),
+                                        float((s2 - r2n).abs().max() / r2n.abs().max()))
+                del r2n
             del r, r2
+        if bias_stats and cout != co:
+            assert bool((out[..., cout:] == 0).all()), "padding output columns are not exactly zero"
+            assert bool((stats[cout:co] == 0).all() and (stats[co + cout:] == 0).all()), "padding statistics"
     del out, ref
     # ---- dgrad
     bar_d = None
@@ -1675,10 +1842,17 @@ def check_tf32x3_layer(dev, layer, N, kernels=_all_three_pass):
         name, ",".join(sorted(tags)), errs["fprop"], bar_f,
         " stats %.1e / %.1e" % (errs["st_self"], errs["st_ref"]) if "st_self" in errs else "",
         " dgrad %.2e (bar %.2e)" % (errs["dgrad"], bar_d) if bar_d else "", errs["wgrad"], R, bar_w))
+    if bias_stats:
+        print("  %-22s worst err / bar: fprop %.3f dgrad %.3f wgrad %.3f stats self %.3f ref %.3f; "
+              "stats without the bias %.3g" % (name, errs["fprop"] / bar_f, errs.get("dgrad", 0.0) / (bar_d or 1.0),
+                                               errs["wgrad"] / bar_w, errs["st_self"] / STATS_SELF_BAR,
+                                               errs["st_ref"] / bar_f, errs["st_nobias"] / bar_f))
     assert kernels is None or kernels(tags), tags
     assert errs["fprop"] <= bar_f, errs
     if "st_self" in errs:
         assert errs["st_self"] <= STATS_SELF_BAR and errs["st_ref"] <= bar_f, errs
+    if bias_stats:
+        assert errs["st_nobias"] > 100 * bar_f, errs
     if bar_d is not None:
         assert errs["dgrad"] <= bar_d, errs
     assert errs["wgrad"] <= bar_w, errs

@@ -26,17 +26,12 @@ import pytest
 import torch
 
 from tests.step_cases import (FPROP_BAR, STATS_SELF_BAR, WGRAD_BAR, _act64, _emul_mma, _fwd64, _geoms, _guarded,
-                              _layer, _ran, _tc_bar, _tf32_np, _trunc_np)
+                              _layer, _ran, _tc_bar, _tf32, _tf32_np, _trunc_np)
 
 gpu = pytest.mark.gpu
 
 
 # ------------------------------------------------------------------ operand rounding
-def _tf32(t):
-    """_tf32_np for a float32 torch tensor (int32 wrap-around == the unsigned add)"""
-    return ((t.contiguous().view(torch.int32) + 0x1000) & -8192).view(torch.float32)
-
-
 def _relerr(a, ref):
     a, ref = a.double(), ref.double()
     return float((a - ref).abs().max() / ref.abs().max().clamp_min(1e-300))

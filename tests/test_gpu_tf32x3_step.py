@@ -14,9 +14,9 @@ read, in image or row chunks where memory needs it.  Bars (u = 2^-24):
     N Hp Wp pixels), since wgmma accumulates toward zero.  Statistics: STATS_SELF_BAR against
     the float64 sums of the kernel's own output, the fprop bar against the reference's sums.
     Every conv kernel that runs must be a three-pass instantiation `<*, 3>`.
-  * bn_bwd_reduce + bn_bwd_apply.  Each thread adds kRowsPerThread = 64 rows in fp32, the CTA's
-    row slots and all CTAs add in double, so with d = 64 + 2, |d dbeta| <= d u sum|g| and
-    |d dgamma| <= (d + 1) u sum|g xhat| + sum|g| e_xhat, where e_xhat = 4u (|xhat| + |mean|
+  * bn_bwd_reduce + bn_bwd_apply (step_cases.check_bn_bwd).  Each thread adds kRowsPerThread =
+    64 rows in fp32, the CTA's row slots and all CTAs add in double, so with d = 64 + 2,
+    |d dbeta| <= d u sum|g| and |d dgamma| <= (d + 1) u sum|g xhat| + sum|g| e_xhat, where e_xhat = 4u (|xhat| + |mean|
     invstd) is the error of the fp32 xhat formed from the fp32 mean and invstd (the same terms
     as test_gpu_bn_chain's backward).  dgamma and dbeta then round once to fp32.  Not from
     max|dgamma|: dgamma cancels.  k0 = gamma invstd, k1 = sum g / M, k2 = sum g xhat / M round
@@ -25,9 +25,9 @@ read, in image or row chunks where memory needs it.  Bars (u = 2^-24):
     g is dy masked by y_out > 0 (the last BatchNorm of a block and every downsample BatchNorm)
     or by the BatchNorm's own ReLU, fma(z, scale, shift) > 0 (every other BatchNorm): the
     float64 sign of z scale + shift is that fma's sign, so the reference masks exactly alike.
-  * bn_act: y = relu(fma(x, s, b) + q), q = fma(r, rs, rb), r or 0: three roundings on the
-    terms, so |d y| <= 4u (|x s| + |b| + |r rs| + |rb|) (|r| for an identity residual); where
-    the float64 value is below minus that bar, y must be exactly 0.
+  * bn_act (step_cases.check_bn_act): y = relu(fma(x, s, b) + q), q = fma(r, rs, rb), r or 0:
+    three roundings on the terms, so |d y| <= 4u (|x s| + |b| + |r rs| + |rb|) (|r| for an
+    identity residual); where the float64 value is below minus that bar, y must be exactly 0.
   * bn_relu_maxpool: the fp32 activations relu(fma(z, s, b)) are recomputed exactly (`_fma32`),
     the pool restated with the kernel's rule (the first strictly greater value in (kh, kw)
     order) must give y and argidx bit for bit, and y is within one rounding, u y64, of the
@@ -45,13 +45,13 @@ import pytest
 import torch
 
 from tests import step_cases as sc
-from tests.step_cases import (C4_LAYERS_TF32X3, EPS, KPIX, RUN_BLOCKS3, U, WGRAD_BAR, _emul_mma, _guarded,
+from tests.step_cases import (C4_LAYERS_TF32X3, KPIX, ROWS_PER_THREAD, RUN_BLOCKS3, U, WGRAD_BAR, _bn_act_check,
+                              _bn_act_ref_bar, _bn_bwd_ratios, _bn_bwd_ref_bar, _bn_stats64, _emul_mma, _guarded,
                               _tc_bar, _tf32_np, _tf32_wgrad_plan, _trunc_np)
 
 gpu = pytest.mark.gpu
 
 NB, HWB, JB, DB, HMB = 128, 256, 16, 64, 64      # one GPU's bench batch: 32 tuples x 4 views
-ROWS_PER_THREAD = 64                             # bn.cu kRowsPerThread
 
 
 def _wgrad_runs(layer, N=NB):
@@ -73,44 +73,7 @@ def test_c4_layer_table_wgrad_runs():
     assert _tc_bar(WGRAD_BAR, R, 3) <= 1e-4
 
 
-# ------------------------------------------------------------------ bars shared by the CPU and GPU tests
-def _bn_stats64(x):
-    """float64 batch mean and invstd of x [M, C] (the fp32 eps, as bn_finalize adds it)"""
-    xd = x.double()
-    mu = xd.mean(0)
-    var = (xd - mu).pow(2).mean(0)
-    return mu, 1 / torch.sqrt(var + float(np.float32(EPS)))
-
-
-def _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv):
-    """float64 BatchNorm backward of g = dy * keep on x [M, C] with batch statistics (mu, inv),
-    and the module's bars: (dbeta, dgamma, dx, bar_b, bar_g, bar_dx)"""
-    M = x.shape[0]
-    g = dy.double() * keep
-    xh = (x.double() - mu) * inv
-    sg, sgx = g.sum(0), (g * xh).sum(0)
-    d = ROWS_PER_THREAD + 2
-    ag = g.abs()
-    e_xh = 4 * U * (xh.abs() + mu.abs() * inv)
-    bar_b = d * U * ag.sum(0)
-    bar_g = (d + 1) * U * (ag * xh.abs()).sum(0) + (ag * e_xh).sum(0)
-    k1, k2 = sg / M, sgx / M
-    a = gamma.double() * inv
-    dx = a * (g - k1 - xh * k2)
-    bar = a.abs() * (4 * U * (ag + k1.abs() + (xh * k2).abs()) + bar_b / M + xh.abs() * (bar_g / M)
-                     + k2.abs() * e_xh) + 2 * U * dx.abs()
-    return sg, sgx, dx, bar_b, bar_g, bar
-
-
-def _bn_bwd_ratios(dbeta, dgamma, dx, ref):
-    """worst err / bar of dbeta, dgamma (each after its one fp32 rounding) and dx"""
-    sg, sgx, dx64, bar_b, bar_g, bar = ref
-    eb = ((dbeta.double() - sg).abs() - U * sg.abs()).clamp_min(0) / (bar_b + 1e-300)   # a fully masked
-    eg = ((dgamma.double() - sgx).abs() - U * sgx.abs()).clamp_min(0) / (bar_g + 1e-300)  # channel: 0 / 0
-    ex = (dx.double() - dx64).abs() / (bar + 1e-300)
-    return float(eb.max()), float(eg.max()), float(ex.max())
-
-
+# ------------------------------------------------------------------ emulations against the bars of step_cases
 def _fma_np(x, s, b):
     return (x.astype(np.float64) * s + b).astype(np.float32)
 
@@ -187,29 +150,6 @@ def test_bn_bwd_bars_hold_for_the_kernel_order_and_reject(mistake):
     print("emulated BatchNorm backward: worst err / bar %.3f; %s: %.3g" % (worst_ok, mistake, worst_bad))
     assert worst_ok <= 1.0
     assert worst_bad > 2.0
-
-
-def _bn_act_ref_bar(x, s, b, r, rs, rb):
-    """float64 x s + b (+ r rs + rb, or + r) and the bar 4u on its terms"""
-    xd = x.double()
-    t = xd * s.double() + b.double()
-    terms = (xd * s.double()).abs() + b.double().abs()
-    if r is not None:
-        rd = r.double()
-        if rs is not None:
-            t = t + rd * rs.double() + rb.double()
-            terms = terms + (rd * rs.double()).abs() + rb.double().abs()
-        else:
-            t = t + rd
-            terms = terms + rd.abs()
-    return t, 4 * U * terms
-
-
-def _bn_act_check(y, t, bar):
-    """(worst |y - relu(t)| / bar, elements below -bar that are not exactly 0, negative y)"""
-    err = (y.double() - t.clamp_min(0)).abs()
-    dead = t < -bar
-    return (float((err / (bar + 1e-300)).max()), int((dead & (y != 0)).sum()), int((y < 0).sum()))
 
 
 def test_bn_act_bar_rejects_a_residual_without_its_affine():
@@ -458,54 +398,19 @@ BN_EDGE = [(524288 - 23, 256, "y_out"), (131072 - 23, 96, "relu"), (131072 - 23,
            (32768 - 23, 1152, "relu")]
 
 
-def _check_bn_bwd(dev, M, C, mode):
-    from epipolarpose_b200 import ops
-    g = torch.Generator(device=dev).manual_seed(M + C)
-    x = torch.randn(M, C, device=dev, generator=g) * (torch.rand(C, device=dev, generator=g) * 2 + 0.2) \
-        + torch.randn(C, device=dev, generator=g) * 2
-    x[:, 0] = 0.37                                           # var 0: invstd = 1 / sqrt(eps)
-    dy = (torch.randn(M, C, device=dev, generator=g) + torch.randn(C, device=dev, generator=g) * 0.5) * 1e-4
-    dy[M // 2, 1] = 3.0                                      # one huge element
-    gamma = torch.rand(C, device=dev, generator=g) + 0.5
-    beta = torch.randn(C, device=dev, generator=g) * 0.1
-    mu, inv = _bn_stats64(x)
-    mean, invstd = mu.float(), inv.float()
-    scale, shift = (gamma.double() * inv).float(), (beta.double() - mu * gamma.double() * inv).float()
-    y_out = None
-    if mode == "relu":
-        scale[2], shift[2] = 0.0, -1.0                       # a fully masked channel
-        keep = (x.double() * scale.double() + shift.double()) > 0
-    else:
-        y_out = torch.relu(torch.randn(M, C, device=dev, generator=g))
-        y_out[:, 2] = 0
-        keep = y_out > 0
-    relu = int(mode == "relu")
-    sums = torch.zeros(2 * C, device=dev, dtype=torch.float64)
-    dx, dg, db = torch.empty(M, C, device=dev), torch.empty(C, device=dev), torch.empty(C, device=dev)
-    ops.bn_bwd_reduce(dy, x, y_out, scale, shift, mean, invstd, relu, M, C, sums)
-    ops.bn_bwd_apply(dy, x, y_out, scale, shift, mean, invstd, gamma, relu, sums, M, C, dx, dg, db)
-    torch.cuda.synchronize()
-    del y_out
-    ref = _bn_bwd_ref_bar(x, dy, keep, gamma, mu, inv)
-    rb, rg, rx = _bn_bwd_ratios(db, dg, dx, ref)
-    print("  bn bwd %7d x %-4d %-5s worst err / bar: dbeta %.3f dgamma %.3f dx %.3f (max dx err %.2e)"
-          % (M, C, mode, rb, rg, rx, float((dx.double() - ref[2]).abs().max())))
-    assert rb <= 1.0 and rg <= 1.0 and rx <= 1.0
-
-
 @gpu
 @pytest.mark.parametrize("M,C,mode", BN_BWD, ids=["%dx%d-%s" % c for c in BN_BWD])
 def test_tf32x3_bn_bwd_vs_float64(dev, M, C, mode):
     """bn_bwd_reduce + bn_bwd_apply at every (M, C) and mask form of the step: dbeta, dgamma per
     channel and dx per element against float64, with a constant channel (invstd = 316), one
     huge gradient element and a fully masked channel beside ordinary ones."""
-    _check_bn_bwd(dev, M, C, mode)
+    sc.check_bn_bwd(dev, M, C, mode)
 
 
 @gpu
 @pytest.mark.parametrize("M,C,mode", BN_EDGE, ids=["%dx%d-%s" % c for c in BN_EDGE])
 def test_tf32x3_bn_bwd_edge_shapes(dev, M, C, mode):
-    _check_bn_bwd(dev, M, C, mode)
+    sc.check_bn_bwd(dev, M, C, mode)
 
 
 BN_ACT = [(524288, 256), (131072, 512), (32768, 1024), (8192, 2048)]
@@ -517,32 +422,7 @@ BN_ACT = [(524288, 256), (131072, 512), (32768, 1024), (8192, 2048)]
 def test_tf32x3_bn_act_vs_float64(dev, M, C, res):
     """bn_act at every block output: the residual with the downsample BatchNorm's affine, the
     identity residual, and ReLU alone; within 4u of the terms, exact zeros below -bar."""
-    from epipolarpose_b200 import ops
-    g = torch.Generator(device=dev).manual_seed(M + C + len(res))
-    x = torch.randn(M, C, device=dev, generator=g) * 3 + 0.5
-    s, b = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
-    r = rs = rb = None
-    if res != "relu":
-        r = torch.randn(M, C, device=dev, generator=g) * 2
-        if res == "identity":
-            r = torch.relu(r)                                     # a block output
-        else:
-            rs, rb = torch.rand(C, device=dev, generator=g) + 0.2, torch.randn(C, device=dev, generator=g) * 0.5
-    y, guard = _guarded((M, C), dev, float("nan"))
-    guard.fill_(1234.5)
-    ops.bn_act(x, s, b, r, rs, rb, 1, y, M, C)
-    torch.cuda.synchronize()
-    assert bool((guard == 1234.5).all()), "guard band overwritten"
-    worst, bad0, neg = 0.0, 0, 0
-    step = max((1 << 24) // C, 1)
-    for r0 in range(0, M, step):
-        sl = slice(r0, r0 + step)
-        t, bar = _bn_act_ref_bar(x[sl], s, b, None if r is None else r[sl], rs, rb)
-        w_, z_, n_ = _bn_act_check(y[sl], t, bar)
-        worst, bad0, neg = max(worst, w_), bad0 + z_, neg + n_
-        del t, bar
-    print("  bn_act %6d x %-4d %-8s worst err / bar %.3f" % (M, C, res, worst))
-    assert worst <= 1.0 and bad0 == 0 and neg == 0, (worst, bad0, neg)
+    sc.check_bn_act(dev, M, C, res)
 
 
 @gpu

@@ -144,6 +144,26 @@ HEAD_C2FLAT = {"epb_avgpool_split", "epb_avgpool_bwd", "epb_heatmap_joint_loss",
                "epb_colsum"}
 GEOMETRY = {"epb_patch_to_image", "epb_triangulate", "epb_project_labels", "epb_relative_pose", "epb_tuple_labels"}
 
+S = "test_gpu_refiner_step.py::"
+COVERAGE_REFINER = {
+    "epb_conv_fprop": [S + "test_refiner_linears_vs_float64"],
+    "epb_conv_wgrad": [S + "test_refiner_linears_vs_float64"],
+    "epb_pack_weight": [S + "test_refiner_pack_weight_bit_exact"],
+    "epb_colsum": [S + "test_refiner_colsum_vs_float64"],
+    "epb_bn_finalize": [S + "test_refiner_bn_finalize_vs_float64", S + "test_refiner_training_forward_vs_float64"],
+    "epb_bn_act": [S + "test_refiner_bn_act_vs_float64"],
+    "epb_bn_bwd_reduce": [S + "test_refiner_bn_bwd_vs_float64"],
+    "epb_bn_bwd_apply": [S + "test_refiner_bn_bwd_vs_float64"],
+    "epb_bn_eval_affine": [S + "test_refiner_bn_eval_affine_vs_float64", S + "test_refiner_training_forward_vs_float64"],
+    "epb_mask_scale": [S + "test_refiner_mask_scale_bit_exact"],
+    "epb_add3": [S + "test_refiner_add3_bit_exact"],
+    "epb_sumsq": [S + "test_refiner_clip_grad_norm_vs_float64"],
+    "epb_clip_scale": [S + "test_refiner_clip_grad_norm_vs_float64"],
+    "epb_adam_step": [S + "test_refiner_fused_adam_vs_float64_on_model_buffer"],
+}
+# the refiner step's entries (refiner/main.py train() and the eval forward of test())
+REFINER = set(COVERAGE_REFINER)
+
 
 def _missing_coverage(recorded, table):
     """entries without a row, and rows that name a test function that does not exist"""
@@ -210,6 +230,19 @@ def _three_pass_convs(tags):
 def _fp32_engine(eng):
     from epipolarpose_b200 import net
     return type(eng) is net.Engine and eng.precision == 3 and eng.wgrad_precision == 3
+
+
+def _refiner_convs(tags):
+    """the refiner's linears: every tensor-core kernel a three-pass instantiation, both CUDA-core
+    kernels (the 48-channel products) and at least one tensor-core fprop and wgrad"""
+    tc = {t for t in tags if "_tc<" in t}
+    return sc._all_three_pass(tc) and tags - tc == {"fprop_simt", "wgrad_simt"} and \
+        any(t.startswith("fprop") for t in tc) and any(t.startswith("wgrad") for t in tc)
+
+
+def _mlp_engine(eng):
+    from epipolarpose_b200 import mlp
+    return type(eng) is mlp.MLPEngine and _fp32_engine(eng.eng)
 
 
 # ------------------------------------------------------------------ steps
@@ -313,7 +346,65 @@ def _graphed_step(dev, row):
     return m, run
 
 
+def _refiner_step(dev, shape, ops=None):
+    """refiner/main.py train() for one epoch of one batch (LinearModelPG(linear_size, 45 -> 45),
+    p_dropout 0.5, FusedAdam, MSELoss on both heads, clip_grad_norm_ to 1), then one eval forward
+    of the batch as main.test() runs it; returns the training loss.  shape: (linear_size, rows).
+    ops: the model's engine and refiner.utils run on it (the emulated ABI), restored after."""
+    import logging
+    import types
+    import lib.utils.utils as Ut
+    from oracle import restate_refiner as rr
+    from epipolarpose_b200.refiner import main as rmain, model as rmodel, utils as rutils
+    L, N = shape
+    m = rmodel.LinearModelPG(linear_size=L, p_dropout=0.5, input_size=45, output_size=45)
+    m.load_state_dict(rr.init_state(rr.param_shapes(L, 45, 45), 3))
+    m = m.to(dev)
+    rmodel.LinearModelPG._backend[0] = ops
+    try:
+        m._engine()                                  # binds the engine to `ops`
+    finally:
+        rmodel.LinearModelPG._backend[0] = None
+    opt = Ut.FusedAdam(list(m.parameters()), lr=1e-3)
+    g = torch.Generator().manual_seed(4)
+    x, t = torch.randn(N, 45, generator=g), torch.randn(N, 45, generator=g) * 0.3
+    args = types.SimpleNamespace(lr=1e-3, lr_decay=100000, lr_gamma=0.96)
+    mse, losses = torch.nn.MSELoss(reduction="mean"), []
+
+    def crit(a, b):
+        loss = mse(a, b)
+        losses.append(loss.detach())
+        return loss
+
+    def run():
+        real = rutils._backend[0]
+        rutils._backend[0] = ops or real
+        try:
+            rmain.train(m, [(x, t)], opt, 0, args.lr, crit, args, logging.getLogger("refiner"))
+            m.eval()
+            with torch.no_grad():
+                p2 = m(x.to(dev))[1]
+            m.train()
+        finally:
+            rutils._backend[0] = real
+        assert bool(torch.isfinite(p2).all())
+        return losses[-2] + losses[-1]
+    return m, run
+
+
+def _refiner_device_step(dev, row):
+    return _refiner_step(dev, row["device"])
+
+
+def _emulated_refiner_step(row):
+    from tests import emul_ops
+    return _refiner_step(torch.device("cpu"), row["emulated"], ops=emul_ops)
+
+
 # ------------------------------------------------------------------ compositions
+# kernel tags a row's predicate accepts (the first) and sets it rejects
+TC3 = {"fprop_tc<64,3>", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
+REFINER_TAGS = {"fprop_simt", "wgrad_simt", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
 # emulated / device: (layers, J, D, image size, and for the device half tuples of 4 views); calls:
 # entries every half must call; online: entries the device half (online labels) must call too
 COMPOSITIONS = {
@@ -335,7 +426,9 @@ COMPOSITIONS = {
         emulated=(18, 16, 64, 64), device=(50, 16, 64, 256, 2),
         calls=FP32_ENGINE | {"epb_adam_step_dev"}, online={"epb_triangulate"},
         not_called=lambda e: e.endswith("_split") or "conv16" in e,
-        engine=_fp32_engine, tags=_three_pass_convs),
+        engine=_fp32_engine, tags=_three_pass_convs,
+        tag_examples=(TC3, [TC3 | {bad} for bad in ("fprop_tc<128,1>", "wgrad_tc<64,1>", "wgrad_simt", "fprop_simt")]
+                      + [set()])),
     "robust_tuples": dict(
         table=COVERAGE_ROBUST, precision="f16x3", method="robust", views=4, driver=_graphed_step,
         emulated=None, device=(18, 16, 64, 256, 2),
@@ -354,6 +447,17 @@ COMPOSITIONS = {
         estimate_extrinsics=True, emulated=None, device=(18, 16, 64, 256, 2),
         calls=set(), online={"epb_relative_pose"}, not_called={"epb_tuple_labels"},
         engine=None, tags=None),
+    # refiner/main.py train() (LinearModelPG through mlp.MLPEngine on the fp32 engine at 3xTF32)
+    # and the eval forward of test(); emulated at linear_size 128, 16 rows
+    "refiner": dict(
+        table=COVERAGE_REFINER, precision="tf32x3", method=None, views=None, driver=_refiner_device_step,
+        emulated_driver=_emulated_refiner_step, emulated=(128, 16), device=(1024, 64),
+        calls=REFINER, online=set(),
+        not_called=lambda e: e == "epb_adam_step_dev" or e.endswith("_split") or "conv16" in e or
+        e.startswith("epb_softargmax_") or e in GEOMETRY,
+        engine=_mlp_engine, tags=_refiner_convs,
+        tag_examples=(REFINER_TAGS, [REFINER_TAGS | {"fprop_tc<128,1>"}, REFINER_TAGS | {"wgrad_tc<128,1>"}]
+                      + [REFINER_TAGS - {t} for t in sorted(REFINER_TAGS)] + [{"fprop_simt", "wgrad_simt"}, set()])),
 }
 EMULATED = [k for k, row in COMPOSITIONS.items() if row["emulated"] is not None]
 
@@ -373,8 +477,9 @@ def _check_calls(row, calls, required, what):
 
 @pytest.mark.parametrize("comp", list(COMPOSITIONS))
 def test_gate_has_teeth(comp):
-    """Deleting any row, or pointing one at a test that does not exist, fails the gate; the kernel
-    tag check rejects a single-pass or CUDA-core conv among three-pass ones, and an empty set."""
+    """Deleting any row, or pointing one at a test that does not exist, fails the gate; the row's
+    kernel tag check accepts its good example and rejects each bad one (a single-pass kernel, a
+    kernel family that must or must not run, an empty set)."""
     table, tags = COMPOSITIONS[comp]["table"], COMPOSITIONS[comp]["tags"]
     rec = sorted(table)
     assert _missing_coverage(rec, table) == ([], [])
@@ -385,11 +490,10 @@ def test_gate_has_teeth(comp):
         t[k] = ["test_gpu_step_kernels.py::test_no_such_test"]
         assert _missing_coverage(rec, t)[1]
     if tags is not None:
-        good = {"fprop_tc<64,3>", "fprop_tc<128,3>", "wgrad_tc<128,3>"}
+        good, bads = COMPOSITIONS[comp]["tag_examples"]
         assert tags(good)
-        for bad in ("fprop_tc<128,1>", "wgrad_tc<64,1>", "wgrad_simt", "fprop_simt"):
-            assert not tags(good | {bad})
-        assert not tags(set())
+        for bad in bads:
+            assert not tags(bad), bad
 
 
 @pytest.mark.parametrize("comp", EMULATED)
