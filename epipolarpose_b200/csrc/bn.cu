@@ -111,10 +111,11 @@ __global__ void bn_eval_affine_kernel(int C, const float* __restrict__ gamma,
                                       float* __restrict__ shift) {
   const int c = blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= C) return;
-  const float invstd = 1.f / sqrtf(rv[c] + eps);
-  const float g = gamma ? gamma[c] : 1.f, b = beta ? beta[c] : 0.f;
-  scale[c] = g * invstd;
-  shift[c] = b - rm[c] * g * invstd;
+  // in double, rounded once: shift = beta - mean * scale cancels when the two are close, and fp32
+  // arithmetic there left shift many of its own ulps off
+  const double s = (gamma ? (double)gamma[c] : 1.0) / sqrt((double)rv[c] + (double)eps);
+  scale[c] = (float)s;
+  shift[c] = (float)((beta ? (double)beta[c] : 0.0) - (double)rm[c] * s);
 }
 
 __device__ __forceinline__ float4 fma4(float4 x, float4 s, float4 b) {

@@ -153,9 +153,9 @@ def bn_finalize(stats, M, C, gamma, beta, eps, momentum, running_mean, running_v
 
 
 def bn_eval_affine(C, gamma, beta, running_mean, running_var, eps, scale, shift):
-    inv = 1.0 / torch.sqrt(running_var + eps)
-    scale.copy_(gamma * inv)
-    shift.copy_(beta - running_mean * gamma * inv)
+    s = gamma.double() / torch.sqrt(running_var.double() + float(torch.tensor(eps, dtype=torch.float32)))
+    scale.copy_(s.float())
+    shift.copy_((beta.double() - running_mean.double() * s).float())
 
 
 def bn_act(x, scale, shift, r, rscale, rshift, relu, y, M, C):

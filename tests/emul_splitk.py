@@ -98,12 +98,18 @@ def conv16_fprop_splitk(g, x, x_sc, w, w_sc, out, bias, stats, S):
 def conv16_calls(plan, N, H=256, W=256, ops=em):
     """(layer name, geometry) of every conv16 fprop call of Engine16.forward at batch N, from the
     plan's shapes alone (stem patch matrix, blocks with their downsample, deconv phases, final)."""
+    return [(conv.name, g) for conv, h, w in conv16_layers(plan, H, W)
+            for g in conv.fprop_geoms(ops, N, h, w, 3) if g is not None]
+
+
+def conv16_layers(plan, H=256, W=256):
+    """(conv, input height, input width) of every conv16 layer of Engine16.forward, in call order"""
     from epipolarpose_b200.net import Conv
     from epipolarpose_b200.net16 import STEM_KPAD16
     out = []
 
     def add(conv, h, w):
-        out.extend((conv.name, g) for g in conv.fprop_geoms(ops, N, h, w, 3) if g is not None)
+        out.append((conv, h, w))
         return conv.out_hw(h, w)
 
     H1, W1 = plan.stem.out_hw(H, W)

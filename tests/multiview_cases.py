@@ -151,3 +151,15 @@ def plant_outliers(u, seed, px=80.0):
         for j in range(J):
             out[t, which[t, j], j] += px * np.array([np.cos(ang[t, j]), np.sin(ang[t, j])])
     return out, which
+
+
+def rig_inputs(T, V, seed, HW=256):
+    """images [T, V, 3, HW, HW], boxes and projection matrices [T, V, 3, 4] of T synthetic rigs,
+    the inputs of MultiViewPredictor"""
+    rng = np.random.default_rng(seed)
+    _, _, _, _, P = restate.synthetic_cameras(rng, T, V)
+    x = rng.standard_normal((T, V, 3, HW, HW)).astype(np.float32)
+    n = T * V
+    boxes = {"center_x": 512 + rng.uniform(-20, 20, n), "center_y": 515 + rng.uniform(-20, 20, n),
+             "width": rng.uniform(40, 80, n), "height": rng.uniform(40, 80, n)}
+    return x, boxes, P

@@ -1,5 +1,5 @@
 """Shared by the training-step tests (test_gpu_step_kernels, test_gpu_c5_step, test_gpu_tf32x3_step,
-test_gpu_c2_flat_step, test_gpu_refiner_step, test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32,
+test_gpu_c2_flat_step, test_gpu_refiner_step, test_gpu_infer_step, test_gpu_bn_chain, test_gpu_split16, test_gpu_tf32,
 test_gpu_predictor, test_gpu_conv16_store and test_step_coverage): the float64 check bodies each composition runs at its own sizes, the bars and
 the emulations they rest on, the restated planners, the layer tables, the device data makers and
 one cache of models and conv outputs keyed by composition.
@@ -661,18 +661,19 @@ def _check_pack_weight_batch(dev, m):
 
 def _check_im2col_split(dev, kpad, N, H):
     """im2col_split of N images of H x H (7 x 7 / 2, pad 3), bit-exact with the CPU emulation on
-    five images"""
+    up to five images"""
     from epipolarpose_b200 import ops, net16
     W = H
     Ho = Wo = H // 2
     g = torch.Generator(device=dev).manual_seed(51)
     img = torch.randn(N, 3, H, W, device=dev, generator=g)
-    img[5, :, 0, :] = 4094.0 / net16.IMG_SCALE              # the static scale's largest magnitude
+    big = min(5, N - 1)
+    img[big, :, 0, :] = 4094.0 / net16.IMG_SCALE            # the static scale's largest magnitude
     col = torch.empty(2, N, Ho, Wo, kpad, device=dev, dtype=torch.float16)
     sc = torch.tensor([net16.IMG_SCALE, 1.0 / net16.IMG_SCALE, 65504.0 / net16.IMG_SCALE, 0.0], device=dev)
     ops.im2col_split(img, col, sc, N, 3, H, W, 7, 7, 2, 3, Ho, Wo, kpad)
     torch.cuda.synchronize()
-    pick = [0, 5, N // 2 - 1, N // 2, N - 1]
+    pick = sorted({0, big, max(0, N // 2 - 1), N // 2, N - 1})
     cimg = img[pick].cpu()
     ccol = torch.empty(2, len(pick), Ho, Wo, kpad, dtype=torch.float16)
     em.im2col_split(cimg, ccol, sc.cpu(), len(pick), 3, H, W, 7, 7, 2, 3, Ho, Wo, kpad)
@@ -778,16 +779,29 @@ def _check_softargmax_fwd(dev, kind, N, J, D, H, W):
     ops.softargmax_fwd(logits, 1, N, J, D, H, W, coords, lse)
     torch.cuda.synchronize()
     S, ppi, d = _nhwc_geometry(N, J, D, H, W)
+    worst_c, worst_l, maxerr, max_ok = _softargmax_ratios(logits, coords, lse, N, J, D, H, W)
+    assert max_ok, "lse[0] is not the maximum"
+    print("  softargmax fwd %-8s S %d ppi %d depth %d: coords max err %.3e worst err / bar %.3f, "
+          "lse[1] worst err / bar %.3f" % (kind, S, ppi, d, maxerr, worst_c, worst_l))
+    assert worst_c <= 1.0 and worst_l <= 1.0
+
+
+def _softargmax_ratios(logits, coords, lse, N, J, D, H, W):
+    """(worst coordinate err / bar, worst lse[1] err / bar, largest coordinate error, lse[0] is the
+    maximum exactly) of an NHWC soft-argmax forward over the fp32 volume `logits` [N, H, W, J*D]
+    that it read, with the bars of _check_softargmax_fwd"""
+    dev = logits.device
+    S, ppi, d = _nhwc_geometry(N, J, D, H, W)
     xs = torch.arange(W, device=dev, dtype=torch.float64).view(1, 1, W, 1, 1) / W
     ys = torch.arange(H, device=dev, dtype=torch.float64).view(1, H, 1, 1, 1) / H
     zs = torch.arange(D, device=dev, dtype=torch.float64).view(1, 1, 1, 1, D) / D
     lk = lse.view(N, J, 2)
-    worst_c, worst_l, maxerr = 0.0, 0.0, 0.0
-    B = 8
-    for n0 in range(0, N, B):
+    worst_c, worst_l, maxerr, max_ok = 0.0, 0.0, 0.0, True
+    for n0 in range(0, N, 8):
+        B = min(8, N - n0)
         v = logits[n0:n0 + B].double().view(B, H, W, J, D)
         m = v.amax((1, 2, 4), keepdim=True)
-        assert torch.equal(lk[n0:n0 + B, :, 0].double(), m.view(B, J)), "lse[0] is not the maximum"
+        max_ok = max_ok and torch.equal(lk[n0:n0 + B, :, 0].double(), m.view(B, J))
         ex = torch.exp(v - m)
         tot = ex.sum((1, 2, 4), keepdim=True)
         p = ex / tot
@@ -806,9 +820,7 @@ def _check_softargmax_fwd(dev, kind, N, J, D, H, W):
         el = (lk[n0:n0 + B, :, 1].double() * tot.view(B, J) - 1).abs()
         worst_l = max(worst_l, float((el / lbar.view(B, J)).max()))
         del p, pe
-    print("  softargmax fwd %-8s S %d ppi %d depth %d: coords max err %.3e worst err / bar %.3f, "
-          "lse[1] worst err / bar %.3f" % (kind, S, ppi, d, maxerr, worst_c, worst_l))
-    assert worst_c <= 1.0 and worst_l <= 1.0
+    return worst_c, worst_l, maxerr, max_ok
 
 
 def _jointloss64(x, t, w, kind, norm, div):
@@ -1994,3 +2006,178 @@ def run_hm_loss(case, N, J, H, W):
     dx = torch.full_like(x, float("nan"))
     ops.heatmap_joint_loss(hm, tg, wh, R, HW, 1.0, x, t, w, x.numel(), 1, float(N), 1.0, loss, dhm, dx)
     return loss, dhm, dx
+
+
+# ------------------------------------------------------------------ inference: split-K conv16, calibrated models, decode
+PATCH = 256.0
+# key -> (layers, J, D, image size, init_state seed) of the predictor models: C1 (MPII), the H36M
+# model of MultiViewPredictor and save_triangulations, C5
+INFER_MODELS = {"c1": (50, 16, 64, 256, 71), "h36m": (50, 17, 64, 256, 72), "c5": (101, 17, 96, 384, 75)}
+
+
+def _bench_conv(layer):
+    """(conv, input size) of a C4_LAYERS_SPLIT16 row"""
+    from epipolarpose_b200 import net
+    name, kind, cin, cout, k, s, p, hw = layer
+    return net.Conv("t", kind, cin, cout, k, s, p, 0), hw
+
+
+def _splitk_layer(dev, conv, hw, N, seed=7, ref=True):
+    """geoms, split operands, bias, the float64 reference [N, Ho, Wo, Cout] with bias (None without
+    `ref`) and the joined float64 operands (x NCHW, w as conv2d / conv_transpose2d take it) of conv
+    at batch N on hw x hw inputs.  Float64 reads the joined planes: the exact values the kernel reads."""
+    import torch.nn.functional as F
+    from epipolarpose_b200 import ops
+    kind, cin, cout, k, s, p = conv.kind, conv.cin, conv.cout, conv.k, conv.stride, conv.pad
+    T = k * k
+    g = torch.Generator(device=dev).manual_seed(seed)
+    x, x_sc, xv = _split_dev(torch.relu(torch.randn(N, hw, hw, cin, device=dev, generator=g)))
+    w = torch.randn((cout, cin, k, k) if kind == "conv" else (cin, cout, k, k), device=dev,
+                    generator=g) * (2.0 / (T * cin)) ** 0.5
+    wf, wf_sc, wfv = _split_dev(conv.pack(ops, w)[0])
+    bias = torch.randn(cout, device=dev, generator=g)
+    pk = wfv.view(cout, T, cin)
+    wq = pk.permute(0, 2, 1).reshape(cout, cin, k, k) if kind == "conv" else \
+        pk.permute(2, 0, 1).reshape(cin, cout, k, k)
+    xa = xv.permute(0, 3, 1, 2).contiguous()
+    del xv
+    out = None
+    if ref:
+        out = F.conv2d(xa, wq, None, s, p) if kind == "conv" else F.conv_transpose2d(xa, wq, None, s, p, conv.opad)
+        out = out.permute(0, 2, 3, 1) + bias.double()
+    geoms = [gm for gm in conv.fprop_geoms(ops, N, hw, hw, 3) if gm is not None]
+    for gm in geoms:
+        gm.in_relu, gm.accumulate = 0, 0
+    return geoms, (x, x_sc, wf, wf_sc), bias, out, (xa, wq)
+
+
+def _splitk_run(geoms, opnds, bias, out, stats, splits):
+    """splits: an int (capped at each call's K/64) or None for the planner's count; the workspace
+    holds exactly the planner's ws_floats at that count"""
+    from epipolarpose_b200 import ops
+    from tests import emul_splitk as es
+    x, x_sc, w, w_sc = opnds
+    for gm in geoms:
+        s = ops.conv16_splits(gm)[0] if splits is None else min(splits, es.kblocks(gm))
+        ws = torch.empty(max(1, s * es.phase_tiles(gm) * 128 * gm.Cout), device=out.device)
+        ops.conv16_fprop_splitk(gm, x, x_sc, w, w_sc, out, bias, stats, s, ws)
+
+
+def _split_partial64(conv, gm, xw, lo, hi):
+    """float64 sum of k-blocks [lo, hi) of a gather conv (k-block = 64 channels of one tap, taps
+    outer, as the split ranges of epb_conv16_fprop_splitk cut K): what one split contributes"""
+    import torch.nn.functional as F
+    xa, wq = xw
+    CB = gm.Cin // 64
+    mask = torch.zeros_like(wq)
+    for kb in range(lo, hi):
+        t, cb = divmod(kb, CB)
+        r, c = divmod(gm.wt[t], conv.k)
+        mask[:, cb * 64:(cb + 1) * 64, r, c] = 1
+    return F.conv2d(xa, wq * mask, None, conv.stride, conv.pad).permute(0, 2, 3, 1)
+
+
+def _coord_bound(dl):
+    """largest move (patch px) of a soft-argmax coordinate whose logits each move by <= dl"""
+    return PATCH * np.expm1(2.0 * np.asarray(dl, dtype=np.float64)) + 1e-3   # + float32 rounding
+
+
+def infer_plan(key):
+    from epipolarpose_b200.net import PoseNetPlan
+    layers, J, D, HW, _ = INFER_MODELS[key]
+    return PoseNetPlan(num_layers=layers, num_joints=J, volume=True, depth_res=D, image_size=(HW, HW))
+
+
+def infer_layers(keys):
+    """(conv, input size) of every distinct conv16 layer the inference forward of the models `keys`
+    runs (emul_splitk.conv16_layers), in call order; the same shape counts once"""
+    from tests import emul_splitk as es
+    seen, out = set(), []
+    for key in keys:
+        HW = INFER_MODELS[key][3]
+        for conv, h, w in es.conv16_layers(infer_plan(key), HW, HW):
+            sig = (conv.kind, conv.cin, conv.cout, conv.k, conv.stride, conv.pad, h, w)
+            if sig not in seen:
+                seen.add(sig)
+                out.append((conv, h))
+    return out
+
+
+def calibrated_state(dev, key, calib=4):
+    """The model's init_state weights with calibrated running statistics, as a trained network has:
+    one float64 training forward of oracle.restate_net over `calib` seeded images, each
+    BatchNorm's running_mean / running_var set to that batch's mean and unbiased variance (momentum
+    1, solved from the forward's momentum-0.1 update), then perturbed per channel so that eval and
+    batch statistics differ: running_var x U(0.5, 2), running_mean + U(-0.5, 0.5) batch std.
+    Cached under "infer_state_" + key."""
+    ck = "infer_state_" + key
+    if ck not in _CACHE:
+        from oracle import restate_net as rn
+        layers, J, D, HW, seed = INFER_MODELS[key]
+        sd = rn.init_state(rn.param_shapes(num_layers=layers, num_joints=J, volume=True, depth_res=D), seed)
+        sd64 = {k: v.to(dev, torch.float64) if v.is_floating_point() else v.to(dev) for k, v in sd.items()}
+        x = torch.from_numpy(np.random.default_rng(seed + 1).standard_normal((calib, 3, HW, HW))).to(dev)
+        ns = {}
+        with torch.no_grad():
+            rn.forward(sd64, x, num_layers=layers, image_size=(HW, HW), training=True, new_stats=ns)
+        del sd64, x
+        rng = np.random.default_rng(seed + 2)
+        m = rn.BN_MOMENTUM
+        for k in sorted(ns):
+            if not k.endswith(".running_mean"):
+                continue
+            p = k[:-len("running_mean")]
+            mean = ((ns[k].cpu() - (1 - m) * sd[k].double()) / m).numpy()
+            var = ((ns[p + "running_var"].cpu() - (1 - m) * sd[p + "running_var"].double()) / m).numpy()
+            C = mean.size
+            sd[p + "running_var"] = torch.from_numpy((var * rng.uniform(0.5, 2.0, C)).astype(np.float32))
+            sd[p + "running_mean"] = torch.from_numpy(
+                (mean + rng.uniform(-0.5, 0.5, C) * np.sqrt(var)).astype(np.float32))
+        _CACHE[ck] = sd
+    return _CACHE[ck]
+
+
+def calibrated_model(dev, key):
+    """the f16x3 network of INFER_MODELS[key] on calibrated_state, in eval()"""
+    import lib.models as models
+    from tools.bench_cfg import make_cfg
+    layers, J, D, HW, _ = INFER_MODELS[key]
+    cfg = make_cfg(num_layers=layers, num_joints=J, volume=True, depth_res=D, image_size=(HW, HW))
+    model = models.pose3d_resnet.get_pose_net(cfg, False, precision="f16x3")
+    model.load_state_dict(calibrated_state(dev, key))
+    return model.to(dev).eval()
+
+
+def _decode64(L, J, D, pairs=None, shift=False):
+    """float64 soft-argmax of float64 logits L [B, J*D, H, W]: normalised coordinates [N, J, 3] as
+    get_joint_location_coords; with pairs, of the flip-test merge of B = 2N images
+    (flip_cases.flip_merge_softargmax)"""
+    B, _, H, W = L.shape
+    if pairs is not None:
+        from lib.core.integral_loss import flip_permutation
+        n = B // 2
+        fb = L[n:].reshape(n, J, D * H, W).flip(-1)[:, flip_permutation(pairs, J)]
+        if shift:
+            fb = torch.cat([fb[..., :1], fb[..., :-1]], -1)
+        L = 0.5 * (L[:n] + fb.reshape(n, J * D, H, W))
+    N = L.shape[0]
+    p = torch.softmax(L.reshape(N, J, -1), -1).reshape(N, J, D, H, W)
+    ar = lambda k: torch.arange(k, device=L.device, dtype=torch.float64)
+    return torch.stack([(p.sum((2, 3)) * ar(W)).sum(-1) / W, (p.sum((2, 4)) * ar(H)).sum(-1) / H,
+                        (p.sum((3, 4)) * ar(D)).sum(-1) / D], -1) - 0.5
+
+
+def _flip_merged32(L2, N, J, D, perm, shift):
+    """the fp32 volume [N, H, W, J*D] that epb_softargmax_flip_fwd merges in registers from the
+    channels-last logits L2 [2N, H, W, J*D] of [x; flip(x)]: 0.5 * (a + b) with b the mirrored pixel
+    of image n + N in the paired joint's channels, read one column to the left under the shift
+    (column 0 keeps its own); an fp32 add and an exact halving, as the kernel rounds"""
+    _, H, W, C = L2.shape
+    out = torch.empty(N, H, W, C, device=L2.device)
+    for n0 in range(0, N, 8):
+        n1 = min(N, n0 + 8)
+        fb = L2[N + n0:N + n1].view(n1 - n0, H, W, J, D).flip(2)[:, :, :, perm]
+        if shift:
+            fb = torch.cat([fb[:, :, :1], fb[:, :, :-1]], 2)
+        out[n0:n1] = (0.5 * (L2[n0:n1].view(n1 - n0, H, W, J, D) + fb)).reshape(n1 - n0, H, W, C)
+    return out

@@ -168,15 +168,7 @@ def c1(dev):
     return _model(dev, gi.SIZE_CASES["c1"], "f16x3", train=False)
 
 
-def _rig_inputs(T, V, seed):
-    rng = np.random.default_rng(seed)
-    from oracle import restate
-    _, _, _, _, P = restate.synthetic_cameras(rng, T, V)
-    x = rng.standard_normal((T, V, 3, 256, 256)).astype(np.float32)
-    n = T * V
-    boxes = {"center_x": 512 + rng.uniform(-20, 20, n), "center_y": 515 + rng.uniform(-20, 20, n),
-             "width": rng.uniform(40, 80, n), "height": rng.uniform(40, 80, n)}
-    return x, boxes, P
+_rig_inputs = mc.rig_inputs
 
 
 def _check_against_composition(mv, pp, x, boxes, P, thr, use_conf):

@@ -26,12 +26,12 @@ import pytest
 import torch
 
 from tests import emul_splitk as es
-from tests.step_cases import C4_LAYERS_SPLIT16, _split_dev
+from tests.step_cases import C4_LAYERS_SPLIT16, _bench_conv, _coord_bound, _splitk_layer
+from tests.step_cases import _splitk_run as _run
 
 pytestmark = pytest.mark.gpu
 
 LOGIT_BAR = 1e-4
-PATCH = 256.0
 
 
 @pytest.fixture(scope="module")
@@ -41,39 +41,11 @@ def dev():
     return torch.device("cuda:0")
 
 
-def _layer(dev, layer, N, seed=7):
-    """conv, geoms, split operands, bias and the float64 reference [N, Ho, Wo, Cout] with bias."""
-    import torch.nn.functional as F
-    from epipolarpose_b200 import net, ops
-    name, kind, cin, cout, k, s, p, hw = layer
-    conv = net.Conv("t", kind, cin, cout, k, s, p, 0)
-    T = k * k
-    g = torch.Generator(device=dev).manual_seed(seed)
-    x, x_sc, xv = _split_dev(torch.relu(torch.randn(N, hw, hw, cin, device=dev, generator=g)))
-    w = torch.randn((cout, cin, k, k) if kind == "conv" else (cin, cout, k, k), device=dev,
-                    generator=g) * (2.0 / (T * cin)) ** 0.5
-    wf, wf_sc, wfv = _split_dev(conv.pack(ops, w)[0])
-    bias = torch.randn(cout, device=dev, generator=g)
-    pk = wfv.view(cout, T, cin)
-    wq = pk.permute(0, 2, 1).reshape(cout, cin, k, k) if kind == "conv" else \
-        pk.permute(2, 0, 1).reshape(cin, cout, k, k)
-    xa = xv.permute(0, 3, 1, 2).contiguous()
-    ref = F.conv2d(xa, wq, None, s, p) if kind == "conv" else F.conv_transpose2d(xa, wq, None, s, p)
-    ref = ref.permute(0, 2, 3, 1) + bias.double()
-    geoms = [gm for gm in conv.fprop_geoms(ops, N, hw, hw, 3) if gm is not None]
-    for gm in geoms:
-        gm.in_relu, gm.accumulate = 0, 0
-    return conv, geoms, (x, x_sc, wf, wf_sc), bias, ref
-
-
-def _run(geoms, opnds, bias, out, stats, splits):
-    """splits: an int (capped at each call's K/64) or None for the planner's count."""
-    from epipolarpose_b200 import ops
-    x, x_sc, w, w_sc = opnds
-    for gm in geoms:
-        s = ops.conv16_splits(gm)[0] if splits is None else min(splits, es.kblocks(gm))
-        ws = torch.empty(max(1, s * es.phase_tiles(gm) * 128 * gm.Cout), device=out.device)
-        ops.conv16_fprop_splitk(gm, x, x_sc, w, w_sc, out, bias, stats, s, ws)
+def _layer(dev, layer, N):
+    """conv, geoms, split operands, bias and the float64 reference [N, Ho, Wo, Cout] with bias"""
+    conv, hw = _bench_conv(layer)
+    geoms, opnds, bias, ref, _ = _splitk_layer(dev, conv, hw, N)
+    return conv, geoms, opnds, bias, ref
 
 
 CASES = [(l, N) for l in C4_LAYERS_SPLIT16 for N in (1, 32)]
@@ -168,11 +140,6 @@ def _eager(model, x):
     with torch.no_grad():
         out = model.eval()(torch.from_numpy(x).cuda())
         return out, il.get_joint_location_result(x.shape[3], x.shape[2], out)
-
-
-def _coord_bound(dl):
-    """largest move (patch px) of a soft-argmax coordinate whose logits each move by <= dl"""
-    return PATCH * np.expm1(2.0 * np.asarray(dl, dtype=np.float64)) + 1e-3   # + float32 rounding
 
 
 def _close(pred, model, x):

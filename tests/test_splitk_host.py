@@ -117,3 +117,20 @@ def test_emulated_splits_match_the_unsplit_product():
         e = float((out - ref).abs().max() / ref.abs().max())
         assert e <= 1e-6, (S, e)
         assert float((st - st_ref).abs().max() / st_ref.abs().max()) <= 1e-6
+
+
+def test_inference_cases_reach_every_split_regime():
+    """The split counts the planner gives the cases of test_gpu_infer_step.test_infer_splitk_vs_float64
+    (every distinct layer of the R50 inference forward at N = 1, 2, 3, 8, 24 and of C5 at N = 1, 2,
+    8): S = 1, S in {2, 3} and S >= 4 all occur, so the float64 test does not silently run S = 1
+    only.  At N = 256 (save_triangulations' batch) no call splits, on the H36M model and on C5."""
+    from tests import step_cases as sc
+    seen = set()
+    for keys, Ns in ((["c1", "h36m"], (1, 2, 3, 8, 24)), (["c5"], (1, 2, 8))):
+        for N in Ns:
+            for conv, hw in sc.infer_layers(keys):
+                seen.update(_planned(g)[0] for g in conv.fprop_geoms(em, N, hw, hw, 3) if g is not None)
+    assert 1 in seen and seen & {2, 3} and max(seen) >= 4, sorted(seen)
+    for key in ("h36m", "c5"):
+        HW = sc.INFER_MODELS[key][3]
+        assert all(_planned(g) == (1, 0) for _, g in es.conv16_calls(sc.infer_plan(key), 256, HW, HW)), key

@@ -5,8 +5,10 @@ against an exact restatement) at that composition's sizes.
 Each row of COMPOSITIONS runs one step of its composition at a reduced size and records the
 entries it calls: on the CPU through the emulated ABI (tests/emul_ops.py; the labels given, since
 the epipolar geometry has no CPU emulation) where the composition has one, and on the device with
-online labels.  A new composition is a new row; its float64 tests go in its own module, with the
-shared check bodies of tests/step_cases.py."""
+online labels.  The inference rows (predict, multiview_h36m, refined, validate_f16x3) run a
+predictor or validate_integral instead of a training step, construction included, and reject every
+backward, optimiser, loss and training-BatchNorm entry.  A new composition is a new row; its
+float64 tests go in its own module, with the shared check bodies of tests/step_cases.py."""
 import contextlib
 import importlib
 import inspect
@@ -163,6 +165,53 @@ COVERAGE_REFINER = {
 }
 # the refiner step's entries (refiner/main.py train() and the eval forward of test())
 REFINER = set(COVERAGE_REFINER)
+
+# the inference forward: PosePredictor and its subclasses on prepared weights (every conv on the
+# split-K entry), and validate_integral's eager eval forward with flip test
+S = "test_gpu_infer_step.py::"
+SK = "test_gpu_step_kernels.py::"
+C2 = "test_gpu_c2_flat_step.py::"
+EVAL_CHAIN = [S + "test_infer_eval_chain_vs_float64"]
+COVERAGE_PREDICT = {
+    "epb_pack_weight_batch": [SK + "test_pack_weight_batch_bit_exact_on_model_jobs",
+                              C2 + "test_c2_pack_weight_batch_bit_exact_on_model_jobs"],
+    "epb_split16_batch": [SK + "test_split16_batch_bit_exact_on_model_jobs",
+                          C2 + "test_c2_split16_batch_bit_exact_on_model_jobs"],
+    "epb_bn_eval_affine": [S + "test_infer_bn_eval_affine_within_one_ulp"],
+    "epb_im2col_split": [S + "test_infer_im2col_split_bit_exact"],
+    "epb_conv16_fprop_splitk": [S + "test_infer_splitk_vs_float64", S + "test_infer_splitk_ragged_final_writes_exactly_its_view",
+                                S + "test_infer_splitk_n256_is_the_fused_kernel"],
+    "epb_act_scale": EVAL_CHAIN,
+    "epb_bn_act_split": EVAL_CHAIN,
+    "epb_bn_relu_maxpool_split": EVAL_CHAIN,
+    "epb_softargmax_fwd": [S + "test_infer_softargmax_fwd_vs_float64"],
+    "epb_softargmax_flip_fwd": [S + "test_infer_softargmax_flip_vs_float64"],
+    "epb_patch_to_image": ["test_gpu_sizes.py::test_c3_selfsup_chain_64_images"],
+}
+COVERAGE_MULTIVIEW = dict(COVERAGE_PREDICT, epb_softargmax_flip_lse_fwd=[S + "test_infer_softargmax_flip_vs_float64"],
+                          epb_triangulate_robust=["test_gpu_multiview.py::test_kernel_vs_restatement"])
+R = "test_gpu_refiner.py::"
+COVERAGE_REFINED = dict(COVERAGE_PREDICT, epb_pose_to_camera=[R + "test_pose_to_camera_is_the_h36m_eval_pred_column"],
+                        epb_refiner_prepare=[R + "test_forward_vs_float64_oracle", R + "test_small_width_tails_vs_float64_oracle"],
+                        epb_refiner_forward=[R + "test_forward_vs_float64_oracle", R + "test_small_width_tails_vs_float64_oracle"])
+COVERAGE_VALIDATE = {k: v for k, v in COVERAGE_PREDICT.items() if k != "epb_conv16_fprop_splitk"}
+COVERAGE_VALIDATE.update(
+    epb_conv16_fprop=["test_gpu_split16.py::test_conv16_bench_layer_shapes_vs_torch_float64",
+                      "test_gpu_bn_chain.py::test_conv16_stats_vs_float64"],
+    epb_softargmax_flip_fwd=["test_gpu_flip.py::test_flip_kernel_vs_float64", S + "test_infer_softargmax_flip_vs_float64"])
+PREPARED = {"epb_conv16_fprop_splitk", "epb_bn_eval_affine", "epb_split16_batch", "epb_pack_weight_batch",
+            "epb_im2col_split", "epb_patch_to_image"}
+
+
+def _training_entry(e):
+    """backward, optimiser, loss and training-BatchNorm entries: no inference forward calls them"""
+    return e == "epb_split16" or any(k in e for k in ("bwd", "wgrad", "adam", "loss", "bn_finalize", "colsum",
+                                                      "sumsq", "clip_scale"))
+
+
+def _prepared_only(e):
+    """and the prepared forward runs every convolution on the split-K entry"""
+    return _training_entry(e) or e == "epb_conv16_fprop"
 
 
 def _missing_coverage(recorded, table):
@@ -396,6 +445,102 @@ def _refiner_device_step(dev, row):
     return _refiner_step(dev, row["device"])
 
 
+class _Predictors:
+    """the predictors a driver built inside the recorded call; _engine() checks them after it"""
+
+    def __init__(self):
+        self.preds = []
+
+    def _engine(self):
+        return self.preds
+
+
+def _prepared_engines(preds):
+    """every predictor runs Engine16 on a prepared state"""
+    from epipolarpose_b200 import net16
+    return bool(preds) and all(type(p.eng) is net16.Engine16 and p.state is not None and
+                               {"packed", "w16", "bn", "fbias"} <= set(p.state) for p in preds)
+
+
+def _images(N, seed, HW=256):
+    import numpy as np
+    return np.random.default_rng(seed).standard_normal((N, 3, HW, HW)).astype(np.float32)
+
+
+def _predict_step(dev, row):
+    """PosePredictor on the calibrated C1 model at N = 1, without and with flip test: construction
+    (prepare_inference), a capture and a replay each"""
+    from lib.core.inference import PosePredictor
+    from lib.dataset.synthetic import MPII_FLIP_PAIRS
+    model, holder, x = sc.calibrated_model(dev, "c1"), _Predictors(), _images(1, 3)
+
+    def run():
+        total = 0.0
+        for flip in (False, True):
+            p = PosePredictor(model, flip_test=flip, shift_heatmap=True, flip_pairs=MPII_FLIP_PAIRS)
+            total += float(abs(p(x)).sum())
+            holder.preds.append(p)
+        return total
+    return holder, run
+
+
+def _multiview_step(dev, row):
+    """MultiViewPredictor on the calibrated H36M model, 2 tuples x 4 views, flip test"""
+    from lib.core.inference import MultiViewPredictor
+    from lib.dataset.synthetic import H36M_FLIP_PAIRS
+    from tests import multiview_cases as mc
+    model, holder = sc.calibrated_model(dev, "h36m"), _Predictors()
+    x, boxes, P = mc.rig_inputs(2, 4, 5)
+
+    def run():
+        p = MultiViewPredictor(model, flip_test=True, shift_heatmap=True, flip_pairs=H36M_FLIP_PAIRS)
+        holder.preds.append(p)
+        return float(abs(p(x, boxes, P)["kps"]).sum())
+    return holder, run
+
+
+def _refined_step(dev, row):
+    """RefinedPosePredictor: the calibrated C1 model and a LinearModelPG(1024, 45 -> 45), N = 1"""
+    import numpy as np
+    from lib.core.inference import RefinedPosePredictor
+    from oracle import restate_refiner as rr
+    from refiner import model as rmodel
+    model, holder, x = sc.calibrated_model(dev, "c1"), _Predictors(), _images(1, 4)
+    rnet = rmodel.LinearModelPG(linear_size=1024, input_size=45, output_size=45)
+    rnet.load_state_dict(rr.init_state(rr.param_shapes(1024, 45, 45), 43))
+    rnet = rnet.to(dev)
+    norm = tuple(np.full(45, v, np.float32) for v in (3.0, 120.0, -2.0, 90.0))
+    boxes = {"center_x": [500.0], "center_y": [480.0], "width": [300.0], "height": [300.0]}
+    cams = {"fl": [[1145.0, 1144.0]], "c_p": [[512.0, 515.0]], "depth": [4500.0]}
+
+    def run():
+        p = RefinedPosePredictor(model, rnet, norm, flip_test=False)
+        holder.preds.append(p)
+        return float(abs(p(x, boxes, cams)["refined"]).sum())
+    return holder, run
+
+
+def _validate_step(dev, row):
+    """validate_integral with flip test (shifted) on the calibrated C1 model's eager Engine16 eval
+    forward, one batch of 4"""
+    import numpy as np
+    from lib.core.function import validate_integral
+    from lib.dataset.synthetic import MPII_FLIP_PAIRS
+    model, x = sc.calibrated_model(dev, "c1"), torch.from_numpy(_images(4, 6))
+
+    class _DS:
+        flip_pairs = MPII_FLIP_PAIRS
+
+        def __len__(self):
+            return 4
+
+    class _Loader(list):
+        dataset = _DS()
+
+    return model, lambda: float(np.abs(validate_integral(_Loader([(x,)]), model, flip_test=True,
+                                                         shift_heatmap=True)).sum())
+
+
 def _emulated_refiner_step(row):
     from tests import emul_ops
     return _refiner_step(torch.device("cpu"), row["emulated"], ops=emul_ops)
@@ -458,6 +603,30 @@ COMPOSITIONS = {
         engine=_mlp_engine, tags=_refiner_convs,
         tag_examples=(REFINER_TAGS, [REFINER_TAGS | {"fprop_tc<128,1>"}, REFINER_TAGS | {"wgrad_tc<128,1>"}]
                       + [REFINER_TAGS - {t} for t in sorted(REFINER_TAGS)] + [{"fprop_simt", "wgrad_simt"}, set()])),
+    # inference (lib/core/inference.py): construction, a capture and a replay inside the recorded call
+    "predict": dict(
+        table=COVERAGE_PREDICT, precision="f16x3", method=None, views=None, driver=_predict_step,
+        emulated=None, device=(50, 16, 64, 256, 1),
+        calls=PREPARED | {"epb_softargmax_fwd", "epb_softargmax_flip_fwd"}, online=set(),
+        not_called=_prepared_only, engine=_prepared_engines, tags=None),
+    "multiview_h36m": dict(
+        table=COVERAGE_MULTIVIEW, precision="f16x3", method=None, views=4, driver=_multiview_step,
+        emulated=None, device=(50, 17, 64, 256, 2),
+        calls=PREPARED | {"epb_softargmax_flip_lse_fwd", "epb_triangulate_robust"}, online=set(),
+        not_called=_prepared_only, engine=_prepared_engines, tags=None),
+    "refined": dict(
+        table=COVERAGE_REFINED, precision="f16x3", method=None, views=None, driver=_refined_step,
+        emulated=None, device=(50, 16, 64, 256, 1),
+        calls=PREPARED | {"epb_pose_to_camera", "epb_refiner_prepare", "epb_refiner_forward"}, online=set(),
+        not_called=_prepared_only, engine=_prepared_engines, tags=None),
+    # validate_integral with flip test: the eager eval forward (fused conv16, bn_eval_affine per
+    # forward).  Device only: the emulated ABI has no epb_softargmax_flip_fwd
+    "validate_f16x3": dict(
+        table=COVERAGE_VALIDATE, precision="f16x3", method=None, views=None, driver=_validate_step,
+        emulated=None, device=(50, 16, 64, 256, 1),
+        calls={"epb_conv16_fprop", "epb_bn_eval_affine", "epb_softargmax_flip_fwd"}, online=set(),
+        not_called=lambda e: _training_entry(e) or e == "epb_conv16_fprop_splitk",
+        engine=lambda eng: type(eng).__name__ == "Engine16", tags=None),
 }
 EMULATED = [k for k, row in COMPOSITIONS.items() if row["emulated"] is not None]
 
@@ -524,11 +693,10 @@ def dev():
 def test_gate_device_step(dev, comp):
     """One step of the composition at a reduced batch (2 tuples x 4 views) with online labels, on
     the device.  Every entry it calls has a row naming existing tests; where the row has a tag
-    predicate, the step runs under the profiler and the conv kernels that ran must meet it."""
+    predicate, the step runs under the profiler and the conv kernels that ran must meet it.  The
+    engine predicate is checked after the step, which builds the inference rows' predictors."""
     row = COMPOSITIONS[comp]
     m, run = row["driver"](dev, row)
-    if row["engine"] is not None:
-        assert row["engine"](m._engine())
     losses, tags = [], None
     with sc._record_calls() as names:
         if row["tags"] is None:
@@ -536,6 +704,8 @@ def test_gate_device_step(dev, comp):
         else:
             tags = sc._ran(lambda: losses.append(float(run())))
         torch.cuda.synchronize()
+    if row["engine"] is not None:
+        assert row["engine"](m._engine())
     assert losses and all(math.isfinite(v) for v in losses)
     if tags is not None:
         print("  conv kernels %s" % sorted(tags))
