@@ -471,7 +471,9 @@ def validate_integral(val_loader, model, flip_test=None, shift_heatmap=None):
     return out[0:len(val_loader.dataset)]
 
 
-def eval_integral(epoch, preds_in_patch_with_score, val_loader, final_output_path, debug=False):
+def eval_integral(epoch, preds_in_patch_with_score, val_loader, final_output_path, debug=False, with_names=False):
+    """perf of the dataset's evaluate, or (perf, [(name, value), ..]) with `with_names`: the values it
+    logs, at full precision."""
     print("Evaluation stage")
     imdb_list = val_loader.dataset.db
     imdb = val_loader.dataset
@@ -483,6 +485,8 @@ def eval_integral(epoch, preds_in_patch_with_score, val_loader, final_output_pat
     name_value, perf = imdb.evaluate(preds_in_img_with_score.copy(), final_output_path, debug=debug)
     for name, value in name_value:
         logger.info('Epoch[%d] Validation-%s %f', epoch, name, value)
+    if with_names:
+        return perf, [(name, float(value)) for name, value in name_value]
     return perf
 
 
