@@ -63,7 +63,9 @@ _PROTOS = {
     "epb_argmax2d": (c_int, [c_p, c_int, c_int, c_int, c_p, c_p, c_p, c_p]),
     "epb_final_preds": (c_int, [c_p, c_int, c_int, c_int, c_int, c_p, c_p, c_int, c_p, c_p, c_p]),
     "epb_patch_to_image": (c_int, [c_p, c_p, c_int, c_int, c_d, c_d, c_d, c_p, c_p]),
-    "epb_triangulate": (c_int, [c_p, c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p]),
+    "epb_heatmap_decode": (c_int, [c_p, c_int, c_int, c_p, c_int, c_p] + [c_int] * 5 + [c_d] * 3 +
+                           [c_int, ctypes.POINTER(c_int), c_int, c_p, c_p]),
+    "epb_triangulate":(c_int, [c_p, c_p, c_int, c_p, c_p, c_int, c_int, c_int, c_d, c_p, c_p, c_p]),
     "epb_triangulate_nview": (c_int, [c_p, c_int, c_p, c_int, c_int, c_int, c_p, c_p, c_p]),
     "epb_relative_pose": (c_int, [c_p, c_int, c_p, c_p, c_int, c_int, c_d, c_p, c_p, c_p, c_p, c_p, c_p,
                                   c_p]),

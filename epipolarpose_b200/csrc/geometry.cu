@@ -621,6 +621,17 @@ __host__ __device__ void patch_affine(const double* box, double patch_w, double 
   }
 }
 
+// A patch pixel (px, py) of a sample with box [6] -> image point k [2].  Shared by the soft-argmax
+// (volume) and heat-map decodes, so both heads map the same patch point to the same image point.
+__host__ __device__ inline void patch_px_to_image(double px, double py, const double* box, double patch_w,
+                                                  double patch_h, double* k) {
+  double M[2][3];
+  patch_affine(box, patch_w, patch_h, 1, M);
+  // img_utils.py:108-111 np.dot(trans, [x, y, 1])
+  k[0] = (M[0][0] * px + M[0][1] * py) + M[0][2];
+  k[1] = (M[1][0] * px + M[1][1] * py) + M[1][2];
+}
+
 // One soft-argmax coordinate c [3] (normalised) of a sample with box [6] -> image point k [4] =
 // (x px, y px, z mm, 1).  Shared by patch_to_image_kernel and the tuple-label entry.
 __host__ __device__ inline void patch_to_image_point(const float* c, const double* box, double patch_w,
@@ -629,11 +640,7 @@ __host__ __device__ inline void patch_to_image_point(const float* c, const doubl
   const double px = ((double)c[0] + 0.5) * patch_w;
   const double py = ((double)c[1] + 0.5) * patch_h;
   const double pz = (double)c[2] * patch_w;
-  double M[2][3];
-  patch_affine(box, patch_w, patch_h, 1, M);
-  // img_utils.py:108-111 np.dot(trans, [x, y, 1])
-  k[0] = (M[0][0] * px + M[0][1] * py) + M[0][2];
-  k[1] = (M[1][0] * px + M[1][1] * py) + M[1][2];
+  patch_px_to_image(px, py, box, patch_w, patch_h, k);
   k[2] = pz / patch_w * rect3d_w;  // img_utils.py:154
   k[3] = 1.0;
 }
@@ -1582,6 +1589,202 @@ __global__ void argmax2d_kernel(const float* __restrict__ hm, int NJ, int HW, in
   }
 }
 
+// ---------------------------------------------------------------- heat-map decode
+// The MODEL.VOLUME = false head -> joints (reference lib/core/inference.py:12-68 get_max_preds /
+// get_final_preds and :144-170 get_depth_preds).  One CTA per image reads all J maps of it: the
+// channels-last [h][w][C] rows of the split-fp16 final conv in place (threads over channels, so a
+// warp reads whole pixel rows; channels >= J are never read), or the NCHW maps one warp per
+// (joint, pixel chunk).  The per-joint bodies below are __host__ __device__:
+// tests/harness/host_heatmap_decode.cu runs them on the CPU.
+constexpr int kHmDecThreads = 512;
+constexpr int kHmDecMaxJ = 1024;
+
+struct HmPerm {
+  unsigned short p[kHmDecMaxJ];
+};
+
+struct HmDec {
+  const float* hm;        // layout 0: [B][J][H][W]; layout 1: [B][H][W][C]
+  const float* depth;     // [B][depth_ld], joint j's logits at j*D .. j*D+D-1
+  const double* box;      // [N][6] or null (patch frame)
+  int layout, C, depth_ld, N, J, H, W, D, post_process, flip, shift;
+  double patch_w, patch_h, depth_range;
+};
+
+__host__ __device__ inline float hm_load(const HmDec& a, int n, int j, int pix) {
+  const int64_t HW = (int64_t)a.H * a.W;
+  return a.layout == 0 ? a.hm[((int64_t)n * a.J + j) * HW + pix] : a.hm[((int64_t)n * HW + pix) * a.C + j];
+}
+
+// the decoded map of (n, j) at (y, x): with flip test 0.5 (a + flip_back(b)), flip_back mirroring the
+// columns of the paired joint's map of image n + N, shifted one column right when `shift` (column 0
+// keeps its own mirror, transforms.py:5-19 and the Simple Baselines merge)
+__host__ __device__ inline float hm_value(const HmDec& a, const unsigned short* perm, int n, int j, int y, int x) {
+  const float v = hm_load(a, n, j, y * a.W + x);
+  if (!a.flip) return v;
+  const int xf = a.shift ? (x == 0 ? a.W - 1 : a.W - x) : a.W - 1 - x;
+  return 0.5f * (v + hm_load(a, n + a.N, perm[j], y * a.W + xf));
+}
+
+// numpy argmax order: the first NaN, else the largest value, first index on ties (argmax2d_kernel)
+__host__ __device__ inline bool hm_better(float v, int i, float bv, int bi) {
+  const bool vn = (v != v), bn = (bv != bv);
+  if (vn || bn) return vn && (!bn || i < bi);
+  return v > bv || (v == bv && i < bi);
+}
+
+// x, y and maxval of joint (n, j) from its argmax (bv, bi) -> k [4] (k[2] is the depth's)
+__host__ __device__ inline void hm_finish_joint(const HmDec& a, const unsigned short* perm, int n, int j,
+                                                float bv, int bi, double* k) {
+  if (bi == 0x7fffffff) bi = 0;                   // all -inf: numpy returns index 0
+  const int W = a.W, H = a.H;
+  const float mask = (bv > 0.f) ? 1.f : 0.f;      // inference.py:35-39
+  float cx = (float)(bi % W) * mask, cy = floorf((float)bi / (float)W) * mask;
+  if (a.post_process) {                           // :49-61
+    const int px = (int)floor((double)cx + 0.5), py = (int)floor((double)cy + 0.5);
+    if (1 < px && px < W - 1 && 1 < py && py < H - 1) {
+      const float dx = hm_value(a, perm, n, j, py, px + 1) - hm_value(a, perm, n, j, py, px - 1);
+      const float dy = hm_value(a, perm, n, j, py + 1, px) - hm_value(a, perm, n, j, py - 1, px);
+      cx += (dx > 0.f ? 0.25f : (dx < 0.f ? -0.25f : 0.f));
+      cy += (dy > 0.f ? 0.25f : (dy < 0.f ? -0.25f : 0.f));
+    }
+  }
+  // heat-map px -> patch px, then the inverse patch affine of epb_patch_to_image
+  const double px = (double)cx * (a.patch_w / (double)W), py = (double)cy * (a.patch_h / (double)H);
+  if (a.box) {
+    patch_px_to_image(px, py, a.box + (int64_t)n * 6, a.patch_w, a.patch_h, k);
+  } else {
+    k[0] = px;
+    k[1] = py;
+  }
+  k[3] = (double)bv;
+}
+
+// e^x for x <= 0 with + - * / and an exact power-of-two scaling only, so that the device and the
+// host round alike (relative error ~1e-16; 0 below -700, where a term no longer counts)
+__host__ __device__ inline double exp_nonpos(double x) {
+  if (!(x > -700.0)) return 0.0;
+  const double kf = floor(x * 1.4426950408889634 + 0.5);
+  const double r = (x - kf * 6.93147180369123816490e-01) - kf * 1.90821492927058770002e-10;
+  double p = 1.0 / 6227020800.0;                  // 1/13!
+  const double inv[13] = {1.0 / 479001600.0, 1.0 / 39916800.0, 1.0 / 3628800.0, 1.0 / 362880.0,
+                          1.0 / 40320.0, 1.0 / 5040.0, 1.0 / 720.0, 1.0 / 120.0, 1.0 / 24.0,
+                          1.0 / 6.0, 0.5, 1.0, 1.0};
+#pragma unroll
+  for (int i = 0; i < 13; ++i) p = p * r + inv[i];
+  return ldexp(p, (int)kf);
+}
+
+__host__ __device__ inline float depth_logit(const HmDec& a, const unsigned short* perm, int n, int j, int k) {
+  const float v = a.depth[(int64_t)n * a.depth_ld + (int64_t)j * a.D + k];
+  if (!a.flip) return v;
+  return 0.5f * (v + a.depth[(int64_t)(n + a.N) * a.depth_ld + (int64_t)perm[j] * a.D + k]);
+}
+
+// get_depth_preds, max-subtracted: lane l of 32 sums the bins k = l, l + 32, .. in float64
+// (s = sum e, t = sum k e, e = exp(v_k - m)); lane 0 adds the 32 partials in lane order
+__host__ __device__ inline void depth_lane(const HmDec& a, const unsigned short* perm, int n, int j, int lane,
+                                           float m, double* s, double* t) {
+  double ss = 0.0, tt = 0.0;
+  for (int k = lane; k < a.D; k += 32) {
+    const double e = exp_nonpos((double)depth_logit(a, perm, n, j, k) - (double)m);
+    ss += e;
+    tt += (double)k * e;
+  }
+  *s = ss;
+  *t = tt;
+}
+
+__host__ __device__ inline double depth_finish(const HmDec& a, const double* s, const double* t) {
+  double ss = 0.0, tt = 0.0;
+  for (int l = 0; l < 32; ++l) {
+    ss += s[l];
+    tt += t[l];
+  }
+  return (tt / ss / (double)a.D - 0.5) * a.depth_range;   // inference.py:160-162
+}
+
+__global__ void __launch_bounds__(1024)
+heatmap_decode_kernel(const HmDec a, const HmPerm pi, double* __restrict__ kps) {
+  __shared__ float sv[1024];
+  __shared__ int si[1024];
+  __shared__ double sd[32][2][32];
+  __shared__ unsigned short perm[kHmDecMaxJ];
+  const int n = blockIdx.x, J = a.J, HW = a.H * a.W;
+  const int T = blockDim.x, lane = threadIdx.x & 31, wid = threadIdx.x >> 5, nw = T >> 5;
+  if (a.flip)
+    for (int j = threadIdx.x; j < J; j += T) perm[j] = pi.p[j];
+  __syncthreads();
+  // ---- argmax partials
+  int per_joint, stride;                           // partial q of joint j at sv[j * stride0 + q * stride]
+  int stride0;
+  if (a.layout == 1) {
+    const int C = a.C, ppi = T / C;                // T = ceil32(C * ppi)
+    const int c = threadIdx.x % C, sub = threadIdx.x / C;
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    if (sub < ppi && c < J) {
+      int pix = sub, y = pix / a.W, x = pix - y * a.W;
+      const int dy = ppi / a.W, dx = ppi - dy * a.W;
+      for (; pix < HW; pix += ppi) {
+        const float v = hm_value(a, perm, n, c, y, x);
+        if (hm_better(v, pix, bv, bi)) { bv = v; bi = pix; }
+        x += dx;
+        y += dy;
+        if (x >= a.W) { x -= a.W; ++y; }
+      }
+    }
+    sv[threadIdx.x] = bv;
+    si[threadIdx.x] = bi;
+    per_joint = ppi; stride0 = 1; stride = C;
+  } else {
+    const int P = nw / J > 1 ? nw / J : 1;        // warps per joint map
+    const int chunk = (HW + P - 1) / P;
+    for (int w = wid; w < J * P; w += nw) {
+      const int j = w / P, q = w - j * P;
+      const int end = min(HW, (q + 1) * chunk);
+      float bv = -INFINITY;
+      int bi = 0x7fffffff;
+      for (int pix = q * chunk + lane; pix < end; pix += 32) {
+        const int y = pix / a.W;
+        const float v = hm_value(a, perm, n, j, y, pix - y * a.W);
+        if (hm_better(v, pix, bv, bi)) { bv = v; bi = pix; }
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv, o);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi, o);
+        if (hm_better(ov, oi, bv, bi)) { bv = ov; bi = oi; }
+      }
+      if (lane == 0) { sv[w] = bv; si[w] = bi; }
+    }
+    per_joint = P; stride0 = P; stride = 1;
+  }
+  __syncthreads();
+  // ---- per joint: merge the partials (a total order: the result does not depend on the partition),
+  // refinement, patch -> image
+  for (int j = threadIdx.x; j < J; j += T) {
+    float bv = -INFINITY;
+    int bi = 0x7fffffff;
+    for (int q = 0; q < per_joint; ++q) {
+      const int e = j * stride0 + q * stride;
+      if (hm_better(sv[e], si[e], bv, bi)) { bv = sv[e]; bi = si[e]; }
+    }
+    hm_finish_joint(a, perm, n, j, bv, bi, kps + ((int64_t)n * J + j) * 4);
+  }
+  // ---- depth: one warp per joint
+  for (int j = wid; j < J; j += nw) {
+    float m = -INFINITY;
+    for (int k = lane; k < a.D; k += 32) m = fmaxf(m, depth_logit(a, perm, n, j, k));
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+    depth_lane(a, perm, n, j, lane, m, &sd[wid][0][lane], &sd[wid][1][lane]);
+    __syncwarp();
+    if (lane == 0) kps[((int64_t)n * J + j) * 4 + 2] = depth_finish(a, sd[wid][0], sd[wid][1]);
+    __syncwarp();
+  }
+}
+
 }  // namespace
 
 extern "C" __attribute__((visibility("default"))) int epb_triangulate(const double* u1, const double* u2, int stride_u, const double* P1,
@@ -1656,6 +1859,43 @@ extern "C" __attribute__((visibility("default"))) int epb_argmax2d(const float* 
   const int threads = 256;
   const int blocks = (NJ * 32 + threads - 1) / threads;
   argmax2d_kernel<<<blocks, threads, 0, as_stream(stream)>>>(hm, NJ, H * W, W, idx, maxval, preds);
+  EPB_LAUNCH_CHECK();
+  return EPB_OK;
+}
+
+extern "C" __attribute__((visibility("default"))) int epb_heatmap_decode(
+    const float* hm, int layout, int C, const float* depth, int depth_ld, const double* box, int N, int J,
+    int H, int W, int D, double patch_w, double patch_h, double depth_range, int post_process,
+    const int* perm_host, int shift, double* kps, epb_stream_t stream) {
+  EPB_CHECK_ARG(hm && depth && kps);
+  EPB_CHECK_ARG(N >= 0 && J > 0 && J <= kHmDecMaxJ && H > 0 && W > 0 && D > 0);
+  EPB_CHECK_ARG((int64_t)H * W < (1LL << 31) && (int64_t)J * D <= depth_ld);
+  EPB_CHECK_ARG(layout == 0 || (layout == 1 && C >= J && C <= kHmDecMaxJ));
+  EPB_CHECK_ARG(patch_w > 0 && patch_h > 0);
+  EPB_CHECK_ARG(shift == 0 || shift == 1);
+  if (N == 0) return EPB_OK;
+  HmPerm pi;
+  if (perm_host) {
+    for (int j = 0; j < J; ++j) {
+      const int q = perm_host[j];
+      if (q < 0 || q >= J || perm_host[q] != j) {
+        epb_set_error("epb_heatmap_decode: perm is not an involution of [0, %d) at joint %d", J, j);
+        return EPB_EINVAL;
+      }
+      pi.p[j] = (unsigned short)q;
+    }
+  }
+  HmDec a;
+  a.hm = hm; a.depth = depth; a.box = box;
+  a.layout = layout; a.C = C; a.depth_ld = depth_ld; a.N = N; a.J = J; a.H = H; a.W = W; a.D = D;
+  a.post_process = post_process ? 1 : 0; a.flip = perm_host ? 1 : 0; a.shift = shift;
+  a.patch_w = patch_w; a.patch_h = patch_h; a.depth_range = depth_range;
+  int threads = kHmDecThreads;
+  if (layout == 1) {
+    const int ppi = kHmDecThreads / C > 0 ? kHmDecThreads / C : 1;   // pixels per pass
+    threads = (C * ppi + 31) / 32 * 32;
+  }
+  heatmap_decode_kernel<<<N, threads, 0, as_stream(stream)>>>(a, pi, kps);
   EPB_LAUNCH_CHECK();
   return EPB_OK;
 }

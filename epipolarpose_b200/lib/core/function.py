@@ -25,7 +25,12 @@ Differences from the reference body (same observable behaviour):
   * validate_integral honours TEST.FLIP_TEST and TEST.SHIFT_HEATMAP (reference
     config.py:118,120, read nowhere by the reference): each batch is one forward of
     [x; flip(x)] and the logits are merged with their flipped-back mirror before the
-    soft-argmax (integral_loss.get_joint_location_result_flip).
+    soft-argmax (integral_loss.get_joint_location_result_flip);
+  * a MODEL.VOLUME = false network, which the reference's result function cannot decode, is
+    validated through the heat-map decode (inference.get_heatmap_location_result's rows: the
+    get_final_preds argmax and refinement, get_depth_preds as the root-relative depth, the heat-map
+    maximum as score), with flip test merged inside the decode; eval_integral scores those rows
+    unchanged.
 """
 import logging
 import time
@@ -36,6 +41,7 @@ import torch
 from ..utils.img_utils import (self_supervision_device,
                                trans_coords_from_patch_to_org_3d_batch)
 from .integral_loss import get_joint_location_coords_flip, get_result_func, joint_location_result_from_coords
+from .inference import check_heatmap_head, heatmap_decode_device, heatmap_rows
 from ..utils.utils import AverageMeter
 from ..dataset.deferred import assemble_batch, cat_meta, is_deferred, view_keys
 from .refine import export_refiner_pairs  # noqa: F401  (public here, next to eval_integral)
@@ -418,9 +424,9 @@ def _validate_flip(val_loader, model, shift_heatmap):
     """Flip-test validation: one forward of the 2B images [x; flip(x, 3)] per batch, merged
     coordinates kept on the device, one copy to the host after the loop."""
     net = getattr(model, 'module', model)
-    if not getattr(net, 'volume', True):
-        raise ValueError("flip test needs the VOLUME head (MODEL.VOLUME: true); the reference's "
-                         "result function has no flip merge for 2-D heat-maps")
+    flat = not getattr(net, 'volume', True)
+    if flat:
+        check_heatmap_head(net)
     pairs = _flip_pairs(val_loader.dataset)
     if pairs is None:
         raise ValueError("flip test needs the dataset's joint pairs: neither dataset.flip_pairs nor "
@@ -436,13 +442,45 @@ def _validate_flip(val_loader, model, shift_heatmap):
             buf[:B].copy_(x, non_blocking=True)
             buf[B:] = torch.flip(buf[:B], [3])
             preds = model(buf)
-            chunks.append(get_joint_location_coords_flip(preds, pairs, shift_heatmap))
+            if flat:
+                chunks.append(_heatmap_decode(preds, pairs, shift_heatmap))
+            else:
+                chunks.append(get_joint_location_coords_flip(preds, pairs, shift_heatmap))
             del preds, buf
     if not chunks:
         return np.zeros((0, 0, 4))
+    if flat:
+        return heatmap_rows(torch.cat(chunks, dim=0).cpu().numpy(), 256)[0:len(val_loader.dataset)]
     coords = torch.cat(chunks, dim=0).cpu().numpy()
     out = joint_location_result_from_coords(256, 256, coords)     # hard-coded 256 as reference :87
     return out[0:len(val_loader.dataset)]
+
+
+def _heatmap_decode(preds, flip_pairs=None, shift_heatmap=False):
+    """(heatmaps, depth) of a MODEL.VOLUME = false network -> kps [N, J, 4] on the device (patch px,
+    root-relative mm, maxval): epb_heatmap_decode with the config's DEPTH_RES, DEPTH_RANGE and
+    TEST.POST_PROCESS."""
+    from .config import config
+    hm, depth = preds
+    return heatmap_decode_device(hm, depth, int(config.MODEL.DEPTH_RES), None, 256, 256,
+                                 float(config.DATASET.DEPTH_RANGE), bool(config.TEST.POST_PROCESS),
+                                 flip_pairs, shift_heatmap)
+
+
+def _validate_heatmap(val_loader, model):
+    """Validation of a MODEL.VOLUME = false network: the heat-map decode of each batch kept on the
+    device, one copy to the host after the loop; rows as get_heatmap_location_result."""
+    check_heatmap_head(getattr(model, 'module', model))
+    model.eval()
+    chunks = []
+    with torch.no_grad():
+        for data in val_loader:
+            batch_data = loader_batch(data)[0].cuda(non_blocking=True)
+            chunks.append(_heatmap_decode(model(batch_data)))
+            del batch_data
+    if not chunks:
+        return np.zeros((0, 0, 4))
+    return heatmap_rows(torch.cat(chunks, dim=0).cpu().numpy(), 256)[0:len(val_loader.dataset)]   # 256 as :87
 
 
 def validate_integral(val_loader, model, flip_test=None, shift_heatmap=None):
@@ -456,6 +494,8 @@ def validate_integral(val_loader, model, flip_test=None, shift_heatmap=None):
     print("Validation stage")
     if flip_test:
         return _validate_flip(val_loader, model, shift_heatmap)
+    if not getattr(getattr(model, 'module', model), 'volume', True):
+        return _validate_heatmap(val_loader, model)
     result_func = get_result_func()
     model.eval()
     chunks = []

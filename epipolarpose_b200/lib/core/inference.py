@@ -9,7 +9,10 @@ Addition: `PosePredictor`, images -> 3-D joints as one CUDA-graph replay per cal
 `MultiViewPredictor`: the calibrated views of a rig -> world-frame joints, the same network on
 every view followed by the robust V-view triangulation inside the same graph.
 `RefinedPosePredictor`: images, boxes and cameras -> camera-frame poses and their refinement by the
-paper's refinement unit, in one graph."""
+paper's refinement unit, in one graph.
+The MODEL.VOLUME = false head: `get_depth_preds` (reference :144-170), `get_heatmap_location_result`
+and `HeatmapPredictor`, all on the fused decode epb_heatmap_decode (argmax, refinement, depth
+soft-argmax, patch -> image)."""
 import numpy as np
 import torch
 
@@ -71,6 +74,103 @@ def get_final_preds(config, batch_heatmaps, center, scale):
     preds, maxvals = get_final_preds_device(hm, np.asarray(center), scale,
                                             config.TEST.POST_PROCESS)
     return preds.cpu().numpy(), maxvals.cpu().numpy().astype(batch_heatmaps.dtype)
+
+
+RECT_3D_W = 2000.0                  # eval_integral's rect_3d_w: z (patch units) / patch_w * 2000 = mm
+
+
+def heatmap_decode_device(heatmaps, depth, depth_res, box=None, patch_width=256, patch_height=256,
+                          depth_range=2000.0, post_process=True, flip_pairs=None, shift_heatmap=False,
+                          out=None):
+    """The MODEL.VOLUME = false head's output -> joints on the device in one launch
+    (epb_heatmap_decode).  heatmaps [B, J, H, W] float32 CUDA, either contiguous or the NCHW view of a
+    channels-last [B, H, W, C] buffer (C >= J, as the split-fp16 final conv writes it: read in place);
+    depth [B, J*depth_res] float32 rows.  box: [N, 6] float64 (c_x, c_y, width, height, scale, rot)
+    for image coordinates, None for patch pixels.  flip_pairs: the batch is [x; flip(x)] (B = 2N) and
+    each map / depth row is merged with its flipped-back mirror (shifted one column with
+    shift_heatmap) before the decode.  -> kps [N, J, 4] float64 = (x, y, root-relative depth mm,
+    maxval)."""
+    from .integral_loss import flip_permutation
+    B, J, H, W = heatmaps.shape
+    N = B // 2 if flip_pairs is not None else B
+    if flip_pairs is not None and B != 2 * N:
+        raise ValueError("flip test needs a batch of 2N rows [x; flip(x)], got %d" % B)
+    s = heatmaps.stride()
+    if heatmaps.is_contiguous():
+        layout, C, store = 0, J, heatmaps
+    elif s[1] == 1 and s[3] >= J and s[2] == W * s[3] and s[0] == H * W * s[3]:
+        C = s[3]
+        layout = 1
+        store = heatmaps.as_strided((B, H, W, C), (H * W * C, W * C, C, 1))
+        if not store.is_contiguous():
+            raise ValueError("channels-last heat-maps must be a dense [B, H, W, C] buffer")
+    else:
+        raise ValueError("heat-maps must be contiguous NCHW or an NCHW view of a channels-last buffer")
+    if depth.dim() != 2 or depth.shape[0] != B or depth.shape[1] < J * depth_res or depth.stride(1) != 1 \
+            or depth.stride(0) < J * depth_res:
+        raise ValueError("expected depth rows [%d, >= %d], got %s" % (B, J * depth_res, tuple(depth.shape)))
+    depth_store = depth.as_strided((B, depth.stride(0)), (depth.stride(0), 1))
+    if out is None:
+        out = torch.empty((N, J, 4), device=heatmaps.device, dtype=torch.float64)
+    perm = flip_permutation(flip_pairs, J) if flip_pairs is not None else None
+    _ops.heatmap_decode(store, layout, C, depth_store, depth.stride(0), box, N, J, H, W, depth_res,
+                        patch_width, patch_height, depth_range, post_process, perm, bool(shift_heatmap), out)
+    return out
+
+
+def check_heatmap_head(net):
+    """ValueError unless `net` is a MODEL.VOLUME = false network whose depth branch can run: depth_fc
+    (reference pose3d_resnet.py:126, nn.Linear(2048, J*D)) reads the average-pooled trunk, which has
+    2048 channels only for the bottleneck ResNets (50 and deeper).  A basic-block trunk (ResNet-18 / 34,
+    512 channels) has no depth for the decode: the reference's forward fails there too, and the depth
+    kernels would read past the trunk."""
+    plan = net._plan
+    if plan.fc is None:
+        raise ValueError("the heat-map decode needs the MODEL.VOLUME: false head; for a VOLUME model use "
+                         "PosePredictor / the soft-argmax")
+    if plan.trunk_channels != plan.fc.cin:
+        raise ValueError("MODEL.VOLUME: false needs a %d-channel trunk for depth_fc (ResNet-50 or deeper); this "
+                         "network's trunk has %d channels" % (plan.fc.cin, plan.trunk_channels))
+
+
+def get_depth_preds(cfg, pred):
+    """reference :144-166: depth logits [N, J*D] (numpy) -> root-relative depth [N, J] float64 in mm,
+    the soft-argmax d = (s / D - 0.5) * DATASET.DEPTH_RANGE (computed with the maximum subtracted, so
+    logits above ~88, where the reference's exp overflows, still decode)."""
+    J, D = int(cfg.MODEL.NUM_JOINTS), int(cfg.MODEL.DEPTH_RES)
+    p = np.ascontiguousarray(np.asarray(pred, dtype=np.float32).reshape(-1, J * D))
+    N = p.shape[0]
+    if N == 0:
+        return np.zeros((0, J))
+    dev = torch.device("cuda")
+    hm = torch.zeros((N, J, 1, 1), device=dev, dtype=torch.float32)      # the 2-D half has one pixel
+    kps = heatmap_decode_device(hm, torch.from_numpy(p).to(dev), D, depth_range=float(cfg.DATASET.DEPTH_RANGE),
+                                post_process=False)
+    return kps[:, :, 2].cpu().numpy()
+
+
+def heatmap_rows(kps, patch_width):
+    """kps [N, J, 4] (patch px, mm, maxval) -> validate_integral's rows: z in patch units."""
+    out = np.asarray(kps, dtype=np.float64).copy()
+    out[:, :, 2] = out[:, :, 2] / RECT_3D_W * patch_width
+    return out
+
+
+def get_heatmap_location_result(patch_width, patch_height, preds, depth_res=None, depth_range=None,
+                                post_process=None, flip_pairs=None, shift_heatmap=False):
+    """The MODEL.VOLUME = false counterpart of get_joint_location_result: preds = (heatmaps [N, J, h, w],
+    depth [N, J*D]) -> numpy float64 [N, J, 4] in validate_integral's units: x, y in patch pixels,
+    z in patch units (eval_integral's z / patch_width * 2000 is the root-relative depth in mm) and
+    the heat-map maximum as score.  depth_res, depth_range and post_process default to the
+    config's MODEL.DEPTH_RES, DATASET.DEPTH_RANGE and TEST.POST_PROCESS; flip_pairs / shift_heatmap
+    as heatmap_decode_device."""
+    from .config import config
+    hm, depth = preds
+    D = int(config.MODEL.DEPTH_RES if depth_res is None else depth_res)
+    rng = float(config.DATASET.DEPTH_RANGE if depth_range is None else depth_range)
+    pp = bool(config.TEST.POST_PROCESS) if post_process is None else bool(post_process)
+    kps = heatmap_decode_device(hm, depth, D, None, patch_width, patch_height, rng, pp, flip_pairs, shift_heatmap)
+    return heatmap_rows(kps.cpu().numpy(), patch_width)
 
 
 class PosePredictor:
@@ -392,3 +492,99 @@ class RefinedPosePredictor(PosePredictor):
             kps = np.ones((N, 16, 4), dtype=np.float64)
             kps[:, :, :3] = ent["kps"][:, :, :3].cpu().numpy()
             return {"kps": kps, "pose": ent["pose"].cpu().numpy(), "refined": ent["refined"].cpu().numpy()}
+
+
+class HeatmapPredictor(PosePredictor):
+    """Images -> joints for the MODEL.VOLUME = false head (2-D heat-maps + depth_fc logits), one
+    CUDA-graph replay per (N, H, W): the prepared split-fp16 network (its depth branch on the
+    average-pooled trunk) and epb_heatmap_decode (argmax, the get_final_preds refinement,
+    get_depth_preds, patch -> image).  Snapshot, refresh() and eval-BatchNorm semantics as
+    PosePredictor.
+
+    pred(images): images float32 [N, 3, H, W] (host or device) -> numpy float64 [N, J, 4], the rows
+    of get_heatmap_location_result(W, H, model.eval()(images)): x, y in patch pixels, z in patch
+    units (z / W * 2000 = root-relative depth in mm) and the heat-map maximum.  pred(images,
+    boxes=meta): meta as PosePredictor; rows (image x, image y, root-relative depth mm, maxval).
+    flip_test / shift_heatmap / flip_pairs as PosePredictor (the 2N batch [x; flip(x)], merged inside
+    the decode); post_process defaults to config.TEST.POST_PROCESS.
+    pred.heatmaps [N or 2N, J, h, w] (an NCHW view of the channels-last buffer) and pred.depth
+    [N or 2N, J*D]: the static outputs of the last call, overwritten by the next call with the same N."""
+
+    def __init__(self, model, flip_test=None, shift_heatmap=None, flip_pairs=None, post_process=None):
+        from .config import config
+        from .integral_loss import flip_permutation
+        net = getattr(model, "module", model)
+        if getattr(net, "volume", True):
+            raise ValueError("HeatmapPredictor decodes the 2-D heat-map head (MODEL.VOLUME: false); "
+                             "for a VOLUME model use PosePredictor")
+        if getattr(net, "precision", None) != 4:
+            raise ValueError("HeatmapPredictor runs the split-fp16 engine (MODEL.PRECISION: f16x3); "
+                             "this model runs another precision")
+        if not _net16.supported(net._plan):
+            raise ValueError("HeatmapPredictor runs the split-fp16 engine, which needs every layer's "
+                             "channels in whole 64-channel blocks; this model's plan has others")
+        check_heatmap_head(net)
+        self.flip_test = bool(config.TEST.FLIP_TEST) if flip_test is None else bool(flip_test)
+        self.shift_heatmap = bool(config.TEST.SHIFT_HEATMAP) if shift_heatmap is None \
+            else bool(shift_heatmap)
+        self.post_process = bool(config.TEST.POST_PROCESS) if post_process is None else bool(post_process)
+        if self.flip_test:
+            if flip_pairs is None:
+                raise ValueError("flip test needs the dataset's joint pairs (flip_pairs)")
+            flip_permutation(flip_pairs, net._plan.num_joints)
+        self.flip_pairs = flip_pairs
+        self.depth_range = float(config.DATASET.DEPTH_RANGE)
+        self.model = net
+        self.dev = next(net.parameters()).device
+        self.eng = _net16.Engine16(net._plan, ops=net._ops)
+        self.stream = torch.cuda.Stream(self.dev)
+        self.graphs = {}
+        self.state = None
+        self.logits = None
+        self.heatmaps = None
+        self.depth = None
+        self.refresh()
+
+    def _forward(self, ent):
+        """The captured work: [flip,] network, heat-map decode."""
+        x, box = ent["x"], ent["box"]
+        N, H, W = box.shape[0], x.shape[2], x.shape[3]
+        if self.flip_test:
+            x[N:] = torch.flip(x[:N], [3])
+        logits, depth, _ = self.eng.forward(x, None, training=False, save=False, prepared=self.state)
+        plan = self.eng.plan
+        hm = logits.permute(0, 3, 1, 2)[:, :plan.final.cout]
+        depth = depth.reshape(depth.shape[0], -1)
+        if "kps" not in ent:
+            ent["kps"] = torch.empty((N, plan.num_joints, 4), device=self.dev, dtype=torch.float64)
+        heatmap_decode_device(hm, depth, plan.depth_res, box, W, H, self.depth_range, self.post_process,
+                              self.flip_pairs if self.flip_test else None, self.shift_heatmap, out=ent["kps"])
+        ent["heatmaps"], ent["depth"] = hm, depth
+
+    def _capture(self, N, H, W):
+        ent = super()._capture(N, H, W)
+        ent["box0"] = ent["box"].clone()            # the identity box: image frame = patch frame
+        return ent
+
+    def __call__(self, images, boxes=None):
+        x = torch.as_tensor(images)
+        if x.dim() != 4 or x.shape[1] != 3:
+            raise ValueError("expected images [N, 3, H, W], got %s" % (tuple(x.shape),))
+        if x.dtype != torch.float32:
+            raise TypeError("expected float32 images, got %s" % x.dtype)
+        N, _, H, W = x.shape
+        with torch.cuda.device(self.dev):
+            ent = self.graphs.get((N, H, W)) or self._capture(N, H, W)
+            ent["x"][:N].copy_(x, non_blocking=x.is_cuda)
+            if boxes is None:
+                ent["box"].copy_(ent["box0"])
+            else:
+                from ..utils.img_utils import _boxes
+                meta = dict(boxes)
+                meta.setdefault("scale", np.ones(N))
+                meta.setdefault("rot", np.zeros(N))
+                ent["box"].copy_(_boxes(meta, N, torch.device("cpu")))
+            ent["graph"].replay()
+            self.heatmaps, self.depth = ent["heatmaps"], ent["depth"]
+            kps = ent["kps"].cpu().numpy()
+            return heatmap_rows(kps, W) if boxes is None else kps

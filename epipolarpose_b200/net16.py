@@ -97,12 +97,11 @@ class Engine16(_net.Engine):
 
     def prepare_inference(self, params, dev, state=None):
         """The weights of an inference forward (forward(..., prepared=...)), prepared once outside
-        the walk: the fp32 pack, the split planes, the BatchNorm eval affines and the final layer's
-        (padded) bias.  With `state` (an earlier result) the same tensors are refilled, so that
-        CUDA graphs captured on them read the new values."""
+        the walk: the fp32 pack, the split planes, the BatchNorm eval affines, the final layer's
+        (padded) bias and, for a VOLUME = false model, depth_fc's (padded) bias.  With `state` (an
+        earlier result) the same tensors are refilled, so that CUDA graphs captured on them read the
+        new values."""
         ops, plan = self.ops, self.plan
-        if plan.fc is not None:
-            raise ValueError("the inference forward needs the VOLUME head (MODEL.VOLUME: true)")
         self.dev = dev
         packed = self._pack_weights(params)
         w16 = self._split_weights(packed)
@@ -117,7 +116,13 @@ class Engine16(_net.Engine):
         fin = plan.final
         fbias = state["fbias"] if state is not None else torch.zeros(fin.cout_p, device=dev)
         fbias[:fin.cout].copy_(params[fin.name + ".bias"])
-        return {"packed": packed, "w16": w16, "bn": bn, "fbias": fbias}
+        out = {"packed": packed, "w16": w16, "bn": bn, "fbias": fbias}
+        if plan.fc is not None:                 # the VOLUME = false depth branch (depth_fc)
+            fc = plan.fc
+            dbias = state["dbias"] if state is not None else torch.zeros(fc.cout_p, device=dev)
+            dbias[:fc.cout].copy_(params[fc.name + ".bias"])
+            out["dbias"] = dbias
+        return out
 
     # ------------------------------------------------------------------ conv helpers
     def _conv_fwd16(self, conv, x, x_sc, N, H, W, w16, bias=None, stats=None, splitk=False):
@@ -352,7 +357,7 @@ class Engine16(_net.Engine):
             pooled = torch.empty((N, 1, 1, 2048), device=self.dev, dtype=torch.float32)
             ops.avgpool_split(tr, tr_sc, pooled, N, th * tw, 2048)
             depth, _, _ = self._conv_fwd(plan.fc, pooled, N, 1, 1, S["packed"][plan.fc.name][0],
-                                         bias=params["depth_fc.bias"])
+                                         bias=prepared["dbias"] if infer else params["depth_fc.bias"])
             S["fc"] = pooled
         tick, self._nbt_tick = self._nbt_tick, None
         if tick:

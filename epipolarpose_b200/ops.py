@@ -360,6 +360,28 @@ def final_preds(hm, N, J, H, W, center, scale, post_process, preds, maxvals):
 
 # ------------------------------------------------------------------ geometry (fp64)
 
+def heatmap_decode(hm, layout, C, depth, depth_ld, box, N, J, H, W, D, patch_w, patch_h, depth_range,
+                   post_process, perm, shift, kps):
+    """hm: contiguous [B][J][H][W] (layout 0) or [B][H][W][C] (layout 1) storage; depth [B][depth_ld];
+    box [N][6] float64 or None; perm: host sequence of J joint indices (flip test, B = 2N) or None;
+    kps [N][J][4] float64."""
+    B = 2 * N if perm is not None else N
+    need_hm = B * H * W * (J if layout == 0 else C)
+    if hm.numel() < need_hm or depth.numel() < B * depth_ld:
+        raise _lib.EpbError("heatmap_decode: hm holds %d of %d values, depth %d of %d"
+                            % (hm.numel(), need_hm, depth.numel(), B * depth_ld))
+    if kps.numel() != N * J * 4 or (box is not None and box.numel() != N * 6):
+        raise _lib.EpbError("heatmap_decode: kps must hold N*J*4 and box N*6 values")
+    pi = None
+    if perm is not None:
+        if len(perm) != J:
+            raise _lib.EpbError("perm has %d entries, expected J = %d" % (len(perm), J))
+        pi = (ctypes.c_int * J)(*[int(v) for v in perm])
+    _call("epb_heatmap_decode", _p(hm), int(layout), int(C), _p(depth), int(depth_ld),
+          _p(box, torch.float64), N, J, H, W, D, float(patch_w), float(patch_h), float(depth_range),
+          int(bool(post_process)), pi, int(shift), _p(kps, torch.float64), _stream())
+
+
 def patch_to_image(coords, box, B, J, patch_w, patch_h, rect3d_w, kps):
     _call("epb_patch_to_image", _p(coords), _p(box, torch.float64), B, J, float(patch_w),
           float(patch_h), float(rect3d_w), _p(kps, torch.float64), _stream())

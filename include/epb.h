@@ -413,6 +413,26 @@ int epb_final_preds(const float* hm, int N, int J, int H, int W, const double* c
                     const double* scale, int post_process, float* preds, float* maxvals,
                     epb_stream_t stream);
 
+/* The MODEL.VOLUME = false head -> joints in one launch (one CTA per image):
+ *   2-D: the argmax of epb_argmax2d (bit-identical x, y and maxval), the +-0.25 px refinement of
+ *        epb_final_preds when post_process != 0, heat-map px -> patch px (x * patch_w / W,
+ *        y * patch_h / H) and, when box != NULL, the inverse patch affine of epb_patch_to_image;
+ *   depth: lib/core/inference.py:144-170 get_depth_preds, the soft-argmax of the joint's D logits
+ *        in float64 with the maximum subtracted, d = (s / D - 0.5) * depth_range (root-relative).
+ * hm float32: layout 0 [B][J][H][W] contiguous; layout 1 [B][H][W][C], C >= J (the channels-last
+ * output of the split-fp16 final conv; channels J..C-1 are never read).  depth [B][depth_ld]
+ * float32, joint j's logits at j*D .. j*D+D-1 (J*D <= depth_ld).  box [N][6] float64 as
+ * epb_patch_to_image, or NULL for patch pixels.  J <= 1024.
+ * Flip test with perm_host (J joint indices, an involution; NULL: none): B = 2N rows [x; flip(x)],
+ * each map decoded as 0.5 (a + flip_back(b)) (b: image n + N, joint perm[j], columns mirrored and,
+ * with shift, moved one column right) and each depth row as 0.5 (a + b[perm[j]]); the merged values
+ * are never written.  B = N without flip.
+ * kps [N][J][4] float64 = (x, y, d mm, maxval). */
+int epb_heatmap_decode(const float* hm, int layout, int C, const float* depth, int depth_ld,
+                       const double* box, int N, int J, int H, int W, int D, double patch_w,
+                       double patch_h, double depth_range, int post_process, const int* perm_host,
+                       int shift, double* kps, epb_stream_t stream);
+
 /* ------------------------------------------------------------------------
  * Epipolar geometry in float64 (OpenCV/numpy call sites).
  * ---------------------------------------------------------------------- */
